@@ -1,4 +1,4 @@
-"""arroy_b200 — B200-native distance / split / re-rank path for arroy (see DESIGN.md).
+"""arroy_b200 — H100-native (sm_90a) distance / split / re-rank path for arroy (see DESIGN.md).
 
 `arroy_b200._capi.Context` is the 1:1 ctypes view of the C ABI in include/arroy_b200.h.
 The compute path is the CUDA library only; importing this package never touches oracle/.

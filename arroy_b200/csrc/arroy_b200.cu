@@ -98,7 +98,7 @@ struct HostWave {  // pinned host copies of one wave's results; kept across buil
 
 struct arroy_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     std::mutex mu;
     std::string err;
@@ -230,7 +230,7 @@ template <class RowSrc>
 void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t ld, RowSrc row_src, float* dst_override = nullptr, size_t chunk_mb_override = 0, bool count_bytes = true,
                          int mode = 0, uint32_t src_dim = 0) {
     if (n == 0) return;
-    unsigned W = 8;   // measured on the B200 box: 8 lanes x 4 MB chunks reach ~48 GB/s (PCIe copy alone: 54 GB/s)
+    unsigned W = 8;   // 8 lanes x 4 MB chunks: decode of one chunk overlaps the PCIe copies of the others
     if (const char* e = getenv("ARROY_B200_STAGE_THREADS")) W = (unsigned)std::max(1, atoi(e));
     W = std::max(1u, std::min(W, std::max(1u, std::thread::hardware_concurrency())));
     size_t chunk_mb = 4;
@@ -988,7 +988,7 @@ const float* xf_candidates(arroy_ctx* c, const uint32_t* rows, uint32_t nc) {
     return c->x_gather.as<float>();
 }
 
-// S (m x nc, pitch lds) = Q . cand^T with TF32 inputs and FP32 accumulation. engine 0: the tcgen05
+// S (m x nc, pitch lds) = Q . cand^T with TF32 inputs and FP32 accumulation. engine 0: the wgmma
 // kernel of tcgemm.cuh; engine 1: cuBLAS (kept as the cross-check of the hand-written kernel)
 void xf_scores(arroy_ctx* c, const float* q, uint32_t m, const float* cand, uint32_t nc, float* S, uint32_t lds, TgEpilogue ep, int engine) {
     if (engine == 0) {
@@ -1192,7 +1192,7 @@ int32_t guarded(arroy_ctx* c, F&& f) {
 // ================================================================================================
 extern "C" {
 
-const char* arroy_b200_version(void) { return "arroy_b200 0.1.0 (sm_100a)"; }
+const char* arroy_b200_version(void) { return "arroy_b200 0.1.0 (sm_90a)"; }
 
 int32_t arroy_b200_create(int32_t device, arroy_ctx** out) {
     if (!out) return ARROY_B200_ERR_INVALID;

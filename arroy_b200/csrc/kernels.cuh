@@ -1,4 +1,4 @@
-// kernels.cuh — data-parallel kernels of the hot path (sm_100a):
+// kernels.cuh — data-parallel kernels of the hot path (sm_90a):
 //   work_kernel      side()/margin scan over row lists + stable left/right partition of id lists
 //                    (src/writer.rs:1201-1207 and its callers :1424-1430, :1494-1500)
 //   norms_kernel     per-item sqrt(dot(v,v)) (Cosine new_header, cosine.rs:39-41;

@@ -1,22 +1,21 @@
-// tcgemm.cuh — S = Q . C^T on the 5th-generation tensor cores (tcgen05, TF32 inputs, FP32
-// accumulation in TMEM), hand-written for sm_100a. It is the first stage of the shared-candidate
-// re-rank (xrerank.cuh, "tensor-core pre-filter"): S only has to *bound* the reference's distance
-// of every (query, candidate) pair, the survivors are re-scored in the reference's exact order.
+// tcgemm.cuh — S = Q . C^T on the Hopper tensor cores (wgmma, TF32 inputs, FP32 accumulation in
+// registers), hand-written for sm_90a. It is the first stage of the shared-candidate re-rank
+// (xrerank.cuh, "tensor-core pre-filter"): S only has to *bound* the reference's distance of every
+// (query, candidate) pair, the survivors are re-scored in the reference's exact order.
 //
-//   Q : m  x K  fp32, row-major, pitch ld (K = ld, padding is zero)      -> UMMA operand A, K-major
-//   C : nc x K  fp32, row-major, pitch ld (item rows, in place)          -> UMMA operand B, K-major
+//   Q : m  x K  fp32, row-major, pitch ld (K = ld, padding is zero)      -> wgmma operand A, K-major
+//   C : nc x K  fp32, row-major, pitch ld (item rows, in place)          -> wgmma operand B, K-major
 //   S : m  x nc fp32, row-major, pitch lds
 //
-// Structure (one persistent CTA per SM, 320 threads):
-//   warp 0     TMA producer: cp.async.bulk.tensor 2D, 128B-swizzled boxes of 32 floats of K
-//              (128 x 32 of Q, 256 x 32 of C) into a 4-stage shared-memory ring, mbarrier tx-counts
-//   warp 1     allocates TMEM (512 columns = two 128 x 256 FP32 accumulators) and issues
-//              tcgen05.mma.cta_group::1.kind::tf32 (M = 128, N = 256, K = 8), four per stage;
-//              tcgen05.commit releases the stage / publishes the accumulator
-//   warps 2-9  epilogue: tcgen05.ld 32x32b.x32 (a warp may read the 32 TMEM lanes = 32 queries of
-//              its quarter; two warps per quarter split the 256 columns), per-column constants of
-//              the tile staged in shared memory, distance estimate, 16-byte stores; the other
-//              accumulator is being filled meanwhile
+// Structure (one persistent CTA per SM, three warpgroups):
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor 2D, 128B-swizzled boxes of 32
+//                   floats of K (128 x 32 of Q, 256 x 32 of C) into a 4-stage shared-memory ring,
+//                   mbarrier tx-counts
+//   warpgroups 1-2  consumers: 64 queries each, wgmma.mma_async m64n256k8 TF32 (four per stage) into a
+//                   64 x 256 FP32 register accumulator; a stage is released as soon as the wgmma group
+//                   that read it has retired (wait_group 1 keeps one group in flight), then the
+//                   distance estimate of the tile is computed and stored straight from the registers
+//                   while the producer already fills the ring for the next tile
 // Tiles are ordered candidates-major so that the CTAs running at the same time share the same
 // candidate rows in L2 and C streams from HBM once.
 #pragma once
@@ -25,20 +24,20 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 namespace ab {
 
-constexpr int TG_BM = 128;      // queries per tile   (UMMA M)
-constexpr int TG_BN = 256;      // candidates per tile (UMMA N)
+constexpr int TG_BM = 128;     // queries per tile   (two consumer warpgroups x wgmma M = 64)
+constexpr int TG_BN = 256;      // candidates per tile (wgmma N)
 constexpr int TG_BK = 32;       // floats of K per stage = one 128-byte swizzle span
-constexpr int TG_UK = 8;        // K of one tcgen05.mma.kind::tf32
+constexpr int TG_UK = 8;        // K of one wgmma .tf32
 constexpr int TG_STAGES = 4;
-constexpr int TG_EPI_WARPS = 8;                // two per TMEM lane quarter, 128 columns each
-constexpr int TG_THREADS = 64 + 32 * TG_EPI_WARPS;
+constexpr int TG_THREADS = 3 * 128;
 constexpr uint32_t TG_A_BYTES = TG_BM * TG_BK * 4;
 constexpr uint32_t TG_B_BYTES = TG_BN * TG_BK * 4;
 constexpr uint32_t TG_STAGE_BYTES = TG_A_BYTES + TG_B_BYTES;
-constexpr size_t TG_SMEM = (size_t)TG_STAGES * TG_STAGE_BYTES + 1024 /* 1024-byte alignment */ + 256 /* barriers */ + 2 * 2 * TG_BN * 4 /* column constants */;
-constexpr uint32_t TG_TMEM_COLS = 512;
+constexpr size_t TG_SMEM = (size_t)TG_STAGES * TG_STAGE_BYTES + 1024 /* 1024-byte alignment */ + 256 /* barriers */;
 
 __device__ __forceinline__ uint32_t tg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -48,8 +47,10 @@ __device__ __forceinline__ void tg_mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void tg_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void tg_mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+// arrive on the barrier at this shared-memory offset in CTA `cta` of the cluster (the own CTA included)
+__device__ __forceinline__ void tg_mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\tmbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+                 ::"r"(bar), "r"(cta) : "memory");
 }
 // Spin on a phase parity. A protocol bug must not hang the GPU: trap after ~2 s.
 __device__ __forceinline__ void tg_mbar_wait(uint32_t bar, uint32_t parity) {
@@ -75,43 +76,51 @@ __device__ __forceinline__ void tg_tma_load_2d_mc(uint32_t dst, const CUtensorMa
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask) : "memory");
 }
-__device__ __forceinline__ void tg_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tg_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, 8-row groups 1024 bytes apart
 __device__ __forceinline__ uint64_t tg_smem_desc(uint32_t addr) {
     uint64_t d = 0;
-    d |= (uint64_t)((addr >> 4) & 0x3fffu);        // start address, 16-byte units
+    d |= (uint64_t)((addr & 0x3ffffu) >> 4);       // start address, 16-byte units
     d |= (uint64_t)1 << 16;                         // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset: next 8-row group
-    d |= (uint64_t)1 << 46;                         // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                         // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                         // SWIZZLE_128B
     return d;
 }
-// instruction descriptor: D = F32, A = B = TF32, both K-major, M = 128, N = 256
-constexpr uint32_t TG_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TG_BN >> 3) << 17) | ((uint32_t)(TG_BM >> 4) << 24);
 
-__device__ __forceinline__ void tg_mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(TG_IDESC), "r"(accumulate) : "memory");
+// d (64 x 256 FP32, wgmma accumulator fragment) (+)= A (64 x 8) . B (256 x 8)^T, both TF32 from shared memory
+__device__ __forceinline__ void tg_wgmma_tf32(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+                 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+                 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+                 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+                 "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+                 "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+                 "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+                 "%128, %129, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+                   "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+                   "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+                   "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+                   "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+                   "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+                   "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+                   "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+                   "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+                 : "l"(desc_a), "l"(desc_b), "r"(accumulate) : "memory");
 }
-__device__ __forceinline__ void tg_commit(uint32_t bar) {   // arrives on `bar` once every MMA issued so far has completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tg_commit_mc(uint32_t bar, uint16_t mask) {   // ... on the barrier at this offset in every CTA of `mask`
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tg_tmem_ld32(uint32_t taddr, uint32_t* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                   "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                   "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                   "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+__device__ __forceinline__ void tg_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tg_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void tg_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // What the epilogue writes for pair (q, c) from the raw contraction s = Q[q] . C[c]:
 //   TG_RAW     s
@@ -143,9 +152,9 @@ __device__ __forceinline__ float tg_finish(int mode, float s, float qa, float qb
 
 // MC = 1: independent CTAs. MC = 2: clusters of two CTAs that work on the same 256 candidates and two
 // neighbouring blocks of 128 queries; each CTA fetches one half of the candidate tile and TMA-multicasts it
-// into both CTAs' shared memory, so the operand traffic L2 -> SM per CTA drops from 48 to 32 KB per stage (that
-// traffic, not the tensor pipe, limits the MC = 1 kernel). A stage is released to both producers by both MMA
-// warps (tcgen05.commit.multicast on the `empty` barriers, which therefore count two arrivals).
+// into both CTAs' shared memory, so the operand traffic L2 -> SM per CTA drops from 48 to 32 KB per stage.
+// A stage is released to both producers by the consumer warpgroups of both CTAs (remote mbarrier arrivals
+// on the `empty` barriers, which therefore count 2 * MC arrivals).
 template <int MC>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
@@ -153,14 +162,9 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     extern __shared__ uint8_t tg_raw[];
     const uint32_t raw = tg_smem_u32(tg_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;                      // swizzle-128B tiles need 1024-byte alignment
-    const uint32_t bars = base + TG_STAGES * TG_STAGE_BYTES;           // full[4], empty[4], tmem_full[2], tmem_empty[2], tmem ptr
+    const uint32_t bars = base + TG_STAGES * TG_STAGE_BYTES;           // full[4], empty[4]
     auto full = [&](int s) { return bars + 8u * s; };
     auto empty = [&](int s) { return bars + 8u * (TG_STAGES + s); };
-    auto tfull = [&](int a) { return bars + 8u * (2 * TG_STAGES + a); };
-    auto tempty = [&](int a) { return bars + 8u * (2 * TG_STAGES + 2 + a); };
-    const uint32_t tmem_slot = bars + 8u * (2 * TG_STAGES + 4);
-    float* cst = reinterpret_cast<float*>(tg_raw + (bars + 256u - raw));   // [2 accumulators][ca, cb][TG_BN]
-    volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(tg_raw + (tmem_slot - raw));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t crank = MC > 1 ? cooperative_groups::this_cluster().block_rank() : 0u;
@@ -169,25 +173,17 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     auto tile_m0 = [&](uint32_t t) { return ((t % num_mb) * MC + crank) * TG_BM; };   // may lie beyond m: zero rows, nothing stored
     auto tile_n0 = [&](uint32_t t) { return (t / num_mb) * TG_BN; };
 
-    if (warp == 0 && lane == 0) {
-        for (int s = 0; s < TG_STAGES; ++s) { tg_mbar_init(full(s), 1); tg_mbar_init(empty(s), MC); }
-        for (int a = 0; a < 2; ++a) { tg_mbar_init(tfull(a), 1); tg_mbar_init(tempty(a), TG_EPI_WARPS); }
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < TG_STAGES; ++s) { tg_mbar_init(full(s), 1); tg_mbar_init(empty(s), 2 * MC); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(TG_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tg_fence_before();
     __syncthreads();
     if (MC > 1) cooperative_groups::this_cluster().sync();   // the peer's barriers exist before anything is multicast to them
-    tg_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        if (threadIdx.x == 0) {
             int stage = 0; uint32_t phase = 0;
             for (uint32_t t = first; t < tiles; t += stride) {
                 const int m0 = (int)tile_m0(t), n0 = (int)tile_n0(t);
@@ -202,93 +198,66 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            int stage = 0; uint32_t phase = 0, it = 0;
-            for (uint32_t t = first; t < tiles; t += stride, ++it) {
-                const uint32_t a = it & 1u, aphase = (it >> 1) & 1u;
-                tg_mbar_wait(tempty(a), aphase ^ 1u);                 // epilogue has drained this accumulator
-                tg_fence_after();
-                const uint32_t d = tmem_base + a * TG_BN;
-                for (uint32_t kb = 0; kb < nk; ++kb) {
-                    tg_mbar_wait(full(stage), phase);                  // TMA has landed this stage
-                    tg_fence_after();
-                    const uint32_t sa = base + stage * TG_STAGE_BYTES, sb = sa + TG_A_BYTES;
-                    const uint64_t da = tg_smem_desc(sa), db = tg_smem_desc(sb);
-#pragma unroll
-                    for (int k = 0; k < TG_BK / TG_UK; ++k)            // +32 bytes of K inside the swizzle span per step
-                        tg_mma_tf32(d, da + (uint64_t)(k * TG_UK * 4 / 16), db + (uint64_t)(k * TG_UK * 4 / 16), (kb | (uint32_t)k) != 0u);
-                    if (MC == 1) tg_commit(empty(stage));              // frees the stage when these MMAs retire
-                    else tg_commit_mc(empty(stage), (uint16_t)((1u << MC) - 1u));   // ... in both CTAs: both producers write into both
-                    if (++stage == TG_STAGES) { stage = 0; phase ^= 1u; }
-                }
-                tg_commit(tfull(a));                                   // accumulator complete
-            }
-        }
     } else {
-        const uint32_t qtr = (uint32_t)warp & 3u;                      // TMEM lane quarter this warp may read
-        const uint32_t half = (uint32_t)(warp - 2) >> 2;               // which 128 columns of the tile
-        const uint32_t et = threadIdx.x - 64u;                         // 0 .. 255 over the epilogue warps
-        uint32_t it = 0;
-        for (uint32_t t = first; t < tiles; t += stride, ++it) {
-            const uint32_t a = it & 1u, aphase = (it >> 1) & 1u;
+        const uint32_t wg = (uint32_t)(warp >> 2) - 1u;               // consumer warpgroup: rows wg * 64 .. + 63 of the tile
+        const uint32_t wr = (uint32_t)(warp & 3) * 16u + (uint32_t)(lane >> 2);   // fragment rows wr and wr + 8
+        const uint32_t wc = (uint32_t)(lane & 3) * 2u;                 // fragment columns 8 j + wc, + 1
+        auto release = [&](int s) {                                    // one arrival per warpgroup on every CTA's barrier
+            if ((threadIdx.x & 127u) == 0)
+                for (uint32_t r = 0; r < (uint32_t)MC; ++r) tg_mbar_arrive_cluster(empty(s), r);
+        };
+        int stage = 0; uint32_t phase = 0;
+        float acc[TG_BN / 2];
+        for (uint32_t t = first; t < tiles; t += stride) {
             const uint32_t m0 = tile_m0(t), n0 = tile_n0(t);
-            float* ca_s = cst + a * 2 * TG_BN;
-            float* cb_s = ca_s + TG_BN;
-            if (ep.mode >= TG_EUCLID) {                                // this tile's column constants -> shared memory
-                const uint32_t col = n0 + et;
-                ca_s[et] = col < nc ? __ldg(ep.ca + col) : 0.f;
-                cb_s[et] = (ep.mode == TG_COSINE && col < nc) ? __ldg(ep.cb + col) : 0.f;
-                asm volatile("bar.sync 1, %0;" ::"n"(32 * TG_EPI_WARPS) : "memory");
+            int prev = -1;
+            for (uint32_t kb = 0; kb < nk; ++kb) {
+                tg_mbar_wait(full(stage), phase);                      // TMA has landed this stage
+                const uint32_t sa = base + stage * TG_STAGE_BYTES + wg * (TG_A_BYTES / 2), sb = base + stage * TG_STAGE_BYTES + TG_A_BYTES;
+                const uint64_t da = tg_smem_desc(sa), db = tg_smem_desc(sb);
+                tg_wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < TG_BK / TG_UK; ++k)                // +32 bytes of K inside the swizzle span per step
+                    tg_wgmma_tf32(acc, da + (uint64_t)(k * TG_UK * 4 / 16), db + (uint64_t)(k * TG_UK * 4 / 16), (kb | (uint32_t)k) != 0u);
+                tg_wgmma_commit();
+                tg_wgmma_wait<1>();                                    // the previous stage's group has retired
+                if (prev >= 0) release(prev);
+                prev = stage;
+                if (++stage == TG_STAGES) { stage = 0; phase ^= 1u; }
             }
-            const uint32_t row = m0 + qtr * 32u + (uint32_t)lane;
-            float qa = 0.f, qb = 0.f;
-            if (row < m && ep.mode >= TG_EUCLID) { qa = ep.qa[row]; if (ep.mode == TG_COSINE) qb = ep.qb[row]; }
-            float* out = S + (size_t)row * lds + n0 + half * 128u;
-            tg_mbar_wait(tfull(a), aphase);
-            tg_fence_after();
-#pragma unroll 1
-            for (uint32_t c = 0; c < 4; ++c) {
-                uint32_t v[32];
-                tg_tmem_ld32(tmem_base + ((qtr * 32u) << 16) + a * TG_BN + half * 128u + c * 32u, v);
-                const uint32_t col = n0 + half * 128u + c * 32u;
-                if (ep.mode == TG_NEG) {
+            tg_wgmma_wait<0>();
+            if (prev >= 0) release(prev);
+
+            const uint32_t r0 = m0 + wg * 64u + wr, r1 = r0 + 8u;
+            float qa0 = 0.f, qb0 = 0.f, qa1 = 0.f, qb1 = 0.f;
+            if (ep.mode >= TG_EUCLID) {
+                if (r0 < m) { qa0 = ep.qa[r0]; if (ep.mode == TG_COSINE) qb0 = ep.qb[r0]; }
+                if (r1 < m) { qa1 = ep.qa[r1]; if (ep.mode == TG_COSINE) qb1 = ep.qb[r1]; }
+            }
+            float* out0 = S + (size_t)r0 * lds;
+            float* out1 = S + (size_t)r1 * lds;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] ^= 0x80000000u;
-                } else if (ep.mode >= TG_EUCLID) {
-                    const float4* ca4 = reinterpret_cast<const float4*>(ca_s + half * 128u + c * 32u);
-                    const float4* cb4 = reinterpret_cast<const float4*>(cb_s + half * 128u + c * 32u);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 x = ca4[j];
-                        float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (ep.mode == TG_COSINE) y = cb4[j];
-                        v[4 * j + 0] = __float_as_uint(tg_finish(ep.mode, __uint_as_float(v[4 * j + 0]), qa, qb, x.x, y.x));
-                        v[4 * j + 1] = __float_as_uint(tg_finish(ep.mode, __uint_as_float(v[4 * j + 1]), qa, qb, x.y, y.y));
-                        v[4 * j + 2] = __float_as_uint(tg_finish(ep.mode, __uint_as_float(v[4 * j + 2]), qa, qb, x.z, y.z));
-                        v[4 * j + 3] = __float_as_uint(tg_finish(ep.mode, __uint_as_float(v[4 * j + 3]), qa, qb, x.w, y.w));
-                    }
+            for (int j = 0; j < TG_BN / 8; ++j) {
+                const uint32_t col = n0 + 8u * (uint32_t)j + wc;
+                float ca0 = 0.f, ca1 = 0.f, cb0 = 0.f, cb1 = 0.f;
+                if (ep.mode >= TG_EUCLID) {
+                    if (col < nc) { ca0 = __ldg(ep.ca + col); if (ep.mode == TG_COSINE) cb0 = __ldg(ep.cb + col); }
+                    if (col + 1u < nc) { ca1 = __ldg(ep.ca + col + 1u); if (ep.mode == TG_COSINE) cb1 = __ldg(ep.cb + col + 1u); }
                 }
-                if (row < m) {
-                    if (col + 32u <= lds) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j)
-                            *reinterpret_cast<uint4*>(out + c * 32u + j * 4) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) if (col + j < nc) out[c * 32u + j] = __uint_as_float(v[j]);
-                    }
+                const float v00 = tg_finish(ep.mode, acc[4 * j + 0], qa0, qb0, ca0, cb0), v01 = tg_finish(ep.mode, acc[4 * j + 1], qa0, qb0, ca1, cb1);
+                const float v10 = tg_finish(ep.mode, acc[4 * j + 2], qa1, qb1, ca0, cb0), v11 = tg_finish(ep.mode, acc[4 * j + 3], qa1, qb1, ca1, cb1);
+                if (col + 1u < nc) {                                   // col is even and lds % 4 == 0: 8-byte aligned
+                    if (r0 < m) *reinterpret_cast<float2*>(out0 + col) = make_float2(v00, v01);
+                    if (r1 < m) *reinterpret_cast<float2*>(out1 + col) = make_float2(v10, v11);
+                } else if (col < nc) {
+                    if (r0 < m) out0[col] = v00;
+                    if (r1 < m) out1[col] = v10;
                 }
             }
-            tg_fence_before();
-            __syncwarp();
-            if (lane == 0) tg_mbar_arrive(tempty(a));
         }
     }
-    tg_fence_before();
     __syncthreads();
-    if (MC > 1) cooperative_groups::this_cluster().sync();   // no CTA leaves while its peer can still multicast into it
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TG_TMEM_COLS) : "memory");
+    if (MC > 1) cooperative_groups::this_cluster().sync();   // no CTA leaves while its peer can still multicast or arrive into it
 }
 
 // the same epilogue as a separate pass (used after the cuBLAS cross-check engine)
@@ -335,20 +304,28 @@ inline bool tcgemm_tf32(const float* Q, uint32_t m, const float* C, uint32_t nc,
     CUtensorMap mq, mcand;
     if (!tg_make_map(&mq, Q, m, ld, TG_BM) || !tg_make_map(&mcand, C, nc, ld, TG_BN / mc)) return false;
     static bool configured = false;
+    static int max_clusters[3] = {0, 0, 0};   // clusters of 1 / 2 CTAs that can be resident at once (GPCs need not hold an even SM count)
     if (!configured) {
         if (cudaFuncSetAttribute(tcgemm_tf32_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
         if (cudaFuncSetAttribute(tcgemm_tf32_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
         configured = true;
     }
-    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + mc - 1) / mc;
-    const uint32_t tiles = num_mb * ((nc + TG_BN - 1) / TG_BN);
-    const uint32_t units = (uint32_t)(sm_count / mc);
-    const int grid = (int)((tiles < units ? tiles : units) * mc);
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(TG_THREADS); cfg.dynamicSmemBytes = TG_SMEM; cfg.stream = stream;
+    cfg.blockDim = dim3(TG_THREADS); cfg.dynamicSmemBytes = TG_SMEM; cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)mc; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
+    if (max_clusters[mc] == 0) {
+        cfg.gridDim = dim3((unsigned)(sm_count / mc * mc));
+        int nclu = 0;
+        const cudaError_t oe = mc == 1 ? cudaOccupancyMaxActiveClusters(&nclu, tcgemm_tf32_kernel<1>, &cfg) : cudaOccupancyMaxActiveClusters(&nclu, tcgemm_tf32_kernel<2>, &cfg);
+        if (oe != cudaSuccess || nclu <= 0) return false;
+        max_clusters[mc] = nclu;
+    }
+    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + mc - 1) / mc;
+    const uint32_t tiles = num_mb * ((nc + TG_BN - 1) / TG_BN);
+    const uint32_t units = (uint32_t)std::min(sm_count / mc, max_clusters[mc]);
+    cfg.gridDim = dim3((unsigned)((tiles < units ? tiles : units) * mc));
     const uint32_t nk = ld / TG_BK;
     cudaError_t e = mc == 1 ? cudaLaunchKernelEx(&cfg, tcgemm_tf32_kernel<1>, mq, mcand, S, m, nc, lds, nk, ep)
                             : cudaLaunchKernelEx(&cfg, tcgemm_tf32_kernel<2>, mq, mcand, S, m, nc, lds, nk, ep);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — index-build throughput (+ QPS@recall) of arroy's distance / split / re-rank hot path on B200.
+"""bench.py — index-build throughput (+ QPS@recall) of arroy's distance / split / re-rank hot path on H100.
 
 One "step" = one complete forest build (Writer::build of the reference, src/writer.rs:487-629)
 over one synthetic item matrix. Contract: `python bench.py --gpus N --steps K --warmup W`
@@ -11,15 +11,15 @@ Workloads (BASELINE.json configs; SURVEY.md §8d synthetic data: element (i,j) =
 number i*d+j of StdRng::from_seed([42;32]) minus 0.5; build rng = fresh StdRng([42;32])):
   c2 (default)  1 000 000 x 768  Cosine      n_trees = 50    <- BASELINE.json configs[1]; `value`, `e2e` and the
                                                                reference arm are quoted on it (the CPU arm cannot
-                                                               finish 10M rows inside the driver's steps)
-  c3            10 000 000 x 768 DotProduct  n_trees = 100
-  c4            10 000 000 x 1536 Cosine     n_trees = 100   (meant for 8 GPUs)
+                                                               finish millions of rows inside the timed steps)
+  c3            5 000 000 x 768 DotProduct   n_trees = 100
+  c4            2 500 000 x 1536 Cosine      n_trees = 100
   c1            10 000 x 64      Euclidean   n_trees = 10    (raw [0,1) data)
   small         100 000 x 768    Cosine      n_trees = 16    (quick check)
   c5            4096 queries x 100 000 shared candidates, d = 768, Cosine, top-100 (own metric: queries/s)
 
 The default (c2) line also carries, as sub-records measured in the same process:
-  headline_10m  BASELINE.json's metric configuration itself: 10M x 768 Cosine, n_trees = 100 — value, roofline,
+  headline_10m  BASELINE.json's metric configuration at the size one 80 GB H100 holds: 5M x 768 Cosine, n_trees = 100 — value, roofline,
                 e2e (host leaf values -> stage_items -> build_trees -> arena sink) and clocks, 2 timed steps
   query         QPS@recall100 on the c2 index: batched and one-at-a-time (p50 latency) through Reader, recall vs exact
                 brute force, the oracle's nns_by_item timed on the same queries (ids compared) as `cpu_baseline`;
@@ -41,12 +41,12 @@ sys.path.insert(0, ROOT)
 SEED = bytes([42] * 32)
 WORKLOADS = {
     "c2": dict(n=1_000_000, d=768, metric="cosine", n_trees=50, centre=0.5, name="C2 1Mx768 Cosine n_trees=50"),
-    "c3": dict(n=10_000_000, d=768, metric="dot-product", n_trees=100, centre=0.5, name="C3 10Mx768 DotProduct n_trees=100"),
-    "c4": dict(n=10_000_000, d=1536, metric="cosine", n_trees=100, centre=0.5, name="C4 10Mx1536 Cosine n_trees=100"),
+    "c3": dict(n=5_000_000, d=768, metric="dot-product", n_trees=100, centre=0.5, name="C3 5Mx768 DotProduct n_trees=100"),
+    "c4": dict(n=2_500_000, d=1536, metric="cosine", n_trees=100, centre=0.5, name="C4 2.5Mx1536 Cosine n_trees=100"),
     "c1": dict(n=10_000, d=64, metric="euclidean", n_trees=10, centre=0.0, name="C1 10kx64 Euclidean n_trees=10"),
     "small": dict(n=100_000, d=768, metric="cosine", n_trees=16, centre=0.5, name="small 100kx768 Cosine n_trees=16"),
     "c5": dict(n=100_000, d=768, metric="cosine", n_trees=0, centre=0.5, nq=4096, k=100, name="C5 4096 queries x 100k candidates re-rank, d=768 Cosine top-100"),
-    "h10m": dict(n=10_000_000, d=768, metric="cosine", n_trees=100, centre=0.5, name="headline 10Mx768 Cosine n_trees=100"),
+    "h10m": dict(n=5_000_000, d=768, metric="cosine", n_trees=100, centre=0.5, name="headline 5Mx768 Cosine n_trees=100"),
 }
 GMM_CLUSTERS, GMM_SCALE, GMM_ROW0 = 256, 0.25, 1 << 40   # mixture centres = rows GMM_ROW0.. of the same ChaCha stream
 
@@ -62,18 +62,18 @@ def load_peaks():
 def peaks():
     d = load_peaks()
     if d:
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
 def tensor_peak(burst=False):
-    """TF32 dense peak: half the measured dense bf16 rate (tcgen05 kind::tf32 runs at half the kind::f16 rate)."""
+    """TF32 dense peak: half the measured dense bf16 rate (wgmma .tf32 runs at half the .bf16 rate)."""
     d = load_peaks()
     if d and "bf16_tflops_sustained" in d:
         if burst and "bf16_tflops" in d:
             return d["bf16_tflops"] / 2.0, "measured bf16 burst %.1f TFLOP/s / 2 (TF32 rate, kernel timed alone; MEASURED_PEAKS.json)" % d["bf16_tflops"]
         return d["bf16_tflops_sustained"] / 2.0, "measured bf16 sustained %.1f TFLOP/s / 2 (TF32 rate; MEASURED_PEAKS.json)" % d["bf16_tflops_sustained"]
-    return 1100.0, "fallback: nominal dense TF32 (B200_PROFILING.md)"
+    return 495.0, "H100 SXM data sheet: 495 TFLOP/s dense TF32 at 700 W (not measured)"
 
 
 class ClockSampler:
@@ -237,7 +237,7 @@ def c5_measure(ctx, torch, dev, wl, steps, warmup, cpu_sample=True):
         "gpu_launches": int(c1["launches"] - c0["launches"]),
         "rerank": {"breakdown_ms": bd, "survivors_per_query": stats["survivors"] / max(stats["queries"], 1), "fallback_chunks": stats["fallback_chunks"],
                    "exact_pairs_per_s": nq * n / (ms_per_step * 1e-3)},
-        "roofline": {"bound": "tensor", "kernel": "tcgemm_tf32_kernel (tcgen05.mma kind::tf32 + TMA + TMEM, fused distance-estimate epilogue)",
+        "roofline": {"bound": "tensor", "kernel": "tcgemm_tf32_kernel (wgmma m64n256k8 tf32 + TMA multicast, fused distance-estimate epilogue)",
                      "achieved": flop / (bd["score_gemm_ms"] * 1e-3) / 1e12, "peak": peak, "unit": "TFLOP/s", "frac": flop / (bd["score_gemm_ms"] * 1e-3) / 1e12 / peak,
                      "peak_source": peak_src, "traffic": None,
                      "timing": "CUDA events on the library stream around the kernel inside the timed arroy_b200_rerank_shared calls"},
@@ -436,8 +436,9 @@ def timed_builds(rig, wl, items, seeds, steps, warmup):
     scanned = 0
     alg_bytes = 0
     shadow_acc = {}
+    counts = None
     for _ in range(steps):
-        one_step()
+        counts = one_step()
         sr = ctx.build_stats()["scanned_rows"]
         sh = ctx.build_shadow_stats()
         scanned += sr
@@ -455,7 +456,90 @@ def timed_builds(rig, wl, items, seeds, steps, warmup):
     st, bd = ctx.build_stats(), ctx.build_breakdown()
     return {"alg_bytes_per_step": ab_step, "shadow_rows_per_step": {k: v / steps for k, v in shadow_acc.items()}, "last_step_alg_bytes": scan_bytes(st["scanned_rows"], ctx.build_shadow_stats(), d),
             "ms_per_step": ms_per_step, "value": n / (ms_per_step * 1e-3), "wall_ms_per_step": wall * 1e3 / steps, "clocks": clocks,
-            "launches": int(c1["launches"] - c0["launches"]), "scanned_rows_per_step": sc, "stats": st, "breakdown": bd, "my_trees": my_trees}
+            "launches": int(c1["launches"] - c0["launches"]), "scanned_rows_per_step": sc, "stats": st, "breakdown": bd, "my_trees": my_trees,
+            "counts": counts}
+
+
+def roaring_ids(b):
+    """RoaringBitmap portable serialization (no run containers, as the library writes it) -> sorted u32 ids."""
+    import numpy as np
+    size = int.from_bytes(b[4:8], "little")
+    hdr = np.frombuffer(b, dtype="<u2", count=2 * size, offset=8).reshape(size, 2)
+    off, out = 8 + 8 * size, []
+    for key, cm1 in hdr.tolist():
+        card = cm1 + 1
+        if card > 4096:
+            bits = np.unpackbits(np.frombuffer(b, np.uint8, 8192, off), bitorder="little")
+            out.append((key << 16) | np.nonzero(bits)[0].astype(np.uint32))
+            off += 8192
+        else:
+            out.append((key << 16) | np.frombuffer(b, "<u2", card, off).astype(np.uint32))
+            off += 2 * card
+    return np.concatenate(out) if out else np.zeros(0, np.uint32)
+
+
+def dump_forest(rig, wl, tb, out_dir, cap=1 << 20, n_normals=2048):
+    """--dump-outputs: the forest this rank built in the last timed step, as a caller of the build receives it (NodeCodec
+    node bytes, encoded here after the timed region from the results the library keeps parked), reduced to float64 /
+    float32 arrays. Node ids are numbered as a single-process Writer::build numbers them (roots 0..T-1, then every other
+    node, last tree first). Larger outputs are sampled with a fixed seed, so that the files stay under ~50 MB:
+      node_counts.npy      [T]        nodes per tree
+      leaf_sizes.npy       [L, 2]     (node id, items) of the Descendants nodes, by id (at most `cap` rows)
+      tree0_item_leaf.npy  [I, 2]     (item, node id of the Descendants node that holds it in tree 0) (at most `cap` items)
+      split_nodes.npy      [S, 4]     (node id, left, right, header[0]) of `n_normals` sampled split nodes, by id
+      split_normals.npy    [S, d]     their normals"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    counts = np.asarray(tb["counts"], dtype=np.uint64)
+    T, d = len(counts), wl["d"]
+    hf = 2 if wl["metric"] == "dot-product" else 1
+    base, nxt = np.zeros(T, np.uint64), T
+    for t in reversed(range(T)):
+        base[t] = nxt
+        nxt += int(counts[t]) - 1
+    arena = rig.ab.Arena()
+    rig.ctx.build_trees_emit(np.arange(T, dtype=np.uint32), base, arena=arena)
+    total = int(nxt)
+    kind = np.zeros(total, np.uint8)
+    left, right, card = np.zeros(total, np.uint32), np.zeros(total, np.uint32), np.zeros(total, np.uint64)
+    for i in range(total):
+        b = arena.get(i)
+        kind[i] = b[0]
+        if b[0] == 1:
+            size = int.from_bytes(b[5:9], "little")
+            card[i] = int(np.frombuffer(b, "<u2", 2 * size, 9)[1::2].astype(np.uint64).sum()) + size
+        else:
+            left[i], right[i] = int.from_bytes(b[1:5], "big"), int.from_bytes(b[5:9], "big")
+    rng = np.random.default_rng(0)
+
+    def sample(a):
+        return a if len(a) <= cap else a[np.sort(rng.choice(len(a), cap, replace=False))]
+    leaves = np.nonzero(kind == 1)[0]
+    np.save(os.path.join(out_dir, "node_counts.npy"), counts.astype(np.float64))
+    np.save(os.path.join(out_dir, "leaf_sizes.npy"), sample(np.stack([leaves, card[leaves]], 1).astype(np.float64)))
+    pairs, stack = [], [0] if T else []
+    while stack:
+        v = stack.pop()
+        if kind[v] == 1:
+            ids = roaring_ids(arena.get(v)[1:])
+            pairs.append(np.stack([ids.astype(np.float64), np.full(len(ids), float(v))], 1))
+        else:
+            stack.extend((int(left[v]), int(right[v])))
+    tl = np.concatenate(pairs) if pairs else np.zeros((0, 2))
+    np.save(os.path.join(out_dir, "tree0_item_leaf.npy"), sample(tl[np.argsort(tl[:, 0], kind="stable")]))
+    splits = np.nonzero(kind == 2)[0]
+    pick = np.sort(rng.choice(splits, min(n_normals, len(splits)), replace=False)) if len(splits) else splits
+    rec, normals = np.zeros((len(pick), 4)), np.zeros((len(pick), d), np.float32)
+    for j, v in enumerate(pick.tolist()):
+        b = arena.get(v)
+        rec[j] = (v, left[v], right[v], np.frombuffer(b, "<f4", 1, 9)[0] if len(b) > 9 else np.nan)
+        if len(b) > 9:
+            normals[j] = np.frombuffer(b, "<f4", d, 9 + 4 * hf)
+        else:
+            normals[j] = np.nan
+    np.save(os.path.join(out_dir, "split_nodes.npy"), rec)
+    np.save(os.path.join(out_dir, "split_normals.npy"), normals)
+    del arena
 
 
 def build_record(wl, tb, world):
@@ -668,7 +752,8 @@ def cpu_build_and_queries(wl, args, gpu_results):
 
 
 def headline_10m(rig, args):
-    """BASELINE.json's metric configuration itself: 10M x 768 Cosine, n_trees = 100 (fits one B200: 30.7 GB)."""
+    """BASELINE.json's metric configuration (Cosine, d = 768, n_trees = 100) at 5M rows. A step holds the item matrix twice (the
+    caller's device tensor it is staged from and the library's copy) plus its bf16 shadow: 10M rows would need ~82 GiB, 5M fit an 80 GB H100."""
     wl = WORKLOADS["h10m"]
     n, d, T = wl["n"], wl["d"], wl["n_trees"]
     ctx = rig.ctx
@@ -690,7 +775,7 @@ def headline_10m(rig, args):
                            "timing": "in the timed schedule: algorithmic scan bytes of one step / the device loop time of that step (all work_kernel launches run concurrently on 100 "
                                      "streams next to the control kernels, so this is a LOWER bound of the kernel's own rate)",
                            "root_scan": {"rows": n, "ms": root_ms, "GBps": n * d * 4 / (root_ms * 1e-3) / 1e9, "frac": n * d * 4 / (root_ms * 1e-3) / 1e9 / hbm,
-                                         "note": "one plain f32 work_kernel launch over all 10M rows, timed alone with CUDA events (30.7 GB: larger than L2)"}}
+                                         "note": "one plain f32 work_kernel launch over all rows, timed alone with CUDA events (15.4 GB: larger than L2)"}}
     if not args.no_e2e:
         e = e2e_single(rig, wl, items, seeds, steps=2, n_warm=1) if rig.world == 1 else e2e_multi(rig, wl, items, seeds, steps=2, n_warm=1)
         rec["e2e"] = e
@@ -711,10 +796,14 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-writer-e2e", action="store_true")
     ap.add_argument("--no-query", action="store_true")
-    ap.add_argument("--no-headline", action="store_true", help="skip the 10M x 768 sub-record of the default workload")
+    ap.add_argument("--no-headline", action="store_true", help="skip the 5M x 768 headline sub-record of the default workload")
     ap.add_argument("--no-c5", action="store_true", help="skip the config-5 sub-record of the default workload")
     ap.add_argument("--queries", type=int, default=1000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the forest the last timed step built as DIR/<name>.npy (see dump_forest)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     wl = WORKLOADS[args.workload]
     if args.workload == "c5":
         run_c5(args, wl)
@@ -733,6 +822,8 @@ def main():
     items = synth_items(rig, wl)     # generated on the device of rank 0 (counter-based ChaCha12 stream)
     seeds = derive_seeds(rig.ab, T)
     tb = timed_builds(rig, wl, items, seeds, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_forest(rig, wl, tb, args.dump_outputs)   # before anything else rebuilds on this context
     line = {
         "metric": "index-build vectors/sec", "value": tb["value"], "unit": "vectors/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": tb["ms_per_step"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",

@@ -1,5 +1,5 @@
 /*
- * arroy_b200.h — C ABI of the B200-native distance / split / re-rank path of arroy.
+ * arroy_b200.h — C ABI of the H100-native (sm_90a) distance / split / re-rank path of arroy.
  *
  * This is the drop-in boundary (SURVEY.md §8b): a fork of the reference binds these
  * entry points over Rust FFI (`extern "C"`, see INTEGRATION.md) and calls them where
@@ -298,7 +298,7 @@ int32_t arroy_b200_counters(arroy_ctx* ctx, uint64_t out[4]);
 
 /* The score matrix of the pre-filter, for tests and profiling: out_scores[q * n_rows + i] ~ dot(query q,
  * item rows[i]) computed with TF32 inputs and FP32 accumulation on the tensor cores; guaranteed within
- * 2^-8 * |q| * |item| of the exact dot product. engine 0 = the library's tcgen05 kernel, 1 = cuBLAS.
+ * 2^-8 * |q| * |item| of the exact dot product. engine 0 = the library's wgmma kernel, 1 = cuBLAS.
  * Needs dim >= 32. */
 int32_t arroy_b200_prefilter_scores(arroy_ctx* ctx, uint32_t nq, const float* queries /* nq x dim */,
                                     const uint32_t* rows, uint64_t n_rows, int32_t engine, float* out_scores);

@@ -9,7 +9,7 @@
 //   src/distance/mod.rs:126-171       two_means
 //   src/distance/{euclidean,cosine,dot_product,manhattan}.rs   the four Distance impls
 // Parity target: x86_64 with AVX+FMA detected (the class of host the reference runs on
-// next to a B200). Compile with -mavx2 -mfma -ffp-contract=off: Rust never contracts
+// next to a GPU). Compile with -mavx2 -mfma -ffp-contract=off: Rust never contracts
 // a*b+c, so every non-intrinsic mul/add below must stay separately rounded.
 #pragma once
 #include <immintrin.h>

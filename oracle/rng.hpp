@@ -3,7 +3,7 @@
 // --impl reference legs may build, link or call it.
 //
 // CPU restatement of the third-party RNG behaviour the reference's results depend
-// on. The crate is NOT vendored under /root/reference; what is restated here is the
+// on. The crate is NOT vendored in the arroy crate; what is restated here is the
 // published algorithm of:
 //   rand 0.8.5        (Cargo.toml:23)   StdRng, Rng::gen, gen_range, seq::index::sample
 //   rand_chacha 0.3.x (transitive)      ChaCha12Rng block layout, 4-block buffer

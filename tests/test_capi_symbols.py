@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_version_string():
-    assert b"sm_100a" in arroy_b200.load().arroy_b200_version()
+    assert b"sm_90a" in arroy_b200.load().arroy_b200_version()
 
 
 def test_create_fails_loudly_without_a_device():

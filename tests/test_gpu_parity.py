@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI,
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI,
 against the CPU oracle on the same seeded inputs. Bit-exact for ids, sides, margins, node bytes;
 distances bit-exact too (the tolerance the north star allows is 1e-5 relative — we assert 0)."""
 import numpy as np

@@ -94,7 +94,7 @@ def test_prefilter_nan_and_inf_inputs(ctx, monkeypatch):
 
 @pytest.mark.parametrize("d,nq,nc", [(768, 300, 5001), (33, 7, 258), (100, 129, 1000), (64, 1, 40)])
 def test_tensor_core_scores_are_within_the_bound(ctx, monkeypatch, d, nq, nc):
-    # the bound the whole pre-filter rests on: |S - q.c| <= 2^-8 |q| |c|, for the hand-written tcgen05
+    # the bound the whole pre-filter rests on: |S - q.c| <= 2^-8 |q| |c|, for the hand-written wgmma
     # kernel (engine 0, single-CTA and 2-CTA multicast variants) and optionally for cuBLAS (engine 1); ragged tile
     # edges in both directions
     n = nc + 50
@@ -127,6 +127,6 @@ def test_prefilter_engines_agree(ctx, monkeypatch):
     monkeypatch.setenv("ARROY_B200_XRERANK", "filter")
     monkeypatch.setenv("ARROY_B200_XGEMM", "cublas")
     a = ctx.rerank_shared(data[n:], h0[n:], rows, k)
-    monkeypatch.setenv("ARROY_B200_XGEMM", "tcgen05")
+    monkeypatch.setenv("ARROY_B200_XGEMM", "wgmma")
     b = ctx.rerank_shared(data[n:], h0[n:], rows, k)
     assert a[0].tolist() == b[0].tolist() and a[1].tobytes() == b[1].tobytes()
