@@ -70,6 +70,8 @@ SIGNATURES = [
     ("arroy_b200_epochs", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_bq_quantize", C.c_uint32, [_f32p, C.c_uint32, _f32p]),
     ("arroy_b200_build_shadow_stats", C.c_int32, [C.c_void_p, _u64p]),
+    ("arroy_b200_build_prefilter_stats", C.c_int32, [C.c_void_p, _u64p]),
+    ("arroy_b200_prefilter_planes", C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, _f32p]),
     ("arroy_b200_selftest_udiv", C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, _u64p, _u64p]),
     ("arroy_b200_stage_begin", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p]),
     ("arroy_b200_stage_rows", C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p)]),
@@ -318,6 +320,22 @@ class Context:
         out = (C.c_uint64 * 4)()
         self._ck(self.lib.arroy_b200_build_shadow_stats(self.h, out))
         return {"rows_via_bf16_shadow": int(out[0]), "rows_rescored_f32": int(out[1]), "rows_in_fused_root_pass": int(out[2]), "fused_root_rows_read": int(out[3])}
+
+    def build_prefilter_stats(self):
+        """Rows of the last build through each stage of side()'s 8-bit pre-filter: all of them read the hi plane (d bytes), the
+        stage-1 leftovers read both planes, the stage-2 leftovers the f32 row."""
+        out = (C.c_uint64 * 5)()
+        self._ck(self.lib.arroy_b200_build_prefilter_stats(self.h, out))
+        return {"rows_via_prefilter": int(out[0]), "rows_stage2": int(out[1]), "rows_rescored_f32": int(out[2]),
+                "rows_in_fused_root_pass": int(out[3]), "fused_root_rows_read": int(out[4])}
+
+    def prefilter_planes(self, n, ld):
+        """The pre-filter's encoding of the staged items: (hi int8 n x ld, lo int8 n x ld, scale f32 n)."""
+        hi = np.empty((n, ld), dtype=np.int8)
+        lo = np.empty((n, ld), dtype=np.int8)
+        scale = np.empty(n, dtype=np.float32)
+        self._ck(self.lib.arroy_b200_prefilter_planes(self.h, hi.ctypes.data, lo.ctypes.data, scale.ctypes.data_as(_f32p)))
+        return hi, lo, scale
 
     def build_stats(self):
         st = (C.c_double * 8)()

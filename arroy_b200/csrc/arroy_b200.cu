@@ -117,7 +117,7 @@ struct arroy_ctx {
     cudaStream_t side_stream = nullptr;   // host -> device flags while the persistent build kernel occupies `stream`
     cudaEvent_t ev_done = nullptr, ev_p0 = nullptr, ev_p1 = nullptr;   // ev_p0 / ev_p1 bracket the persistent build kernel
     double stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    uint64_t shadow_rows = 0, shadow_rescored = 0, fused_root_rows = 0, fused_root_read = 0;
+    uint64_t shadow_rows = 0, shadow_rescored = 0, shadow_stage2 = 0, fused_root_rows = 0, fused_root_read = 0;
     uint64_t wave_key[4] = {0, 0, 0, 0}, wave_max = 0, wave_trees_ok = 0; bool wave_key_valid = false;   // shapes of the last successful build (do_build_begin)   // last build: rows scanned through the bf16 shadow / re-scored from f32
     uint64_t n_launches = 0, h2d_bytes = 0, d2h_bytes = 0;  // since create (arroy_b200_counters)
     cudaEvent_t tev0 = nullptr, tev1 = nullptr;
@@ -155,7 +155,11 @@ struct arroy_ctx {
     // fused re-rank with a bf16 shadow of the items (frerank.cuh); built lazily by the first query after staging
     DevBuf fr_shadow, fr_norm, fr_gmax, fr_status;
     bool fr_valid = false;
-    bool shadow_valid = false;   // fr_shadow holds the bf16 copy of the staged items (also used by the build's scans)
+    bool shadow_valid = false;   // fr_shadow holds the bf16 copy of the staged items
+    // the build's side() pre-filter (kernels.cuh scan_claim_planes): 8-bit planes + row scales of the staged items, built by the
+    // first build after staging
+    DevBuf pl_hi, pl_lo, pl_scale;
+    bool planes_valid = false;
     uint64_t fr_batches = 0, fr_fallbacks = 0;   // last search_batch call, ms: bitmap clear + tree walk, candidate sort, distances, top-k   // last rerank_shared call, ms: prep, score GEMM, select, re-score, top-k, exact dense path
 };
 
@@ -200,9 +204,9 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
     if (is_bq(metric)) dim = (dim + 63u) / 64u * 64u;   // the bit string's length (binary_quantized.rs:80-92)
     if (n > 0xffffffffull) throw ArgError("too many items");
     for (uint64_t i = 1; i < n; ++i) if (ids[i] <= ids[i - 1]) throw ArgError("ids must be strictly ascending");
-    // a restage invalidates everything derived from the previous items: the bf16 shadow and the device forest
+    // a restage invalidates everything derived from the previous items: the bf16 shadow, the 8-bit planes and the device forest
     // (its descendant rows were validated against the previous item count)
-    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->forest_loaded = false; c->staging_open = false;
+    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false; c->staging_open = false;
     c->stage_epoch += 1;
     c->metric = metric; c->dim = dim; c->ld = (dim + 31u) & ~31u; c->n = n;
     c->ids.assign(ids, ids + n);
@@ -374,7 +378,7 @@ inline void launch_control(const void* fn, unsigned n_trees, int cs, size_t smem
     CK(cudaLaunchKernelExC(&cfg, fn, args));
 }
 
-void shadow_prepare(arroy_ctx* c);
+void planes_prepare(arroy_ctx* c);
 void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const uint8_t (*seeds)[32], uint32_t K, uint32_t cap_mult,
                 arroy_b200_cancel_fn cancel, void* cancel_arg, std::vector<BuiltTree>& out_trees, uint32_t& out_pool_stride, Subsets sub = Subsets{}) {
     const uint64_t n = c->n;
@@ -464,7 +468,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     if (ctrl_smem > 48 * 1024) CK(cudaFuncSetAttribute(control_fn(true, 1, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
     const size_t wsmem = work_smem(ld, (int)tw);
     if (wsmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-    if (wsmem + 4ull * ld > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + 4ull * ld)));
+    const size_t perm_smem = 4ull * planes_perm_floats(ld);   // work_kernel_shadow's second copy of the normal
+    if (wsmem + perm_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + perm_smem)));
     const int work_grid = c->sm_count * 3;
 
     // Two schedules over the same kernels:
@@ -523,15 +528,15 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             if (persist) if (const char* ge = getenv("ARROY_B200_PGRID")) pgrid = std::max((int)tw + 16, std::min(pgrid, atoi(ge)));   // experiments: fewer resident CTAs
         }
     }
-    // scans through the bf16 shadow of the items (kernels.cuh scan_claim_shadow): nodes of more than shadow_min_units units
+    // scans through the 8-bit planes of the items (kernels.cuh scan_claim_planes): nodes of more than shadow_min_units units
     {
         const char* se = getenv("ARROY_B200_SHADOW");
-        const bool want = !(se && atoi(se) == 0) && !is_bq(c->metric) && P.d >= 64 && P.d <= SHADOW_MAX_D && n * (uint64_t)ld >= (1ull << 22);
+        const bool want = !(se && atoi(se) == 0) && !is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && n * (uint64_t)ld >= (1ull << 22);
         if (want) {
-            shadow_prepare(c);
-            P.shadow = c->fr_shadow.as<uint16_t>();
-            W.shadow_stats.ensure(16);
-            CK(cudaMemsetAsync(W.shadow_stats.p, 0, 16, c->stream));
+            planes_prepare(c);
+            P.planes = PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()};
+            W.shadow_stats.ensure(24);
+            CK(cudaMemsetAsync(W.shadow_stats.p, 0, 24, c->stream));
             P.shadow_stats = W.shadow_stats.as<unsigned long long>();
             // many trees per GPU: bandwidth decides, every node goes through the shadow; few: the chain of attempts decides and
             // small nodes keep the one-unit claims of the exact scan (more CTAs per node)
@@ -561,12 +566,12 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
 
     auto launch_step = [&](cudaStream_t s) {  // lockstep: all trees per launch
         launch_control(ctrl1, tw, 1, ctrl_smem, s, P, 0u);
-        if (P.shadow) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + 4ull * ld, s>>>(P.jobs, (int)tw, P.items, P.shadow, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+        if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + perm_smem, s>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
         else work_kernel<<<work_grid, WORK_THREADS, wsmem, s>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric, interleave);
     };
     auto launch_tree_step = [&](uint32_t t, cudaStream_t s) {  // async: one tree per launch
         launch_control(ctrlc, 1, cluster, ctrl_smem, s, P, t);
-        if (P.shadow) work_kernel_shadow<<<tree_grid, WORK_THREADS, wsmem1 + 4ull * ld, s>>>(P.jobs + t, 1, P.items, P.shadow, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+        if (P.planes.hi) work_kernel_shadow<<<tree_grid, WORK_THREADS, wsmem1 + perm_smem, s>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
         else work_kernel<<<tree_grid, WORK_THREADS, wsmem1, s>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric, 0);
     };
     if (!lockstep) {
@@ -671,7 +676,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             for (int i = 0; i < steps_per_batch; ++i) {
                 launch_control(ctrl1, tw, 1, ctrl_smem, c->stream, P, 0u);
                 CK(cudaEventRecord(pev[2 * i], c->stream));
-                if (P.shadow) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + 4ull * ld, c->stream>>>(P.jobs, (int)tw, P.items, P.shadow, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+                if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + perm_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
                 else work_kernel<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric, interleave);
                 CK(cudaEventRecord(pev[2 * i + 1], c->stream));
             }
@@ -755,10 +760,10 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     }
     if (persist && P.root_fused) { c->fused_root_rows += (uint64_t)tw * n; c->fused_root_read += n; }
     if (P.shadow_stats) {
-        unsigned long long hs[2] = {0, 0};
-        CK(cudaMemcpyAsync(hs, P.shadow_stats, 16, cudaMemcpyDeviceToHost, c->stream));
+        unsigned long long hs[3] = {0, 0, 0};
+        CK(cudaMemcpyAsync(hs, P.shadow_stats, 24, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
-        c->shadow_rows += hs[0]; c->shadow_rescored += hs[1];
+        c->shadow_rows += hs[0]; c->shadow_rescored += hs[1]; c->shadow_stage2 += hs[2];
     }
     CK(cudaStreamSynchronize(c->stream));
     c->d2h_bytes += (uint64_t)pool_used * pool_stride * 4 + sizeof(TreeState) * tw + sizeof(Record) * total_recs + 4ull * n * tw;
@@ -771,7 +776,7 @@ void do_build_begin(arroy_ctx* c, uint32_t n_trees, const uint8_t (*seeds)[32], 
     require_staged(c);
     set_device(c);
     for (auto& s : c->stats) s = 0;
-    c->shadow_rows = 0; c->shadow_rescored = 0; c->fused_root_rows = 0; c->fused_root_read = 0;
+    c->shadow_rows = 0; c->shadow_rescored = 0; c->shadow_stage2 = 0; c->fused_root_rows = 0; c->fused_root_read = 0;
     c->pending_waves.clear(); c->pending_wave_t0.clear(); c->pending_n_trees = 0;
     const uint32_t K = split_after ? split_after : c->dim;
     if (!sub.rows && c->n <= K) throw ArgError("build_trees needs more items than split_after (a single Descendants node is the caller's job, src/writer.rs:499-501)");
@@ -1016,7 +1021,7 @@ bool frerank_enabled(arroy_ctx* c, uint32_t k) {
     return !off && c->metric != MANHATTAN && !is_bq(c->metric) && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
 }
 
-// bf16 copy of the staged items (round to nearest even; padding stays zero), shared by the fused re-rank and the build's scans
+// bf16 copy of the staged items (round to nearest even; padding stays zero) for the fused re-rank
 void shadow_prepare(arroy_ctx* c) {
     if (c->shadow_valid) return;
     const uint64_t total4 = (uint64_t)c->n * c->ld / 4;
@@ -1025,6 +1030,20 @@ void shadow_prepare(arroy_ctx* c) {
     CK(cudaGetLastError());
     c->n_launches += 1;
     c->shadow_valid = true;
+}
+
+// the build's pre-filter encoding of the staged items (kernels.cuh planes_encode_kernel): two int8 planes and a scale per row
+void planes_prepare(arroy_ctx* c) {
+    if (c->planes_valid) return;
+    const size_t bytes = std::max<size_t>(16, (size_t)c->n * c->ld);
+    c->pl_hi.ensure(bytes);
+    c->pl_lo.ensure(bytes);
+    c->pl_scale.ensure(std::max<size_t>(16, (size_t)c->n * 4));
+    const uint64_t blocks = std::max<uint64_t>(1, std::min<uint64_t>((c->n + 7) / 8, (uint64_t)c->sm_count * 16));
+    planes_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(c->items.as<float>(), c->n, c->ld, c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>());
+    CK(cudaGetLastError());
+    c->n_launches += 1;
+    c->planes_valid = true;
 }
 
 void frerank_prepare(arroy_ctx* c) {
@@ -1236,7 +1255,7 @@ void arroy_b200_destroy(arroy_ctx* c) {
     DevBuf* bufs[] = {&c->items, &c->h0, &c->h1, &c->norms, &c->maxbits, &c->s_rows, &c->s_flags, &c->s_margins, &c->s_normal, &c->s_unit, &c->s_job,
                       &c->s_keys, &c->s_keys2, &c->s_dists, &c->s_q, &c->s_qh0, &c->s_off, &c->s_orows, &c->s_odist, &c->s_olen, &c->s_misc};
     for (auto* b : bufs) b->release();
-    { DevBuf* xb[] = {&c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag}; for (auto* b : xb) b->release(); }
+    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag}; for (auto* b : xb) b->release(); }
     if (c->blas) cublasDestroy(c->blas);
     for (auto& e : c->xev) if (e) cudaEventDestroy(e);
     if (c->cached_exec) cudaGraphExecDestroy(c->cached_exec);
@@ -1569,6 +1588,25 @@ int32_t arroy_b200_build_stats(arroy_ctx* c, double stats[8]) {
 }
 int32_t arroy_b200_build_shadow_stats(arroy_ctx* c, uint64_t out[4]) {
     return guarded(c, [&] { if (!out) throw ArgError("null argument"); out[0] = c->shadow_rows; out[1] = c->shadow_rescored; out[2] = c->fused_root_rows; out[3] = c->fused_root_read; });
+}
+int32_t arroy_b200_build_prefilter_stats(arroy_ctx* c, uint64_t out[5]) {
+    return guarded(c, [&] {
+        if (!out) throw ArgError("null argument");
+        out[0] = c->shadow_rows; out[1] = c->shadow_stage2; out[2] = c->shadow_rescored; out[3] = c->fused_root_rows; out[4] = c->fused_root_read;
+    });
+}
+int32_t arroy_b200_prefilter_planes(arroy_ctx* c, int8_t* hi, int8_t* lo, float* scale) {
+    return guarded(c, [&] {
+        if (!hi || !lo || !scale) throw ArgError("null argument");
+        require_staged(c);
+        set_device(c);
+        planes_prepare(c);
+        const size_t bytes = (size_t)c->n * c->ld;
+        CK(cudaMemcpyAsync(hi, c->pl_hi.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(lo, c->pl_lo.p, bytes, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpyAsync(scale, c->pl_scale.p, (size_t)c->n * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+    });
 }
 
 int32_t arroy_b200_rerank(arroy_ctx* c, const float* query, float qhdr0, float qhdr1, const uint32_t* rows, uint64_t n_rows, uint32_t k,

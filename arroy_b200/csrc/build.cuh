@@ -105,10 +105,11 @@ struct BuildParams {
     const volatile int* abort;    // set by the host (cancel): control CTAs stop at their next wait
     // fused root scan: when every tree of the wave starts at the root of the whole index, the first split's side() scans of all
     // trees read the same rows — the workers do them in ONE pass over the item matrix (proot below)
-    // bf16 copy of the item matrix (n x ld), or NULL: scans of more than shadow_min_units units go through it (scan_claim_shadow)
-    const uint16_t* shadow;
+    // the 8-bit planes of the item matrix (kernels.cuh), or NULLs: scans of more than shadow_min_units units go through them
+    // (scan_claim_planes)
+    PlaneRows planes;
     uint32_t shadow_min_units, shadow_small_chunk, shadow_big_units, shadow_big_chunk;
-    unsigned long long* shadow_stats;   // [0] rows scanned through the shadow, [1] of them re-scored from the f32 row
+    unsigned long long* shadow_stats;   // [0] rows scanned through the planes, [1] of them re-scored from the f32 row, [2] through stage 2
     int32_t root_fused;
     uint32_t* root_ready;         // number of trees whose root normal is published
     uint32_t* root_ticket;        // next unclaimed chunk of the fused pass
@@ -991,15 +992,17 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ uint32_t w_t, w_u0, w_n, w_seq, w_pseq, w_found, w_exit, w_count;
     __shared__ PSlot w_job;        // fields of the claimed job (first 64 bytes)
     __shared__ uint32_t w_sm[16];
-    __shared__ uint32_t w_list[SCAN_UNIT * SHADOW_CHUNK];   // positions the bf16 pass could not decide
-    __shared__ uint32_t w_cnt[SHADOW_CHUNK + 1];
-    float* sm_perm = sm_normal + P.ld;                      // the normal in the bf16 rows' lane order
+    __shared__ uint32_t w_list[SCAN_UNIT * PLANES_CHUNK], w_list2[SCAN_UNIT * PLANES_CHUNK];   // positions stage 1 / stage 2 could not decide
+    __shared__ uint32_t w_cnt[PLANES_CHUNK + 2];
+    __shared__ double w_l1[CTRL_THREADS / 32];
+    float* sm_perm = sm_normal + P.ld;                      // the normal in the planes' lane order
     const uint32_t T = P.n_trees;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t rot = (blockIdx.x - T) * 7u;
     const bool latency_class = ((blockIdx.x - T) & P.lat_mask) == 0u;
     uint32_t loaded_t = 0xffffffffu, loaded_seq = 0xffffffffu;
     float nh0 = 0.f;
+    float2 wf = make_float2(0.f, 0.f);   // the loaded normal's bound factors (scan_claim_planes)
     if (tid == 0) w_exit = 0;
     if (P.root_fused) proot(P, sm_normal);
     for (;;) {
@@ -1078,21 +1081,25 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
             if (jb.kind == JOB_SCAN) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
                 if (want_normal || seq != w_pseq) {
+                    double l1 = 0.0;
 #pragma unroll
                     for (int u = 0; u < 8; ++u) {
                         const uint32_t i = tid + u * CTRL_THREADS;
                         if (i < P.ld) {
                             sm_normal[i] = nreg[u];
-                            if (P.shadow != nullptr) { const uint32_t q = i >> 3, w = i & 7u; sm_perm[(((q >> 3) * 16u + (w >> 2) * 8u + (q & 7u)) << 2) + (w & 3u)] = nreg[u]; }
+                            if (P.planes.hi != nullptr) { sm_perm[planes_perm_index(i)] = nreg[u]; l1 += (double)fabsf(nreg[u]); }
                         }
                     }
+                    if (P.planes.hi != nullptr) { l1 = warp_sum_f64(l1); if (lane == 0) w_l1[warp] = l1; }
                     nh0 = __ldcg(nsrc);
                     loaded_t = t; loaded_seq = seq;
                     __syncthreads();
+                    if (P.planes.hi != nullptr) wf = planes_job_factors(w_l1, P.d);
                 }
-                if (P.shadow != nullptr && units > P.shadow_min_units)
-                    for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += SHADOW_CHUNK)
-                        scan_claim_shadow(jb, u, min(min(units, (g0 + 1u) * chunk), u + SHADOW_CHUNK), P.items, P.shadow, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_perm, nh0, w_list, w_cnt, P.shadow_stats);
+                if (P.planes.hi != nullptr && units > P.shadow_min_units)
+                    for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
+                        scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_perm, nh0,
+                                          wf.x, wf.y, w_list, w_list2, w_cnt, P.shadow_stats);
                 else
                     for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
             } else if (jb.kind == JOB_PARTITION) {
@@ -1326,8 +1333,8 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
                         atomicAdd(P.root_ready, 1u);
                         s_wait_ok = pwait(P, P.slots[t], s_pseq, units) ? 1 : 0;
                     } else {
-                    // a claim = `chunk` units: four for the big scans (and for everything that goes through the bf16 shadow)
-                    const bool via_shadow = P.shadow != nullptr && units > P.shadow_min_units;
+                    // a claim = `chunk` units: four for the big scans (and for everything that goes through the 8-bit planes)
+                    const bool via_shadow = P.planes.hi != nullptr && units > P.shadow_min_units;
                     const uint32_t chunk = via_shadow ? (units > P.shadow_big_units ? P.shadow_big_chunk : (units > 128u ? 4u : P.shadow_small_chunk)) : (units > 1024u ? 4u : 1u), groups = (units + chunk - 1) / chunk;
                     ppublish(P.slots[t], job, s_pseq, groups, chunk);
                     s_wait_ok = pwait(P, P.slots[t], s_pseq, groups) ? 1 : 0;

@@ -141,47 +141,144 @@ __device__ __forceinline__ void scan_unit(const Job& jb, uint32_t unit, const fl
     if (threadIdx.x == 0 && jb.unit_left) jb.unit_left[unit] = *sm_count;
 }
 
-// ---- side() through a bf16 shadow of the items --------------------------------------------------------------------------
-// side() only needs the SIGN of the margin, and a scan is bound by the bytes of the rows it reads. The claim's rows are first
-// read from a bf16 copy of the item matrix (half the bytes): with x~ = bf16(x) (round to nearest: |x~ - x| <= 2^-9 |x|) an
-// ordinary f32 dot m~ = sum n_i x~_i and A~ = sum |n_i| |x~_i| satisfy, against the margin m_ref the reference computes in its
-// own order (|m_ref - sum n_i x_i| <= gamma A, gamma ~ d 2^-24, A = sum |n_i x_i|),
-//        |m~ + c - (m_ref's exact value)| <= (2^-9 + 2 gamma) A~ / (1 - 2^-9 - gamma) < (2^-9 (1 + 2^-8) + 2.5 d 2^-24) A~ =: rel(d) A~
-// (c = the bias / extra_dim term, formed exactly as the reference forms it; fl(a + b) has the sign of a + b; rel(768) = 0.00208,
-// rel(8192) = 0.0033). So when |m~ + c| > rel(d) A~ the side is certain; every other row — near the hyperplane, zero, non-finite — is put on a list and scored
-// from the f32 row in the reference's summation order (the code of scan_unit). Flags and unit counts are the exact scan's.
-// sm_perm: the normal re-laid for the bf16 row layout: the 8 elements of 16-byte word q = 8 c + g of a row sit at float4
-// 16 c + g and 16 c + 8 + g, so that the eight lanes of a row read consecutive float4s.
-__host__ __device__ __forceinline__ float shadow_rel(uint32_t d) { return 0.001962f + (float)d * 1.6e-7f; }   // both constants rounded up
-constexpr uint32_t SHADOW_MAX_D = 8192;
-constexpr uint32_t SHADOW_CHUNK = 4;         // scan units per claim on this path (256 rows)
+// ---- side() through a two-plane 8-bit pre-filter of the items -----------------------------------------------------------
+// side() only needs the SIGN of the margin, and a scan is bound by the bytes of the rows it reads. Every row is encoded once per
+// staging (planes_encode_kernel) as a scale s = fl(M / 127), M = max_i |x_i|, and two int8 planes (u = 2^-24):
+//     q_i = fl(x_i / s),   h_i = rint(q_i),   l_i = rint(fl((q_i - h_i) * 254))      (q_i - h_i is exact)
+// The quotient is rounded once and the constants are rounded up to cover it (|q_i| <= 127 (1 + u)): |x_i - s h_i| <= s E1,
+// E1 = 1/2 + 128 u, and with y_i = 254 h_i + l_i (an exact integer in f32), |x_i - s y_i / 254| <= s E2, E2 = 1/508 + 129 u < 0.001977.
+// A row whose scale is not a normal finite f32 keeps zero planes and is never decided through them: M = 0 stores s = 0 (the
+// row's dot is exactly 0), M = inf stores +inf, a NaN or tiny (M < 127 FLT_MIN) row stores NaN (0x7fffffff); the tests below
+// are false for NaN and +inf.
+// The reference's margin is fl(dot + c) (c = the bias / extra-dim term, formed exactly as the reference forms it; fl keeps the
+// sign of dot + c), with |dot - sum n_i x_i| <= gamma_R sum |n_i x_i|, gamma_R <= 1.001 d u in any summation order, and
+// sum |n_i x_i| <= 127.001 s |n|_1. A lane sums a row in two f32 chains of at most ld/16 + 7 terms, then 1 + 3 adds: gamma_k <=
+// (d/8 + 16) u for either stage. N1 >= |n|_1 is summed in f64 once per job and rounded up.
+//  stage 1, hi plane only (d bytes per row): t = f32 sum n_i h_i (sum |n_i h_i| <= 127 |n|_1), and
+//    |dot - fl(s t)| <= s |n|_1 (E1 + 127.001 (gamma_R + gamma_k + u)) <= s N1 K1(d) / (1 + 2^-20),  K1(d) = 0.5002 + 8.6e-6 d;
+//    the row is certain when |fl(fl(s t) + c)| > fl(s w1), w1 = N1 K1(d) rounded up (the factor 1 + 2^-20 covers the test's
+//    own roundings).
+//  stage 2, the rows stage 1 left (both planes; the hi row was just streamed by this CTA): m = f32 sum n_i y_i,
+//    A = f32 sum |n_i| |y_i|, s2 = fl(s / 254), and
+//    |dot - fl(s2 m)| <= s2 (254 E2 |n|_1 (1 + gamma_R) + A (gamma_R + gamma_k + 4 u)) <= s2 (N1 W2(d) + rel2(d) A) / (1 + 2^-20),
+//    W2(d) = 0.50216 (1 + 6.1e-8 (d + 16)), rel2(d) = 1.3e-6 + 6.8e-8 d; certain when |fl(fl(s2 m) + c)| > fl(s2 fl(w2 + fl(rel2 A))),
+//    w2 = N1 W2(d) rounded up.
+//  stage 3: every other row — near the hyperplane, zero, non-finite — is scored from the f32 row in the reference's summation
+//    order (scan_unit's arithmetic). Flags and unit counts are the exact scan's.
+// The bounds are relative: like any such rule they assume that no product n_i x_i underflows.
+// sm_perm: the normal re-laid for the planes' lane order: the 16 elements of 16-byte word q = 8 c + g of a row sit at float4
+// 32 c + 8 j + g (j = 0..3, four elements each), so that the eight lanes of a row read consecutive float4s.
+__host__ __device__ __forceinline__ float planes_k1(uint32_t d) { return 0.5002f + (float)d * 8.6e-6f; }
+__host__ __device__ __forceinline__ float planes_w2(uint32_t d) { return 0.50216f * (1.0f + 6.1e-8f * (float)(d + 16u)); }
+__host__ __device__ __forceinline__ float planes_rel2(uint32_t d) { return 1.3e-6f + (float)d * 6.8e-8f; }
+__host__ __device__ __forceinline__ uint32_t planes_perm_floats(uint32_t ld) { return (ld + 127u) & ~127u; }   // sm_perm's size
+__host__ __device__ __forceinline__ uint32_t planes_perm_index(uint32_t i) {
+    const uint32_t q = i >> 4, w = i & 15u;
+    return (((q >> 3) * 32u + (w >> 2) * 8u + (q & 7u)) << 2) + (w & 3u);
+}
+constexpr uint32_t PLANES_MAX_D = 8192;
+constexpr uint32_t PLANES_CHUNK = 4;          // scan units per claim on this path (256 rows)
+
+struct PlaneRows {
+    const int8_t* hi;       // n x ld, h_i
+    const int8_t* lo;       // n x ld, l_i
+    const float* scale;     // n, s
+};
+
+// Encoder: one warp per row. Padding columns are zero in the items, so they are zero in both planes.
+__global__ void __launch_bounds__(256) planes_encode_kernel(const float* __restrict__ items, uint64_t n, uint32_t ld, int8_t* __restrict__ hi,
+                                                            int8_t* __restrict__ lo, float* __restrict__ scale) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t n4 = ld >> 2;
+    const uint64_t nw = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t r = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nw) {
+        const float4* row = reinterpret_cast<const float4*>(items + r * ld);
+        uint32_t mb = 0;   // max of |x| as bits: the uint order of non-negative floats, with NaN above +inf
+        for (uint32_t k = lane; k < n4; k += 32) {
+            const float4 v = row[k];
+            mb = max(max(mb, __float_as_uint(fabsf(v.x))), max(__float_as_uint(fabsf(v.y)), max(__float_as_uint(fabsf(v.z)), __float_as_uint(fabsf(v.w)))));
+        }
+        mb = __reduce_max_sync(0xffffffffu, mb);
+        const float M = __uint_as_float(mb);
+        float s = __fdiv_rn(M, 127.0f);
+        const bool ok = s >= 1.17549435e-38f && s <= 3.40282347e+38f;
+        if (!ok && mb != 0u && mb != 0x7f800000u) s = __int_as_float(0x7fffffff);
+        uint32_t* H = reinterpret_cast<uint32_t*>(hi + r * ld);
+        uint32_t* L = reinterpret_cast<uint32_t*>(lo + r * ld);
+        for (uint32_t k = lane; k < n4; k += 32) {
+            const float4 v = row[k];
+            const float x[4] = {v.x, v.y, v.z, v.w};
+            uint32_t hw = 0, lw = 0;
+            if (ok) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float q = __fdiv_rn(x[j], s), h = rintf(q);
+                    const float l = rintf(__fmul_rn(__fsub_rn(q, h), 254.0f));
+                    hw |= ((uint32_t)(int)h & 0xffu) << (8 * j);
+                    lw |= ((uint32_t)(int)l & 0xffu) << (8 * j);
+                }
+            }
+            H[k] = hw; L[k] = lw;
+        }
+        if (lane == 0) scale[r] = s;
+    }
+}
 
 __device__ __forceinline__ uint4 ldg_stream_u4(const uint4* p) {
     uint4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
-__device__ __forceinline__ void shadow_fma8(const uint4 v, const float4 y0, const float4 y1, float& m0, float& m1, float& a0, float& a1) {
-    const float x0 = __uint_as_float(v.x << 16), x1 = __uint_as_float(v.x & 0xffff0000u), x2 = __uint_as_float(v.y << 16), x3 = __uint_as_float(v.y & 0xffff0000u);
-    const float x4 = __uint_as_float(v.z << 16), x5 = __uint_as_float(v.z & 0xffff0000u), x6 = __uint_as_float(v.w << 16), x7 = __uint_as_float(v.w & 0xffff0000u);
-    m0 = fmaf(x0, y0.x, m0); m1 = fmaf(x1, y0.y, m1); m0 = fmaf(x2, y0.z, m0); m1 = fmaf(x3, y0.w, m1);
-    m0 = fmaf(x4, y1.x, m0); m1 = fmaf(x5, y1.y, m1); m0 = fmaf(x6, y1.z, m0); m1 = fmaf(x7, y1.w, m1);
-    a0 = fmaf(fabsf(x0), fabsf(y0.x), a0); a1 = fmaf(fabsf(x1), fabsf(y0.y), a1); a0 = fmaf(fabsf(x2), fabsf(y0.z), a0); a1 = fmaf(fabsf(x3), fabsf(y0.w), a1);
-    a0 = fmaf(fabsf(x4), fabsf(y1.x), a0); a1 = fmaf(fabsf(x5), fabsf(y1.y), a1); a0 = fmaf(fabsf(x6), fabsf(y1.z), a0); a1 = fmaf(fabsf(x7), fabsf(y1.w), a1);
+// byte k of w (signed) as a float, without I2F: b ^ 0x80 = b + 128 is put into the mantissa of 2^23 (exactly 2^23 + 128 + b),
+// one add removes the offset. wx = w ^ 0x80808080.
+__device__ __forceinline__ float s8_to_f32(uint32_t wx, uint32_t k) {
+    return __fsub_rn(__uint_as_float(__byte_perm(wx, 0x4B000000u, 0x7540u | k)), 8388736.0f);
+}
+// 16 hi-plane elements of one word times their normal elements (y: the four float4s of sm_perm for this word): two chains
+__device__ __forceinline__ void planes_fma16(const uint4 v, const float4 (&y)[4], float& m0, float& m1) {
+    const uint32_t w[4] = {v.x ^ 0x80808080u, v.y ^ 0x80808080u, v.z ^ 0x80808080u, v.w ^ 0x80808080u};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        m0 = fmaf(s8_to_f32(w[j], 0), y[j].x, m0); m1 = fmaf(s8_to_f32(w[j], 1), y[j].y, m1);
+        m0 = fmaf(s8_to_f32(w[j], 2), y[j].z, m0); m1 = fmaf(s8_to_f32(w[j], 3), y[j].w, m1);
+    }
+}
+// the same word of both planes: y = 254 h + l (exact), m += n y, a += |n| |y|
+__device__ __forceinline__ void planes_fma16x2(const uint4 vh, const uint4 vl, const float4 (&y)[4], float& m0, float& m1, float& a0, float& a1) {
+    const uint32_t wh[4] = {vh.x ^ 0x80808080u, vh.y ^ 0x80808080u, vh.z ^ 0x80808080u, vh.w ^ 0x80808080u};
+    const uint32_t wl[4] = {vl.x ^ 0x80808080u, vl.y ^ 0x80808080u, vl.z ^ 0x80808080u, vl.w ^ 0x80808080u};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float n4[4] = {y[j].x, y[j].y, y[j].z, y[j].w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float v = fmaf(s8_to_f32(wh[j], (uint32_t)k), 254.0f, s8_to_f32(wl[j], (uint32_t)k));
+            if (k & 1) { m1 = fmaf(v, n4[k], m1); a1 = fmaf(fabsf(v), fabsf(n4[k]), a1); }
+            else { m0 = fmaf(v, n4[k], m0); a0 = fmaf(fabsf(v), fabsf(n4[k]), a0); }
+        }
+    }
 }
 
-// scan units [u0, u1) (at most SHADOW_CHUNK) of a job. sm_list: 64 * SHADOW_CHUNK positions; sm_cnt: SHADOW_CHUNK + 1 counters.
-__device__ __forceinline__ void scan_claim_shadow(const Job& jb, uint32_t u0, uint32_t u1, const float* __restrict__ items, const uint16_t* __restrict__ shadow,
+__device__ __forceinline__ float prefilter_finish(int metric, float v, float nh0, float item_h0) {
+    if (metric == COSINE) return v;
+    if (metric == DOT_PRODUCT) return __fadd_rn(v, __fmul_rn(nh0, item_h0));
+    return __fadd_rn(nh0, v);
+}
+
+// scan units [u0, u1) (at most PLANES_CHUNK) of a job. sm_list, sm_list2: 64 * PLANES_CHUNK positions each (the rows stage 1,
+// stage 2 left); sm_cnt: PLANES_CHUNK + 2 counters. w1, w2: the job's bound factors (above). stats (optional): [0] rows through
+// the pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
+__device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, uint32_t u1, const float* __restrict__ items, const PlaneRows pl,
                                                   const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric, const float* sm_normal, const float* sm_perm,
-                                                  float nh0, uint32_t* sm_list, uint32_t* sm_cnt, unsigned long long* stats) {
+                                                  float nh0, float w1, float w2, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt, unsigned long long* stats) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
-    if (tid <= (int)SHADOW_CHUNK) sm_cnt[tid] = 0;
+    if (tid <= (int)PLANES_CHUNK + 1) sm_cnt[tid] = 0;
     __syncthreads();
     const uint32_t base = u0 * SCAN_UNIT, end = min(jb.len, u1 * SCAN_UNIT);
-    const uint32_t nq = ld >> 3;                       // 16-byte words per shadow row
+    const uint32_t nq = ld >> 4;                       // 16-byte words per plane row
     const int nsteps = (int)((nq + 7) >> 3);
     const float4* PN = reinterpret_cast<const float4*>(sm_perm);
-    const float rel = shadow_rel(d);
+    // ---- stage 1: the hi plane of every row ----
     for (uint32_t pbase = base; pbase < end; pbase += 128) {
         uint32_t pos[4], rid[4];
         const uint4* S[4];
@@ -189,11 +286,11 @@ __device__ __forceinline__ void scan_claim_shadow(const Job& jb, uint32_t u0, ui
         for (int r = 0; r < 4; ++r) {
             pos[r] = pbase + warp * 16 + grp * 4 + r;
             rid[r] = pos[r] < end ? (jb.rows ? __ldcg(jb.rows + pos[r]) : pos[r]) : 0u;
-            S[r] = reinterpret_cast<const uint4*>(shadow + (size_t)rid[r] * ld) + g8;
+            S[r] = reinterpret_cast<const uint4*>(pl.hi + (size_t)rid[r] * ld) + g8;
         }
-        float m0[4], m1[4], a0[4], a1[4];
+        float m0[4], m1[4];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) { m0[r] = 0.f; m1[r] = 0.f; a0[r] = 0.f; a1[r] = 0.f; }
+        for (int r = 0; r < 4; ++r) { m0[r] = 0.f; m1[r] = 0.f; }
         for (int c0 = 0; c0 < nsteps; c0 += 3) {
             uint4 v[3][4];
 #pragma unroll
@@ -206,42 +303,86 @@ __device__ __forceinline__ void scan_claim_shadow(const Job& jb, uint32_t u0, ui
 #pragma unroll
             for (int sidx = 0; sidx < 3; ++sidx) {
                 const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                float4 y0 = make_float4(0.f, 0.f, 0.f, 0.f), y1 = y0;
-                if (q < nq) { y0 = PN[(c0 + sidx) * 16 + g8]; y1 = PN[(c0 + sidx) * 16 + 8 + g8]; }
+                float4 y[4];
 #pragma unroll
-                for (int r = 0; r < 4; ++r) shadow_fma8(v[sidx][r], y0, y1, m0[r], m1[r], a0[r], a1[r]);
+                for (int j = 0; j < 4; ++j) y[j] = q < nq ? PN[(c0 + sidx) * 32 + j * 8 + g8] : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                for (int r = 0; r < 4; ++r) planes_fma16(v[sidx][r], y, m0[r], m1[r]);
             }
         }
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-            float m = m0[r] + m1[r], a = a0[r] + a1[r];
+            float t = m0[r] + m1[r];
 #pragma unroll
-            for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
+            for (int o = 1; o < 8; o <<= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
             const bool valid = pos[r] < end;
-            float mt;
-            if (metric == COSINE) mt = m;
-            else if (metric == DOT_PRODUCT) mt = m + __fmul_rn(nh0, valid ? ih0[rid[r]] : 0.f);
-            else mt = nh0 + m;
-            const bool certain = fabsf(mt) > rel * a;                 // false for NaN / Inf / an all-zero row
+            const float s = valid ? __ldg(pl.scale + rid[r]) : 0.f;
+            const float mt = prefilter_finish(metric, __fmul_rn(s, t), nh0, (metric == DOT_PRODUCT && valid) ? ih0[rid[r]] : 0.f);
+            const bool certain = fabsf(mt) > __fmul_rn(s, w1);      // false for NaN / Inf scales
             const bool leader = g8 == 0 && valid;
             const int side = mt > 0.f ? 1 : 0;
             if (leader && certain) jb.flags[pos[r]] = (uint8_t)side;
-            if (leader && !certain) sm_list[atomicAdd(&sm_cnt[SHADOW_CHUNK], 1u)] = pos[r];
+            if (leader && !certain) sm_list[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = pos[r];
             const unsigned lefts = __ballot_sync(0xffffffffu, leader && certain && side == 0);
             // the four groups of a warp hold positions of the same unit (16 consecutive positions per warp)
             if (lane == 0 && lefts) atomicAdd(&sm_cnt[(pbase + warp * 16 - base) / SCAN_UNIT], (uint32_t)__popc(lefts));
         }
     }
     __syncthreads();
-    // the uncertain rows, exactly: one 8-lane group per row, scan_unit's arithmetic
-    const uint32_t nl = sm_cnt[SHADOW_CHUNK];
-    if (stats != nullptr && tid == 0) { atomicAdd(stats, (unsigned long long)(end - base)); if (nl) atomicAdd(stats + 1, (unsigned long long)nl); }   // rows through the shadow / re-scored
+    // ---- stage 2: both planes of the rows stage 1 left, one 8-lane group per row ----
+    const uint32_t n1 = sm_cnt[PLANES_CHUNK];
+    const float rel2 = planes_rel2(d);
+    for (uint32_t it = 0; it * 32u < n1; ++it) {
+        const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
+        const bool act = idx < n1;
+        const uint32_t p = act ? sm_list[idx] : base;
+        const uint32_t r = jb.rows ? __ldcg(jb.rows + p) : p;
+        const uint4* Hr = reinterpret_cast<const uint4*>(pl.hi + (size_t)r * ld) + g8;
+        const uint4* Lr = reinterpret_cast<const uint4*>(pl.lo + (size_t)r * ld) + g8;
+        float m0 = 0.f, m1 = 0.f, a0 = 0.f, a1 = 0.f;
+        for (int c0 = 0; c0 < nsteps; c0 += 3) {
+            uint4 vh[3], vl[3];
+#pragma unroll
+            for (int sidx = 0; sidx < 3; ++sidx) {
+                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
+                vh[sidx] = q < nq ? ldg_stream_u4(Hr + (c0 + sidx) * 8) : make_uint4(0u, 0u, 0u, 0u);
+                vl[sidx] = q < nq ? ldg_stream_u4(Lr + (c0 + sidx) * 8) : make_uint4(0u, 0u, 0u, 0u);
+            }
+#pragma unroll
+            for (int sidx = 0; sidx < 3; ++sidx) {
+                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
+                float4 y[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) y[j] = q < nq ? PN[(c0 + sidx) * 32 + j * 8 + g8] : make_float4(0.f, 0.f, 0.f, 0.f);
+                planes_fma16x2(vh[sidx], vl[sidx], y, m0, m1, a0, a1);
+            }
+        }
+        float m = m0 + m1, a = a0 + a1;
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
+        const float s2 = __fdiv_rn(__ldg(pl.scale + r), 254.0f);
+        const float mt = prefilter_finish(metric, __fmul_rn(s2, m), nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f);
+        const bool certain = fabsf(mt) > __fmul_rn(s2, __fadd_rn(w2, __fmul_rn(rel2, a)));
+        const int side = mt > 0.f ? 1 : 0;
+        if (act && g8 == 0) {
+            if (certain) { jb.flags[p] = (uint8_t)side; if (side == 0) atomicAdd(&sm_cnt[(p - base) / SCAN_UNIT], 1u); }
+            else sm_list2[atomicAdd(&sm_cnt[PLANES_CHUNK + 1], 1u)] = p;
+        }
+    }
+    __syncthreads();
+    // ---- stage 3: the rows left, exactly: one 8-lane group per row, scan_unit's arithmetic ----
+    const uint32_t nl = sm_cnt[PLANES_CHUNK + 1];
+    if (stats != nullptr && tid == 0) {
+        atomicAdd(stats, (unsigned long long)(end - base));
+        if (nl) atomicAdd(stats + 1, (unsigned long long)nl);
+        if (n1) atomicAdd(stats + 2, (unsigned long long)n1);
+    }
     const int nch = (int)(d >> 5);
     const float4* N = reinterpret_cast<const float4*>(sm_normal);
     for (uint32_t it = 0; it * 32u < nl; ++it) {
         const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
         const bool act = idx < nl;
-        const uint32_t p = act ? sm_list[idx] : base;
+        const uint32_t p = act ? sm_list2[idx] : base;
         const uint32_t r = jb.rows ? __ldcg(jb.rows + p) : p;
         const float4* A = reinterpret_cast<const float4*>(items + (size_t)r * ld);
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -268,6 +409,20 @@ __device__ __forceinline__ void scan_claim_shadow(const Job& jb, uint32_t u0, ui
     }
     __syncthreads();
     if (tid < (int)(u1 - u0)) jb.unit_left[u0 + tid] = sm_cnt[tid];
+}
+
+// The bound factors of a job's normal from the per-warp partial sums of |n_i| (f64, eight warps): {w1, w2}, rounded up.
+__device__ __forceinline__ float2 planes_job_factors(const double* sm_l1, uint32_t d) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += sm_l1[w];
+    s *= 1.0 + 0x1p-30;    // the f64 sum's own rounding (< 8192 * 2^-53)
+    return make_float2(__double2float_ru(s * (double)planes_k1(d)), __double2float_ru(s * (double)planes_w2(d)));
+}
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
 }
 
 // Stable partition of one PART_UNIT block of ids. left_before = number of Left flags in all
@@ -374,25 +529,26 @@ work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ i
     }
 }
 
-// work_kernel for contexts that hold the bf16 shadow of the items: scan jobs of more than min_units units are cut into items of
-// SHADOW_CHUNK units and go through scan_claim_shadow; everything else is work_kernel's. Shared memory: two normals (plain and in
-// the shadow rows' lane order) + the prefix table.
+// work_kernel for contexts that hold the 8-bit planes of the items: scan jobs of more than min_units units are cut into items of
+// PLANES_CHUNK units and go through scan_claim_planes; everything else is work_kernel's. Shared memory: the normal, the normal in
+// the planes' lane order (planes_perm_floats(ld) floats) and the prefix table.
 __global__ void __launch_bounds__(WORK_THREADS, 2)
-work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const uint16_t* __restrict__ shadow, const float* __restrict__ ih0,
+work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const PlaneRows planes, const float* __restrict__ ih0,
                    uint32_t d, uint32_t ld, int metric, uint32_t min_units, unsigned long long* stats) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sm_normal = reinterpret_cast<float*>(smem_raw);
     float* sm_perm = sm_normal + ld;
-    uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_perm + ld);
+    uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_perm + planes_perm_floats(ld));
     __shared__ uint32_t sm_count;
     __shared__ uint32_t sm_w[16];
-    __shared__ uint32_t sm_list[SCAN_UNIT * SHADOW_CHUNK];
-    __shared__ uint32_t sm_cnt[SHADOW_CHUNK + 1];
+    __shared__ uint32_t sm_list[SCAN_UNIT * PLANES_CHUNK], sm_list2[SCAN_UNIT * PLANES_CHUNK];
+    __shared__ uint32_t sm_cnt[PLANES_CHUNK + 2];
+    __shared__ double sm_l1[WORK_THREADS / 32];
     auto via_shadow = [&](const Job& jb) { return jb.kind == JOB_SCAN && jb.margins == nullptr && (jb.len + SCAN_UNIT - 1) / SCAN_UNIT > min_units; };
     for (int j = threadIdx.x; j < njobs; j += blockDim.x) {
         const Job jb = jobs[j];
         const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
-        sm_prefix[j] = jb.kind == JOB_SCAN ? (via_shadow(jb) ? (units + SHADOW_CHUNK - 1) / SHADOW_CHUNK : units) : (jb.kind == JOB_PARTITION ? (jb.len + PART_UNIT - 1) / PART_UNIT : 0u);
+        sm_prefix[j] = jb.kind == JOB_SCAN ? (via_shadow(jb) ? (units + PLANES_CHUNK - 1) / PLANES_CHUNK : units) : (jb.kind == JOB_PARTITION ? (jb.len + PART_UNIT - 1) / PART_UNIT : 0u);
     }
     __syncthreads();
     if (threadIdx.x < 32) {
@@ -410,6 +566,7 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
     const uint32_t total = sm_prefix[njobs];
     int loaded_job = -1;
     float nh0 = 0.f;
+    float2 wf = make_float2(0.f, 0.f);
     for (uint32_t u = blockIdx.x; u < total; u += gridDim.x) {
         int lo = 0, hi = njobs;  // last j with prefix[j] <= u
         while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (sm_prefix[mid] <= u) lo = mid; else hi = mid; }
@@ -419,19 +576,24 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
         if (jb.kind == JOB_SCAN) {
             if (loaded_job != j) {
                 __syncthreads();
+                double l1 = 0.0;
                 for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) {
                     const float v = jb.normal[NORMAL_HDR + i];
                     sm_normal[i] = v;
-                    const uint32_t q = i >> 3, w = i & 7u;
-                    sm_perm[(((q >> 3) * 16u + (w >> 2) * 8u + (q & 7u)) << 2) + (w & 3u)] = v;
+                    sm_perm[planes_perm_index(i)] = v;
+                    l1 += (double)fabsf(v);
                 }
+                l1 = warp_sum_f64(l1);
+                if ((threadIdx.x & 31) == 0) sm_l1[threadIdx.x >> 5] = l1;
                 nh0 = jb.normal[0];
                 loaded_job = j;
                 __syncthreads();
+                wf = planes_job_factors(sm_l1, d);
             }
             if (via_shadow(jb)) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
-                scan_claim_shadow(jb, item * SHADOW_CHUNK, min(units, (item + 1u) * SHADOW_CHUNK), items, shadow, ih0, d, ld, metric, sm_normal, sm_perm, nh0, sm_list, sm_cnt, stats);
+                scan_claim_planes(jb, item * PLANES_CHUNK, min(units, (item + 1u) * PLANES_CHUNK), items, planes, ih0, d, ld, metric, sm_normal, sm_perm, nh0, wf.x, wf.y,
+                                  sm_list, sm_list2, sm_cnt, stats);
             } else scan_unit<true>(jb, item, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
         } else {
             partition_block(jb.rows, jb.flags, jb.dst, item * PART_UNIT, jb.len, jb.unit_left[item * (PART_UNIT / SCAN_UNIT)], jb.total_left, sm_w);

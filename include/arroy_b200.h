@@ -202,11 +202,20 @@ int32_t arroy_b200_build_trees_emit_mapped(arroy_ctx* ctx, const uint32_t* root_
  * ARROY_B200_PROFILE=1), stats[6] = tree nodes emitted, stats[7] = create_split calls whose
  * speculative two_means was redone sequentially (a mis-predicted branch; results are identical either way). */
 int32_t arroy_b200_build_stats(arroy_ctx* ctx, double stats[8]);
-/* Of the rows counted in stats[0], how many went through side()'s bf16 pre-filter (out[0]: the shadow copy of the items, half the
- * bytes per row) and how many of those could not be decided by its error bound and were scored from the f32 row (out[1]). The
+/* Of the rows counted in stats[0], how many went through side()'s 8-bit pre-filter (out[0]: the two-plane encoding of the items,
+ * one or two bytes per element) and how many of those could not be decided by its error bounds and were scored from the f32
+ * row (out[1]). The
  * other rows took the plain f32 scan. out[2]: rows of stats[0] that were covered by the fused root pass (trees x items), which
  * read out[3] rows from the item matrix for all of them. Flags are identical either way. */
 int32_t arroy_b200_build_shadow_stats(arroy_ctx* ctx, uint64_t out[4]);
+/* The same accounting with the stages of the pre-filter apart: out[0] = rows that went through it (its first stage reads the
+ * hi plane, one byte per element), out[1] = of them, rows its first stage could not decide (second stage: both planes),
+ * out[2] = of them, rows the second stage could not decide either (scored from the f32 row), out[3], out[4] = out[2], out[3] of
+ * arroy_b200_build_shadow_stats. */
+int32_t arroy_b200_build_prefilter_stats(arroy_ctx* ctx, uint64_t out[5]);
+/* The pre-filter's encoding of the staged items (built here if no build has built it since staging): hi and lo receive
+ * n x ld int8 each (ld = dim rounded up to 32, padding zero), scale n floats; see kernels.cuh planes_encode_kernel. */
+int32_t arroy_b200_prefilter_planes(arroy_ctx* ctx, int8_t* hi, int8_t* lo, float* scale);
 
 /* ---- re-rank: replaces the loop of src/reader.rs:381-399 ------------------------------- */
 
