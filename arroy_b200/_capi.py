@@ -50,6 +50,8 @@ SIGNATURES = [
     ("arroy_b200_rerank_shared", C.c_int32, [C.c_void_p, C.c_uint32, _f32p, _f32p, _u32p, C.c_uint64, C.c_uint32, _u32p, _f32p, _u32p]),
     ("arroy_b200_load_forest", C.c_int32, [C.c_void_p, C.c_uint32, _u8p, _u32p, _u32p, _u32p, _f32p, _u32p, _u32p, C.c_uint32, _f32p, C.c_uint64, _u32p, C.c_uint32, _u32p]),
     ("arroy_b200_search_batch", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, _f32p, C.c_uint64, C.c_uint64, _u32p, _f32p, _u32p, C.POINTER(C.c_int32)]),
+    ("arroy_b200_search_batch_filtered", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, _f32p, C.c_uint64, C.c_uint64, _u32p, _u32p, _f32p, _u32p, C.POINTER(C.c_int32)]),
+    ("arroy_b200_search_stats", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_synth_device", C.c_int32, [C.c_void_p, _u8p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_float, C.c_void_p]),
     ("arroy_b200_time_scan", C.c_int32, [C.c_void_p, _f32p, C.c_float, C.c_float, _u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, _f32p, _u64p]),
     ("arroy_b200_arena_new", C.c_void_p, []),
@@ -120,6 +122,13 @@ def _fp(a):
 
 def _up(a):
     return a.ctypes.data_as(_u32p) if a is not None else None
+
+
+def row_bitmap(rows, n):
+    """The filter arroy_b200_search_batch_filtered takes: ceil(n / 32) uint32 words, bit r set for every r in rows (< n)."""
+    bits = np.zeros(((n + 31) // 32) * 32, dtype=bool)
+    bits[np.asarray(rows, dtype=np.int64)] = True
+    return np.packbits(bits, bitorder="little").view("<u4").astype(np.uint32)
 
 
 def bq_quantize(vector):
@@ -388,6 +397,17 @@ class Context:
                                                  normals.shape[0] if normals.ndim == 2 else 0, _fp(normals), desc_rows.size, _up(desc_rows), roots.size, _up(roots)))
 
     def search_batch(self, count, query_rows=None, queries=None, qhdr0=None, search_k=0):
+        return self._search(count, query_rows, queries, qhdr0, search_k, None)
+
+    def search_batch_filtered(self, count, filter_bits, query_rows=None, queries=None, qhdr0=None, search_k=0):
+        """search_batch with one row filter for every query: filter_bits = ceil(n / 32) uint32 words, bit r = row r passes
+        (row_bitmap builds it from row indices)."""
+        bits = np.ascontiguousarray(filter_bits, dtype=np.uint32)
+        if bits.size != (self.n + 31) // 32:
+            raise ValueError("filter_bits must hold ceil(n / 32) = %d words" % ((self.n + 31) // 32))
+        return self._search(count, query_rows, queries, qhdr0, search_k, bits)
+
+    def _search(self, count, query_rows, queries, qhdr0, search_k, bits):
         if query_rows is not None:
             query_rows = np.ascontiguousarray(query_rows, dtype=np.uint32)
             nq = query_rows.size
@@ -399,9 +419,18 @@ class Context:
         out_dist = np.empty((nq, max(count, 1)), dtype=np.float32)
         out_len = np.zeros(nq, dtype=np.uint32)
         status = np.zeros(nq, dtype=np.int32)
-        self._ck(self.lib.arroy_b200_search_batch(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, _up(out_rows), _fp(out_dist), _up(out_len),
-                                                  status.ctypes.data_as(C.POINTER(C.c_int32))))
+        st = status.ctypes.data_as(C.POINTER(C.c_int32))
+        if bits is None:
+            self._ck(self.lib.arroy_b200_search_batch(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, _up(out_rows), _fp(out_dist), _up(out_len), st))
+        else:
+            self._ck(self.lib.arroy_b200_search_batch_filtered(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, _up(bits), _up(out_rows), _fp(out_dist),
+                                                               _up(out_len), st))
         return out_rows, out_dist, out_len, status
+
+    def search_stats(self):
+        out = (C.c_uint64 * 4)()
+        self._ck(self.lib.arroy_b200_search_stats(self.h, out))
+        return {"filtered_queries": int(out[0]), "shortcut_queries": int(out[1]), "failed_queries": int(out[2]), "nodes_popped": int(out[3])}
 
     # -- helpers ---------------------------------------------------------------------------------
     def synth_device(self, seed, dim, row0, rows, centre, device_ptr):

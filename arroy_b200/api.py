@@ -51,6 +51,8 @@ HOST_SIGNATURES = [
     ("arroy_reader_nns_by_item", C.c_int32, [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, C.c_int64, _u32p, _f32p, _u64p, C.POINTER(C.c_int32)]),
     ("arroy_reader_nns_by_vector", C.c_int32, [C.c_void_p, _f32p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, C.c_int64, _u32p, _f32p, _u64p]),
     ("arroy_reader_nns_batch_by_item", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _f32p, _u32p, C.POINTER(C.c_double)]),
+    ("arroy_reader_nns_batch", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, C.c_int64, _u32p, _f32p, _u32p,
+                                           C.POINTER(C.c_double)]),
 ]
 
 _BOUND = False
@@ -428,13 +430,26 @@ class Reader:
     def nns(self, count):
         return QueryBuilder(self, count)
 
-    def nns_batch_by_item(self, items, count, search_k=None, oversampling=None):
+    def nns_batch_by_item(self, items, count, search_k=None, oversampling=None, candidates=None):
+        """One nns(count).search_k(..).oversampling(..).candidates(..).by_item(it) per item, in one call; candidates (optional)
+        is shared by every query. Returns (ids nq x count, distances nq x count, lengths nq, timings)."""
         items = np.ascontiguousarray(items, dtype=np.uint32)
-        nq = items.size
+        return self._nns_batch(items.size, items.ctypes.data_as(_u32p), None, count, search_k, oversampling, candidates, items)
+
+    def nns_batch_by_vector(self, vectors, count, search_k=None, oversampling=None, candidates=None):
+        """nns_batch_by_item for query vectors (nq x dimensions), as QueryBuilder::by_vector."""
+        vectors = np.ascontiguousarray(vectors, dtype=np.float32)
+        if vectors.ndim != 2 or vectors.shape[1] != self.dimensions():
+            raise ArroyError(100, "Invalid vector dimensions. Got %s but expected %d" % (vectors.shape[1:] or vectors.shape, self.dimensions()))
+        return self._nns_batch(vectors.shape[0], None, vectors.ctypes.data_as(_f32p), count, search_k, oversampling, candidates, vectors)
+
+    def _nns_batch(self, nq, items_p, vectors_p, count, search_k, oversampling, candidates, _keep):
         out_ids = np.zeros((nq, max(count, 1)), dtype=np.uint32)
         out_dist = np.zeros((nq, max(count, 1)), dtype=np.float32)
         out_len = np.zeros(nq, dtype=np.uint32)
         ms = (C.c_double * 2)()
-        _ck(_lib().arroy_reader_nns_batch_by_item(self.h, nq, items.ctypes.data_as(_u32p), count, search_k or 0, oversampling or 0,
-                                                  out_ids.ctypes.data_as(_u32p), out_dist.ctypes.data_as(_f32p), out_len.ctypes.data_as(_u32p), ms))
+        cand = None if candidates is None else np.ascontiguousarray(sorted(candidates), dtype=np.uint32)
+        _ck(_lib().arroy_reader_nns_batch(self.h, nq, items_p, vectors_p, count, min(search_k or 0, 2**64 - 1), oversampling or 0,
+                                          None if cand is None else cand.ctypes.data_as(_u32p), -1 if cand is None else cand.size,
+                                          out_ids.ctypes.data_as(_u32p), out_dist.ctypes.data_as(_f32p), out_len.ctypes.data_as(_u32p), ms))
         return out_ids, out_dist, out_len, {"tree_walk_ms": ms[0], "rerank_ms": ms[1]}

@@ -133,6 +133,14 @@ struct arroy_ctx {
     uint64_t stage_epoch = 0, forest_epoch = 0;  // bumped by every (re)staging / forest upload: owners compare them (arroy_b200_epochs)
     DevBuf w_heaps, w_cand, w_cand2, w_count, w_bitmap, w_status, w_beg, w_end, w_qrows, w_tmp, w_pre;
     uint32_t f_n_normals = 0;
+    // what filtered searches need from the forest (load_forest): parent per node (tree-shaped forests), nodes reachable from the
+    // roots, nodes pinned live (a missing node and its ancestors), rows that some reachable leaf holds
+    DevBuf f_parent, f_reach, f_pin, f_inleaf;
+    bool f_tree = false;       // every reachable node has one parent: pruning by the live flags is exact
+    bool f_complete = false;   // no reachable node is missing: the small-filter shortcut is exact
+    // per-call scratch of filtered searches (arroy_b200_search_batch_filtered)
+    DevBuf w_fbits, w_fcount, w_live, w_ftotal, w_pops, w_spill, w_scount, w_soff;
+    uint64_t filter_stats[4] = {0, 0, 0, 0};   // arroy_b200_search_stats
     // results of the last build_trees_begin, waiting for build_trees_emit
     std::vector<std::vector<struct BuiltTreeView>> pending_waves;
     std::vector<uint32_t> pending_wave_t0;
@@ -1790,13 +1798,50 @@ int32_t arroy_b200_load_forest(arroy_ctx* c, uint32_t n_nodes, const uint8_t* ki
         c->f_rec.ensure(std::max<size_t>(32, 32ull * n_nodes)); c->f_nofn.ensure(std::max<size_t>(16, 4ull * n_normals));
         if (n_nodes) { forest_pack_kernel<<<(n_nodes + 255) / 256, 256, 0, c->stream>>>(F, c->f_rec.as<uint4>(), c->f_nofn.as<uint32_t>()); CK(cudaGetLastError()); CK(cudaStreamSynchronize(c->stream)); }
         F.rec = c->f_rec.as<uint4>(); F.node_of_normal = c->f_nofn.as<uint32_t>();
+        // One depth-first pass from the roots for filtered searches: parents, reachability, and the pins that keep every
+        // ancestor of a missing node live, so that a pruned walk still pops it exactly when the reference would.
+        std::vector<uint32_t> parent(n_nodes, NO_PARENT), stack(roots, roots + n_roots);
+        std::vector<uint8_t> reach(n_nodes, 0), pin(n_nodes, 0);
+        bool tree = true, complete = true;
+        while (!stack.empty()) {
+            const uint32_t x = stack.back();
+            stack.pop_back();
+            if (reach[x]) { tree = false; continue; }
+            reach[x] = 1;
+            if (kind[x] == 0) { complete = false; for (uint32_t y = x; y != NO_PARENT && !pin[y]; y = parent[y]) pin[y] = 1; }
+            else if (kind[x] == 2)
+                for (uint32_t ch : {left[x], right[x]}) {
+                    if (reach[ch] || parent[ch] != NO_PARENT) tree = false;
+                    else parent[ch] = x;
+                    stack.push_back(ch);
+                }
+        }
+        const uint32_t words = (uint32_t)((c->n + 31) / 32);
+        up(c->f_parent, parent.data(), 4ull * n_nodes); up(c->f_reach, reach.data(), n_nodes); up(c->f_pin, pin.data(), n_nodes);
+        c->f_inleaf.ensure(std::max<size_t>(16, 4ull * words));
+        CK(cudaMemsetAsync(c->f_inleaf.p, 0, 4ull * words, c->stream));
+        if (n_nodes) { forest_inleaf_kernel<<<(uint32_t)(((uint64_t)n_nodes * 32 + 255) / 256), 256, 0, c->stream>>>(F, c->f_reach.as<uint8_t>(), c->f_inleaf.as<uint32_t>()); CK(cudaGetLastError()); }
+        CK(cudaStreamSynchronize(c->stream));
+        c->f_tree = tree; c->f_complete = complete;
         c->forest = F; c->forest_max_desc = max_desc; c->forest_n = c->n; c->forest_epoch += 1; c->forest_loaded = true;
     });
 }
 
-int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
-                                uint64_t count, uint64_t search_k, uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status) {
-    return guarded(c, [&] {
+extern "C++" {
+namespace {
+
+template <bool FILTER> void configure_walk_kernels() {
+    static bool configured = false;
+    if (configured) return;
+    CK(cudaFuncSetAttribute(walk_kernel<FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)WALK_WARPS * WALK_SHEAP * 8)));
+    CK(cudaFuncSetAttribute(walk1_kernel<FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk1_smem<FILTER>(W1_MAX_LD)));
+    configured = true;
+}
+
+// arroy_b200_search_batch, and with filter_bits != NULL arroy_b200_search_batch_filtered: one row filter for every query
+void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
+                       uint64_t count, uint64_t search_k, const uint32_t* filter_bits, uint32_t* out_rows, float* out_dist, uint32_t* out_len,
+                       int32_t* out_status) {
         require_staged(c); set_device(c);
         if (!c->forest_loaded || c->forest_n != c->n) throw NotStaged("no forest loaded on this context for the staged items (arroy_b200_load_forest)");
         if (nq == 0) return;
@@ -1806,24 +1851,76 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
         if (query_rows) for (uint32_t q = 0; q < nq; ++q) if (query_rows[q] >= c->n) throw ArgError("query row out of range");
         const uint32_t ld = c->ld, k = (uint32_t)count;
         const DevForest& F = c->forest;
+        const bool filtered = filter_bits != nullptr;
         if (search_k == 0) search_k = count * F.n_roots;  // reader.rs:330
-        const uint64_t cand_cap64 = std::min<uint64_t>(c->n, search_k + c->forest_max_desc);
-        const uint64_t heap_cap64 = (uint64_t)F.n_roots + std::min<uint64_t>(F.n_nodes, 2 * std::min<uint64_t>(search_k, c->n) + 1024);
+        // (filtered: saturating, so that search_k near 2^64 still leaves room for every filtered row the shortcut may take)
+        const uint64_t sk_plus = filtered && search_k > UINT64_MAX - c->forest_max_desc ? UINT64_MAX : search_k + c->forest_max_desc;
+        const uint64_t cand_cap64 = std::min<uint64_t>(c->n, sk_plus);
+        // a filtered walk may push every node once (a filter can keep it going through the whole forest)
+        const uint64_t heap_cap64 = (uint64_t)F.n_roots + (filtered ? (uint64_t)F.n_nodes : std::min<uint64_t>(F.n_nodes, 2 * std::min<uint64_t>(search_k, c->n) + 1024));
         if (cand_cap64 > 0x7fffffffull || heap_cap64 > 0x7fffffffull) throw ArgError("search_k too large for the device walk");
         const uint32_t cand_cap = (uint32_t)std::max<uint64_t>(cand_cap64, 1), heap_cap = (uint32_t)heap_cap64;
         const uint32_t bm_words = (uint32_t)((c->n + 31) / 32);
         const size_t walk_smem = (size_t)WALK_WARPS * WALK_SHEAP * 8;
-        { static bool configured = false; if (!configured) { CK(cudaFuncSetAttribute(walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk_smem)); configured = true; } }
+        if (filtered) configure_walk_kernels<true>(); else configure_walk_kernels<false>();
         for (double& x : c->sbreak) x = 0;
         int nte = 0;
         auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
+        // ---- the filter's summary: fcount / live per node and ftotal (search.cuh filter_count_kernel). When ftotal <= search_k
+        //      the reference's walk only ends with an empty queue, so its candidates are every filtered row of a reachable leaf:
+        //      the shortcut takes those without a walk (only where no reachable node is missing and pruning is exact).
+        WalkFilter Fl{};
+        bool shortcut = false;
+        std::vector<int32_t> h_status;
+        std::vector<uint32_t> h_pops;
+        auto filter_tally = [&](uint32_t m, bool walked) {   // after the stream is idle: statistics of m filtered queries
+            if (!filtered) return;
+            h_status.resize(m); h_pops.resize(m);
+            CK(cudaMemcpy(h_status.data(), c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost));
+            if (walked) CK(cudaMemcpy(h_pops.data(), c->w_pops.p, 4ull * m, cudaMemcpyDeviceToHost));
+            for (uint32_t q = 0; q < m; ++q) {
+                if (h_status[q] == 0) { c->filter_stats[0] += 1; c->filter_stats[1] += walked ? 0 : 1; }
+                else c->filter_stats[2] += 1;
+                if (walked) c->filter_stats[3] += h_pops[q];
+            }
+        };
+        if (filtered) {
+            c->w_fbits.ensure(4ull * bm_words); c->w_fcount.ensure(std::max<size_t>(16, 4ull * F.n_nodes)); c->w_live.ensure(std::max<size_t>(16, F.n_nodes));
+            c->w_ftotal.ensure(16); c->w_pops.ensure(4ull * std::max<uint32_t>(nq, 1));
+            CK(cudaMemcpyAsync(c->w_fbits.p, filter_bits, 4ull * bm_words, cudaMemcpyHostToDevice, c->stream));
+            if (c->f_tree) CK(cudaMemcpyAsync(c->w_live.p, c->f_pin.p, F.n_nodes, cudaMemcpyDeviceToDevice, c->stream));
+            else CK(cudaMemsetAsync(c->w_live.p, 1, F.n_nodes, c->stream));
+            CK(cudaMemsetAsync(c->w_ftotal.p, 0, 8, c->stream));
+            if (F.n_nodes) {
+                filter_count_kernel<<<(uint32_t)(((uint64_t)F.n_nodes * 32 + 255) / 256), 256, 0, c->stream>>>(F, c->w_fbits.as<uint32_t>(), c->f_reach.as<uint8_t>(),
+                                                                                                              c->f_tree ? c->f_parent.as<uint32_t>() : nullptr, c->w_fcount.as<uint32_t>(),
+                                                                                                              c->w_live.as<uint8_t>(), c->w_ftotal.as<unsigned long long>());
+                CK(cudaGetLastError());
+                c->n_launches += 1;
+            }
+            unsigned long long ftotal = 0;
+            CK(cudaMemcpyAsync(&ftotal, c->w_ftotal.p, 8, cudaMemcpyDeviceToHost, c->stream));
+            CK(cudaStreamSynchronize(c->stream));
+            c->h2d_bytes += 4ull * bm_words;
+            Fl.bits = c->w_fbits.as<uint32_t>(); Fl.fcount = c->w_fcount.as<uint32_t>(); Fl.live = c->w_live.as<uint8_t>(); Fl.pops = c->w_pops.as<uint32_t>();
+            shortcut = c->f_tree && c->f_complete && ftotal <= search_k && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
+            if (shortcut) {   // the rows, ascending: popcounts per word, an exclusive scan, then every query's segment is written
+                c->w_scount.ensure(4ull * bm_words); c->w_soff.ensure(4ull * bm_words);
+                filter_select_count_kernel<<<(bm_words + 255) / 256, 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), bm_words, c->w_scount.as<uint32_t>());
+                CK(cudaGetLastError());
+                size_t tmp_bytes = 0;
+                CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
+                c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
+                CK(cub::DeviceScan::ExclusiveSum(c->w_tmp.p, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
+                c->n_launches += 2;
+            }
+        }
         // ---- a few queries: latency path, one CTA per query (search.cuh walk1_kernel), then the plain distance + top-k kernels on
         //      all SMs. Any query it cannot hold (heap / candidate overflow) sends the call through the general path below.
-        if (nq <= 16 && cand_cap64 <= (uint64_t)W1_CAND && getenv("ARROY_B200_NO_WALK1") == nullptr) {
+        if (!shortcut && nq <= 16 && cand_cap64 <= (uint64_t)W1_CAND && getenv("ARROY_B200_NO_WALK1") == nullptr) {
             const uint32_t m = nq;
-            const size_t w1smem = walk1_smem(ld);
-            { static bool configured = false; if (!configured) { CK(cudaFuncSetAttribute(walk1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(Walk1Shared) + 16 + 4 * 8192))); configured = true; } }
-            if (w1smem <= sizeof(Walk1Shared) + 16 + 4 * 8192) {
+            const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
+            if (ld <= W1_MAX_LD) {
                 c->w_cand2.ensure(4ull * cand_cap * m); c->w_count.ensure(4ull * m); c->w_status.ensure(4ull * m);
                 c->w_beg.ensure(8ull * (m + 1)); c->w_end.ensure(8ull * (m + 1));
                 c->s_keys.ensure(8ull * cand_cap * m); c->s_dists.ensure(4ull * cand_cap * m);
@@ -1863,8 +1960,16 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
                         d_pre = c->w_pre.as<float>();
                     }
                 }
-                walk1_kernel<<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, getenv("ARROY_B200_WALK1_DEBUG") ? 1 : 0, search_k,
-                                                                  c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>());
+                const int w1debug = getenv("ARROY_B200_WALK1_DEBUG") ? 1 : 0;
+                if (filtered) {
+                    Fl.spill_cap = F.n_roots + F.n_nodes;
+                    c->w_spill.ensure(8ull * Fl.spill_cap * m);
+                    Fl.spill = c->w_spill.as<unsigned long long>();
+                    walk1_kernel<true><<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
+                                                                            c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
+                } else
+                    walk1_kernel<false><<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
+                                                                             c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
                 CK(cudaGetLastError());
                 mark1();
                 walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
@@ -1895,6 +2000,7 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
                 for (uint32_t q = 0; q < m; ++q) all_ok = all_ok && h_st[q] == 0;
                 if (all_ok) {
                     if (out_status) for (uint32_t q = 0; q < m; ++q) out_status[q] = 0;
+                    filter_tally(m, true);
                     c->d2h_bytes += 8ull * m * k + 8ull * m;
                     return;
                 }
@@ -1928,10 +2034,23 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
                 CK(cudaGetLastError());
             } else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
             nte = 0; mark();
+            if (shortcut) {
+                filter_select_scatter_kernel<<<dim3((bm_words + 255) / 256, m), 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), c->w_soff.as<uint32_t>(), bm_words,
+                                                                                                    c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>());
+                CK(cudaGetLastError());
+                mark();
+                walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
+                CK(cudaGetLastError());
+            } else {
             CK(cudaMemsetAsync(c->w_bitmap.p, 0, 4ull * bm_words * m, c->stream));
-            walk_kernel<<<(m + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(),
-                                                                                       search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
-                                                                                       c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>());
+            if (filtered)
+                walk_kernel<true><<<(m + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(),
+                                                                                             search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
+                                                                                             c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
+            else
+                walk_kernel<false><<<(m + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(),
+                                                                                              search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
+                                                                                              c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
             CK(cudaGetLastError());
             mark();
             walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
@@ -1943,6 +2062,7 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
             c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
             CK(cub::DeviceSegmentedSort::SortKeys(c->w_tmp.p, tmp_bytes, c->w_cand.as<uint32_t>(), c->w_cand2.as<uint32_t>(), (int64_t)cand_cap * m, (int64_t)m,
                                                   c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->stream));
+            }
             mark();
             bool fused = frerank_enabled(c, k);
             if (fused) {   // one fused kernel per query: bf16 pre-filter + exact re-score + top-k (frerank.cuh)
@@ -1970,8 +2090,32 @@ int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query
             if (out_status) CK(cudaMemcpyAsync(out_status + q0, c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
             CK(cudaStreamSynchronize(c->stream));
             for (int i = 0; i + 1 < nte; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); c->sbreak[i] += ms; }
+            filter_tally(m, !shortcut);
             c->d2h_bytes += 8ull * m * k + 8ull * m;
         }
+}
+
+}  // namespace
+}  // extern "C++"
+
+int32_t arroy_b200_search_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
+                                uint64_t count, uint64_t search_k, uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status) {
+    return guarded(c, [&] { search_batch_body(c, nq, query_rows, queries, qhdr0, count, search_k, nullptr, out_rows, out_dist, out_len, out_status); });
+}
+
+int32_t arroy_b200_search_batch_filtered(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
+                                         uint64_t count, uint64_t search_k, const uint32_t* filter_bits, uint32_t* out_rows, float* out_dist,
+                                         uint32_t* out_len, int32_t* out_status) {
+    return guarded(c, [&] {
+        if (!filter_bits) throw ArgError("null filter");
+        search_batch_body(c, nq, query_rows, queries, qhdr0, count, search_k, filter_bits, out_rows, out_dist, out_len, out_status);
+    });
+}
+
+int32_t arroy_b200_search_stats(arroy_ctx* c, uint64_t out[4]) {
+    return guarded(c, [&] {
+        if (!out) throw ArgError("null argument");
+        for (int i = 0; i < 4; ++i) out[i] = c->filter_stats[i];
     });
 }
 

@@ -1183,30 +1183,77 @@ inline void tree_walk(const arroy_reader* r, const float* qv, float qh0, uint64_
     }
 }
 
+// QueryBuilder::candidates as the device takes it: bit r set when row r (= r->items[r]) is a candidate. Ids that are not in
+// the index drop out, as `descendants & candidates` drops them in the reference. `sorted_ids` ascending.
+inline std::vector<uint32_t> candidate_row_bits(const arroy_reader* r, const std::vector<uint32_t>& sorted_ids) {
+    const size_t n = r->items.size();
+    std::vector<uint32_t> bits((n + 31) / 32, 0u);
+    if (n && r->items.front() == 0 && r->items.back() == n - 1) {   // ids 0..n-1: row = id
+        for (uint32_t id : sorted_ids) { if (id >= n) break; bits[id >> 5] |= 1u << (id & 31); }
+        return bits;
+    }
+    size_t j = 0;
+    for (uint32_t id : sorted_ids) {
+        while (j < r->items.size() && r->items[j] < id) ++j;
+        if (j == r->items.size()) break;
+        if (r->items[j] == id) bits[j >> 5] |= 1u << (j & 31);
+    }
+    return bits;
+}
+
+// Where the host walk of one filtered query beats the device on an H100 (tools/bench_filtered_search.py on C2, DESIGN §7.1):
+//   - the filter holds at least 1/20 of the items: few leaves reach search_k, so the host walk is short and the device's fixed
+//     cost per filtered call (the bitmap upload and the summary pass over every leaf) dominates;
+//   - the filter is a dense row range (at least half of the rows between its first and last row pass) of at least 1/1000 of the
+//     items and at least 1000 rows: the host walk's per-row binary searches stay in cache and its walk is as short as for a
+//     random filter of that size.
+inline bool filter_prefers_host_walk(const std::vector<uint32_t>& bits, uint64_t n) {
+    uint64_t in_filter = 0, first = UINT64_MAX, last = 0;
+    for (size_t w = 0; w < bits.size(); ++w) {
+        if (!bits[w]) continue;
+        in_filter += __builtin_popcount(bits[w]);
+        if (first == UINT64_MAX) first = 32 * w + __builtin_ctz(bits[w]);
+        last = 32 * w + 31 - __builtin_clz(bits[w]);
+    }
+    if (in_filter * 20 >= n) return true;
+    return in_filter >= 1000 && in_filter * 1000 >= n && in_filter * 2 >= last - first + 1;
+}
+
+inline uint64_t effective_search_k(const arroy_reader* r, uint64_t count, uint64_t search_k, uint64_t oversampling) {
+    unsigned __int128 sk = search_k ? (unsigned __int128)search_k : (unsigned __int128)count * r->roots.size();   // reader.rs:330-335
+    sk *= oversampling ? oversampling : 1;
+    return sk > (unsigned __int128)UINT64_MAX ? UINT64_MAX : std::max<uint64_t>((uint64_t)sk, 1);
+}
+
 inline void nns_by_leaf(arroy_reader* r, const float* qv, float qh0, float qh1, uint64_t count, uint64_t search_k, uint64_t oversampling,
                         const uint32_t* cand, int64_t n_cand, uint32_t* out_ids, float* out_dist, uint64_t* out_len, int64_t qrow = -1) {
     *out_len = 0;
+    std::vector<uint32_t> cv, rows;
+    if (n_cand >= 0) { cv.assign(cand, cand + n_cand); std::sort(cv.begin(), cv.end()); }
     // One query, whole search on the device (the forest stays resident after the first call): the priority-queue walk, the
-    // candidate sort and the re-rank are one arroy_b200_search_batch call with nq = 1 — no host walk over 50 trees, no candidate
-    // list crossing PCIe. Queries with a `candidates` filter or count > 2048 keep the host walk below.
-    if (n_cand < 0 && count > 0 && count <= 2048 && !r->items.empty() && r->ctx && getenv("ARROY_B200_HOST_WALK") == nullptr) {
+    // candidate sort and the re-rank are one arroy_b200_search_batch(_filtered) call with nq = 1 — no host walk over 50 trees, no
+    // candidate list crossing PCIe. count > 2048, a device walk that gives up (nonzero status), or a filter whose host walk is
+    // cheaper (filter_prefers_host_walk) keeps the host walk below.
+    std::vector<uint32_t> fbits;
+    const bool device = count > 0 && count <= 2048 && !r->items.empty() && r->ctx && getenv("ARROY_B200_HOST_WALK") == nullptr;
+    if (device && n_cand >= 0) fbits = candidate_row_bits(r, cv);
+    if (device && (n_cand < 0 || !filter_prefers_host_walk(fbits, r->items.size()))) {
         ensure_forest(r);
-        unsigned __int128 sk = search_k ? (unsigned __int128)search_k : (unsigned __int128)count * r->roots.size();   // reader.rs:330-335
-        sk *= oversampling ? oversampling : 1;
-        const uint64_t eff = sk > (unsigned __int128)UINT64_MAX ? UINT64_MAX : std::max<uint64_t>((uint64_t)sk, 1);
+        const uint64_t eff = effective_search_k(r, count, search_k, oversampling);
         std::vector<uint32_t> orow(count);
         uint32_t olen = 0, qr = (uint32_t)qrow;
         int32_t status = 0;
-        dev_ck(r->ctx, arroy_b200_search_batch(r->ctx, 1, qrow >= 0 ? &qr : nullptr, qrow >= 0 ? nullptr : qv, qrow >= 0 ? nullptr : &qh0, count, eff,
-                                               orow.data(), out_dist, &olen, &status));
+        const uint32_t* qrp = qrow >= 0 ? &qr : nullptr;
+        const float* qvp = qrow >= 0 ? nullptr : qv;
+        const float* qhp = qrow >= 0 ? nullptr : &qh0;
+        if (n_cand >= 0) dev_ck(r->ctx, arroy_b200_search_batch_filtered(r->ctx, 1, qrp, qvp, qhp, count, eff, fbits.data(), orow.data(), out_dist, &olen, &status));
+        else dev_ck(r->ctx, arroy_b200_search_batch(r->ctx, 1, qrp, qvp, qhp, count, eff, orow.data(), out_dist, &olen, &status));
         if (status == 0) {
             for (uint32_t i = 0; i < olen; ++i) out_ids[i] = r->items[orow[i]];
             *out_len = olen;
             return;
         }
     }
-    std::vector<uint32_t> cv, rows;
-    if (n_cand >= 0) { cv.assign(cand, cand + n_cand); std::sort(cv.begin(), cv.end()); }
     tree_walk(r, qv, qh0, count, search_k, oversampling, n_cand >= 0 ? &cv : nullptr, rows);
     *out_len = 0;
     if (rows.empty() || count == 0) return;
@@ -1424,19 +1471,31 @@ int32_t arroy_reader_nns_by_vector(arroy_reader* r, const float* vector, uint32_
         nns_by_leaf(r, vector, h0, h1, count, search_k, oversampling, cand, n_cand, out_ids, out_dist, out_len);
     });
 }
-int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint32_t* items, uint64_t count, uint64_t search_k, uint64_t oversampling,
-                                       uint32_t* out_ids, float* out_dist, uint32_t* out_len, double* out_ms) {
+int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count, uint64_t search_k,
+                               uint64_t oversampling, const uint32_t* cand, int64_t n_cand, uint32_t* out_ids, float* out_dist, uint32_t* out_len,
+                               double* out_ms) {
     return hguard([&] {
         const uint32_t d = r->dims;
         const int hf = header_floats(r->metric);
+        if ((items == nullptr) == (vectors == nullptr)) throw HostError(ARROY_ERR_PANIC, "exactly one of items / vectors must be given");
         check_fresh(r);
         std::vector<float> q, qh0, qh1;
         std::vector<std::vector<uint32_t>> rows;
-        for (uint32_t i = 0; i < nq; ++i)
-            if (row_of(r, items[i]) < 0) throw HostError(ARROY_ERR_MISSING_KEY, "Internal error: Item(" + std::to_string(items[i]) + ") is missing in index `" + std::to_string(r->index) + "`");
-        // the query vectors are only needed by the host walk (the device path addresses the staged rows)
+        std::vector<uint32_t> cv, fbits;
+        if (n_cand >= 0) { cv.assign(cand, cand + n_cand); std::sort(cv.begin(), cv.end()); }
+        if (items)
+            for (uint32_t i = 0; i < nq; ++i)
+                if (row_of(r, items[i]) < 0) throw HostError(ARROY_ERR_MISSING_KEY, "Internal error: Item(" + std::to_string(items[i]) + ") is missing in index `" + std::to_string(r->index) + "`");
+        // by_item: the query vectors are only needed by the host walk (the device path addresses the staged rows);
+        // by_vector: their headers come from new_header, as in nns_by_vector (reader.rs:72-73)
         auto load_queries = [&] {
-            q.resize((size_t)nq * d); qh0.resize(nq); qh1.resize(nq); rows.resize(nq);
+            qh0.resize(nq); qh1.resize(nq); rows.resize(nq);
+            if (vectors) {
+                q.assign(vectors, vectors + (size_t)nq * d);
+                for (uint32_t i = 0; i < nq; ++i) new_header(r->metric, vectors + (size_t)i * d, d, qh0[i], qh1[i]);
+                return;
+            }
+            q.resize((size_t)nq * d);
             std::lock_guard<std::mutex> lk(r->env->mu);
             for (uint32_t i = 0; i < nq; ++i) {
                 int64_t row = row_of(r, items[i]);
@@ -1445,6 +1504,7 @@ int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint3
                 qh0[i] = r->hdr0[row]; qh1[i] = r->hdr1[row];
             }
         };
+        if (vectors) load_queries();
         const uint32_t k_dev = (uint32_t)count;
         std::vector<int32_t> status(nq, 0);
         std::vector<uint32_t> orow_dev;
@@ -1453,14 +1513,18 @@ int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint3
             // whole search on the device: walk + dedup/sort + re-rank in one call
             ensure_forest(r);
             auto t0d = clk::now();
-            std::vector<uint32_t> qrows(nq);
-            for (uint32_t i = 0; i < nq; ++i) qrows[i] = (uint32_t)row_of(r, items[i]);
+            std::vector<uint32_t> qrows;
+            if (items) { qrows.resize(nq); for (uint32_t i = 0; i < nq; ++i) qrows[i] = (uint32_t)row_of(r, items[i]); }
             orow_dev.resize((size_t)nq * std::max<uint32_t>(k_dev, 1));
-            unsigned __int128 sk = search_k ? (unsigned __int128)search_k : (unsigned __int128)count * r->roots.size();   // reader.rs:330-335
-            sk *= oversampling ? oversampling : 1;
-            const uint64_t eff_search_k = sk > (unsigned __int128)UINT64_MAX ? UINT64_MAX : std::max<uint64_t>((uint64_t)sk, 1);
-            dev_ck(r->ctx, arroy_b200_search_batch(r->ctx, nq, qrows.data(), nullptr, nullptr, count, eff_search_k,
-                                                   orow_dev.data(), out_dist, out_len, status.data()));
+            const uint64_t eff_search_k = effective_search_k(r, count, search_k, oversampling);
+            const uint32_t* qrp = items ? qrows.data() : nullptr;
+            const float* qvp = items ? nullptr : q.data();
+            const float* qhp = items ? nullptr : qh0.data();
+            if (n_cand >= 0) {
+                fbits = candidate_row_bits(r, cv);
+                dev_ck(r->ctx, arroy_b200_search_batch_filtered(r->ctx, nq, qrp, qvp, qhp, count, eff_search_k, fbits.data(), orow_dev.data(), out_dist, out_len, status.data()));
+            } else
+                dev_ck(r->ctx, arroy_b200_search_batch(r->ctx, nq, qrp, qvp, qhp, count, eff_search_k, orow_dev.data(), out_dist, out_len, status.data()));
             bool all_ok = true;
             for (uint32_t i = 0; i < nq; ++i) {
                 if (status[i] != 0) { all_ok = false; continue; }
@@ -1470,13 +1534,13 @@ int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint3
             if (all_ok) return;
         }
         // host walk (all queries, or only the ones the device walk gave up on)
-        load_queries();
+        if (items) load_queries();
         auto t0 = clk::now();
         std::atomic<uint32_t> next{0};
         std::string err; std::mutex emu;
         const bool only_failed = !host_walk;
         auto worker = [&] {
-            try { for (;;) { uint32_t i = next.fetch_add(1); if (i >= nq) return; if (only_failed && status[i] == 0) continue; tree_walk(r, &q[(size_t)i * d], qh0[i], count, search_k, oversampling, nullptr, rows[i]); } }
+            try { for (;;) { uint32_t i = next.fetch_add(1); if (i >= nq) return; if (only_failed && status[i] == 0) continue; tree_walk(r, &q[(size_t)i * d], qh0[i], count, search_k, oversampling, n_cand >= 0 ? &cv : nullptr, rows[i]); } }
             catch (const std::exception& e) { std::lock_guard<std::mutex> lk(emu); err = e.what(); }
         };
         unsigned nt = std::max(1u, std::min<unsigned>(nq, std::thread::hardware_concurrency()));
@@ -1516,6 +1580,10 @@ int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint3
             }
         if (out_ms) out_ms[1] += ms_since(t0);
     });
+}
+int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint32_t* items, uint64_t count, uint64_t search_k, uint64_t oversampling,
+                                       uint32_t* out_ids, float* out_dist, uint32_t* out_len, double* out_ms) {
+    return arroy_reader_nns_batch(r, nq, items, nullptr, count, search_k, oversampling, nullptr, -1, out_ids, out_dist, out_len, out_ms);
 }
 
 }  // extern "C"

@@ -86,14 +86,74 @@ __device__ __forceinline__ unsigned long long heap_pop(unsigned long long* h, ui
 
 constexpr int WALK_WARPS = 8;
 constexpr uint32_t WALK_SHEAP = 512;    // heap entries per query kept in shared memory (spills to the global heap beyond)
+constexpr uint32_t NO_PARENT = 0xffffffffu;
+
+// ---- filtered walks (QueryBuilder::candidates, reader.rs:350-357) -----------------------------------------------------
+// One row filter is shared by every query of a call. The reference keeps only `descendants & candidates` of each popped
+// Descendants node and stops once it holds search_k of those (duplicates included), so a walk adds fcount[node] to its stop
+// count and appends only the filtered rows. It also never pushes a child whose live flag is 0: such a subtree holds no filtered
+// row (and no missing node, whose ancestors load_forest pins live), so it adds nothing to the count or the candidates, and
+// since every key is distinct (the node id is its low half) the remaining nodes pop in the reference's order.
+struct WalkFilter {
+    const uint32_t* bits;       // bit r set = row r passes
+    const uint32_t* fcount;     // per Descendants node: |desc(node) & filter|
+    const uint8_t* live;        // per node: its subtree holds a filtered row or a missing node
+    uint32_t* pops;             // per query: nodes popped
+    unsigned long long* spill;  // walk1_kernel: per query, frontier entries past the shared-memory slots (spill_cap each)
+    uint32_t spill_cap;
+};
+
+// fcount for every Descendants node (one warp per node) and ftotal = their sum over the nodes reachable from the roots. With
+// `parent` (a tree-shaped forest), a node with a filtered row flags itself and its ancestors live, stopping at the first one
+// already flagged; without it the caller has set every flag.
+__global__ void filter_count_kernel(DevForest F, const uint32_t* __restrict__ bits, const uint8_t* __restrict__ reach, const uint32_t* __restrict__ parent,
+                                    uint32_t* __restrict__ fcount, volatile uint8_t* live, unsigned long long* __restrict__ ftotal) {
+    const uint32_t node = (uint32_t)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (node >= F.n_nodes || F.kind[node] != 1) return;
+    const uint32_t off = F.desc_off[node], len = F.desc_len[node];
+    uint32_t cnt = 0;
+    for (uint32_t i = lane; i < len; i += 32) { const uint32_t row = F.desc_rows[off + i]; cnt += (bits[row >> 5] >> (row & 31)) & 1u; }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if (lane != 0) return;
+    fcount[node] = cnt;
+    if (cnt == 0) return;
+    if (reach[node]) atomicAdd(ftotal, (unsigned long long)cnt);
+    if (parent) for (uint32_t x = node; x != NO_PARENT && !live[x]; x = parent[x]) live[x] = 1;
+}
+
+// bit r of `inleaf` = row r is a descendant of some reachable Descendants node (once per forest upload)
+__global__ void forest_inleaf_kernel(DevForest F, const uint8_t* __restrict__ reach, uint32_t* __restrict__ inleaf) {
+    const uint32_t node = (uint32_t)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (node >= F.n_nodes || F.kind[node] != 1 || !reach[node]) return;
+    const uint32_t off = F.desc_off[node], len = F.desc_len[node];
+    for (uint32_t i = lane; i < len; i += 32) { const uint32_t row = F.desc_rows[off + i]; atomicOr(&inleaf[row >> 5], 1u << (row & 31)); }
+}
+
+// The small-filter shortcut: every filtered row of a reachable leaf, ascending, copied to each query's candidate segment.
+__global__ void filter_select_count_kernel(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ inleaf, uint32_t words, uint32_t* __restrict__ counts) {
+    const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+    if (w < words) counts[w] = __popc(bits[w] & inleaf[w]);
+}
+__global__ void filter_select_scatter_kernel(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ inleaf, const uint32_t* __restrict__ offs, uint32_t words,
+                                             uint32_t* __restrict__ cand, uint32_t cand_cap, uint32_t* __restrict__ cand_count, int32_t* __restrict__ status) {
+    const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x, q = blockIdx.y;
+    if (w >= words) return;
+    uint32_t m = bits[w] & inleaf[w], o = offs[w];
+    uint32_t* out = cand + (size_t)q * cand_cap;
+    for (; m; m &= m - 1) out[o++] = w * 32 + (uint32_t)(__ffs((int)m) - 1);
+    if (w == words - 1) { cand_count[q] = o; status[q] = 0; }
+}
 
 // query q: vector = qrows ? items[qrows[q]] : queries[q] (ld floats); qh0 = extra_dim for DotProduct margins
+template <bool FILTER>
 __global__ void __launch_bounds__(WALK_WARPS * 32)
 walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t ld, int metric, uint32_t nq,
             const uint32_t* __restrict__ qrows, const float* __restrict__ queries, const float* __restrict__ qh0,
             unsigned long long search_k, unsigned long long* __restrict__ heaps, uint32_t heap_cap,
             uint32_t* __restrict__ cand, uint32_t cand_cap, uint32_t* __restrict__ cand_count,
-            uint32_t* __restrict__ bitmap, uint32_t bitmap_words, int32_t* __restrict__ status) {
+            uint32_t* __restrict__ bitmap, uint32_t bitmap_words, int32_t* __restrict__ status, WalkFilter Fl) {
     const int lane = threadIdx.x & 31;
     const uint32_t q = blockIdx.x * WALK_WARPS + (threadIdx.x >> 5);
     if (q >= nq) return;
@@ -111,10 +171,10 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
     if (F.n_roots > cap) { heap = gheap; cap = heap_cap; }
     if (lane == 0) {
         const unsigned long long inf_key = (unsigned long long)ordered_key(__uint_as_float(0x7f800000u)) << 32;
-        for (uint32_t r = 0; r < F.n_roots && size < cap; ++r) heap_push(heap, size, inf_key | F.roots[r]);
+        for (uint32_t r = 0; r < F.n_roots && size < cap; ++r) if (!FILTER || Fl.live[F.roots[r]]) heap_push(heap, size, inf_key | F.roots[r]);
     }
     unsigned long long total = 0;   // nns.len() of the reference (duplicates included)
-    uint32_t unique = 0;
+    uint32_t unique = 0, pops = 0;
     int st = 0;
     for (;;) {
         size = __shfl_sync(0xffffffffu, size, 0);
@@ -122,6 +182,7 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
         unsigned long long top = 0;
         if (lane == 0) top = heap_pop(heap, size);
         top = __shfl_sync(0xffffffffu, top, 0);
+        pops += 1;
         const uint32_t node = (uint32_t)top;
         const float dist = key_to_dist((uint32_t)(top >> 32));
         const int kind = node < F.n_nodes ? F.kind[node] : 0;
@@ -134,7 +195,7 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
                 if (i < len) {
                     row = F.desc_rows[off + i];
                     uint32_t bit = 1u << (row & 31);
-                    fresh = (atomicOr(&bm[row >> 5], bit) & bit) == 0;
+                    fresh = (!FILTER || (Fl.bits[row >> 5] & bit)) && (atomicOr(&bm[row >> 5], bit) & bit) == 0;
                 }
                 unsigned m = __ballot_sync(0xffffffffu, fresh);
                 if (fresh) {
@@ -143,9 +204,11 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
                 }
                 unique += __popc(m);
             }
-            total += len;
+            total += FILTER ? Fl.fcount[node] : len;
         } else if (kind == 2) {
             const uint32_t ni = F.normal_idx[node];
+            bool push_l = true, push_r = true;
+            if (FILTER && lane == 0) { push_l = Fl.live[F.left[node]]; push_r = Fl.live[F.right[node]]; }
             float mg = 0.0f;
             if (ni != 0xffffffffu) {
                 const float* nv = F.normals + (size_t)ni * ld;
@@ -163,8 +226,8 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
             if (lane == 0) {
                 if (size + 2 > cap) st = 2;
                 else {
-                    heap_push(heap, size, ((unsigned long long)ordered_key(f32_min_dev(-mg, dist)) << 32) | F.left[node]);
-                    heap_push(heap, size, ((unsigned long long)ordered_key(f32_min_dev(mg, dist)) << 32) | F.right[node]);
+                    if (push_l) heap_push(heap, size, ((unsigned long long)ordered_key(f32_min_dev(-mg, dist)) << 32) | F.left[node]);
+                    if (push_r) heap_push(heap, size, ((unsigned long long)ordered_key(f32_min_dev(mg, dist)) << 32) | F.right[node]);
                 }
             }
         } else {
@@ -173,7 +236,7 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
         st = __reduce_max_sync(0xffffffffu, st);
         if (st) break;
     }
-    if (lane == 0) { cand_count[q] = unique < cand_cap ? unique : cand_cap; status[q] = st; }
+    if (lane == 0) { cand_count[q] = unique < cand_cap ? unique : cand_cap; status[q] = st; if (FILTER) Fl.pops[q] = pops; }
 }
 
 // offsets[q] = q * cand_cap (begin), ends[q] = begin + count — segment descriptors for the sort
@@ -203,18 +266,22 @@ constexpr int W1_THREADS = 256;
 constexpr uint32_t W1_HEAP = 1024;     // heap entries in shared memory
 constexpr uint32_t W1_CAND = 8192;     // candidate slots in shared memory (duplicates included)
 constexpr uint32_t W1_LEAFQ = 128;     // Descendants nodes queued for the copier warps
+constexpr uint32_t W1_LEAFQ_FILTER = 2048;   // a filtered walk publishes more, smaller leaves (only those with a filtered row)
 
-struct Walk1Shared {
+template <uint32_t LEAFQ>
+struct Walk1SharedT {
     unsigned long long heap[W1_HEAP];
     uint32_t cand[W1_CAND];
-    volatile uint32_t lq_off[W1_LEAFQ], lq_len[W1_LEAFQ], lq_dst[W1_LEAFQ];   // (volatile: read by the copier warps right after `produced`)
+    volatile uint32_t lq_off[LEAFQ], lq_len[LEAFQ], lq_dst[LEAFQ];   // (volatile: read by the copier warps right after `produced`)
     uint32_t scan[W1_THREADS / 32];
     volatile uint32_t produced;
     volatile int done;
     uint32_t total;
     int status;
 };
-inline size_t walk1_smem(uint32_t ld) { return sizeof(Walk1Shared) + (size_t)ld * 4 + 16; }
+template <bool FILTER> using Walk1Shared = Walk1SharedT<FILTER ? W1_LEAFQ_FILTER : W1_LEAFQ>;
+constexpr size_t W1_MAX_LD = 8192;
+template <bool FILTER> inline size_t walk1_smem(uint32_t ld) { return sizeof(Walk1Shared<FILTER>) + (size_t)ld * 4 + 16; }
 
 // dots[q][node] = the reference's dot of query q with the normal of split node `node`, for EVERY normal of the forest (one warp per pair, the same
 // exact_warp the walker would call). A single query's walk is a chain of ~160 dependent pops, each of which would otherwise load
@@ -235,30 +302,41 @@ forest_dots_kernel(DevForest F, uint32_t n_normals, const float* __restrict__ it
     }
 }
 
+// FILTER: the frontier may outgrow the W1_HEAP shared-memory slots (a selective filter keeps the walk going through many more
+// splits); entries past them continue the same unsorted array in the query's global spill slot, so the arg-max, and with it
+// the pop order, is unchanged.
+template <bool FILTER>
 __global__ void __launch_bounds__(W1_THREADS)
 walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t ld, int metric, uint32_t nq,
              const uint32_t* __restrict__ qrows, const float* __restrict__ queries, const float* __restrict__ qh0,
-             const float* __restrict__ pre_dots, uint32_t n_normals, int debug, unsigned long long search_k, uint32_t* __restrict__ out_cand, uint32_t cand_cap, uint32_t* __restrict__ out_count, int32_t* __restrict__ status) {
+             const float* __restrict__ pre_dots, uint32_t n_normals, int debug, unsigned long long search_k, uint32_t* __restrict__ out_cand, uint32_t cand_cap, uint32_t* __restrict__ out_count, int32_t* __restrict__ status,
+             WalkFilter Fl) {
     extern __shared__ __align__(16) unsigned char w1_smem[];
-    Walk1Shared& S = *reinterpret_cast<Walk1Shared*>(w1_smem);
-    float* sq = reinterpret_cast<float*>(w1_smem + ((sizeof(Walk1Shared) + 15) & ~(size_t)15));
+    Walk1Shared<FILTER>& S = *reinterpret_cast<Walk1Shared<FILTER>*>(w1_smem);
+    float* sq = reinterpret_cast<float*>(w1_smem + ((sizeof(Walk1Shared<FILTER>) + 15) & ~(size_t)15));
+    constexpr uint32_t LEAFQ = FILTER ? W1_LEAFQ_FILTER : W1_LEAFQ;
     const uint32_t q = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* qv = qrows ? items + (size_t)qrows[q] * ld : queries + (size_t)q * ld;
     const float qhdr = qh0 ? qh0[q] : 0.f;
+    unsigned long long* spill = FILTER ? Fl.spill + (size_t)q * Fl.spill_cap : nullptr;
+    const uint32_t hcap = FILTER ? W1_HEAP + Fl.spill_cap : W1_HEAP;
+    auto hget = [&](uint32_t i) -> unsigned long long { return (!FILTER || i < W1_HEAP) ? S.heap[i] : spill[i - W1_HEAP]; };
+    auto hset = [&](uint32_t i, unsigned long long v) { if (!FILTER || i < W1_HEAP) S.heap[i] = v; else spill[i - W1_HEAP] = v; };
     for (uint32_t i = tid; i < ld; i += W1_THREADS) sq[i] = qv[i];
     if (tid == 0) { S.produced = 0; S.done = 0; S.total = 0; S.status = 0; }
     __syncthreads();
     const long long dbg_t0 = clock64();
-    uint32_t dbg_pops = 0, dbg_leaves = 0;
+    uint32_t dbg_pops = 0, dbg_leaves = 0, dbg_front = 0;
     if (warp == 0) {
         uint32_t size = 0, produced = 0, total32 = 0;
         unsigned long long total = 0;
         int st = 0;
         if (lane == 0) {
             const unsigned long long inf_key = (unsigned long long)ordered_key(__uint_as_float(0x7f800000u)) << 32;
-            for (uint32_t r = 0; r < F.n_roots && size < W1_HEAP; ++r) S.heap[size++] = inf_key | F.roots[r];
-            if (F.n_roots > W1_HEAP) st = 2;
+            uint32_t r = 0;
+            for (; r < F.n_roots && size < hcap; ++r) if (!FILTER || Fl.live[F.roots[r]]) hset(size++, inf_key | F.roots[r]);
+            if (FILTER ? r < F.n_roots : F.n_roots > W1_HEAP) st = 2;
         }
         st = __shfl_sync(0xffffffffu, st, 0);
         // The priority queue is an UNSORTED array: a push appends (lane 0), a pop is a warp-wide arg-max over the <= 1024 entries
@@ -270,7 +348,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
             __syncwarp();
             unsigned long long top = 0;
             uint32_t ti = 0xffffffffu;
-            for (uint32_t i = lane; i < size; i += 32) { const unsigned long long v = S.heap[i]; if (ti == 0xffffffffu || v > top) { top = v; ti = i; } }
+            for (uint32_t i = lane; i < size; i += 32) { const unsigned long long v = hget(i); if (ti == 0xffffffffu || v > top) { top = v; ti = i; } }
             {   // warp arg-max of a 64-bit key in two REDUX steps: the high halves, then the low halves among the lanes that hold the
                 // winning high half (a lane without an entry contributes 0 / loses the ballot)
                 const uint32_t hi = ti != 0xffffffffu ? (uint32_t)(top >> 32) : 0u;
@@ -282,7 +360,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
                 ti = __shfl_sync(0xffffffffu, ti, src);
                 top = ((unsigned long long)mh << 32) | ml;
             }
-            if (lane == 0) { S.heap[ti] = S.heap[size - 1]; size -= 1; }
+            if (lane == 0) { hset(ti, hget(size - 1)); size -= 1; }
             __syncwarp();
             dbg_pops += 1;
             const uint32_t node = (uint32_t)top;
@@ -292,18 +370,24 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
             const int kind = (int)r0.x;
             if (kind == 1) {
                 const uint32_t off = r1.y, len = r1.z;
-                if (total32 + len > W1_CAND || produced >= W1_LEAFQ) { st = 1; break; }
-                if (lane == 0) { S.lq_off[produced] = off; S.lq_len[produced] = len; S.lq_dst[produced] = total32; __threadfence_block(); S.produced = produced + 1; }
-                produced += 1; total32 += len; total += len; dbg_leaves += 1;
+                const uint32_t cnt = FILTER ? Fl.fcount[node] : len;   // slots this leaf fills
+                if (total32 + cnt > W1_CAND || produced >= LEAFQ) { st = 1; break; }
+                if (!FILTER || cnt) {
+                    if (lane == 0) { S.lq_off[produced] = off; S.lq_len[produced] = len; S.lq_dst[produced] = total32; __threadfence_block(); S.produced = produced + 1; }
+                    produced += 1;
+                }
+                total32 += cnt; total += cnt; dbg_leaves += 1;
             } else if (kind == 2) {
                 const uint32_t ni = r0.w;
                 const uint32_t lc = r0.y, rc = r0.z;
                 // the children will be popped soon (one of them usually next): have their records and dots on the way
+                uint32_t lv = 1;
                 if (lane < 2) {
                     const uint32_t ch = lane == 0 ? lc : rc;
                     if (ch < F.n_nodes) {
                         asm volatile("prefetch.global.L1 [%0];" :: "l"(F.rec + 2 * (size_t)ch));
                         if (pre_dots) asm volatile("prefetch.global.L1 [%0];" :: "l"(pre_dots + (size_t)q * F.n_nodes + ch));
+                        if (FILTER) { asm volatile("prefetch.global.L1 [%0];" :: "l"(Fl.fcount + ch)); lv = Fl.live[ch]; }
                     }
                 }
                 float mg = 0.0f;
@@ -312,17 +396,51 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
                     const float dt = pre_dots ? pre_dots[(size_t)q * F.n_nodes + node] : exact_warp<false>(nv, sq, (int)d);
                     mg = margin_finish(metric, dt, __uint_as_float(r1.x), qhdr);
                 }
+                const uint32_t live_r = FILTER ? __shfl_sync(0xffffffffu, lv, 1) : 1u;
                 if (lane == 0) {
-                    if (size + 2 > W1_HEAP) st = 2;
+                    if (size + 2 > hcap) st = 2;
                     else {
-                        S.heap[size++] = ((unsigned long long)ordered_key(f32_min_dev(-mg, dist)) << 32) | lc;
-                        S.heap[size++] = ((unsigned long long)ordered_key(f32_min_dev(mg, dist)) << 32) | rc;
+                        if (!FILTER || lv) hset(size++, ((unsigned long long)ordered_key(f32_min_dev(-mg, dist)) << 32) | lc);
+                        if (!FILTER || live_r) hset(size++, ((unsigned long long)ordered_key(f32_min_dev(mg, dist)) << 32) | rc);
                     }
+                    if (FILTER) dbg_front = max(dbg_front, size);
                 }
                 st = __shfl_sync(0xffffffffu, st, 0);
             } else st = 3;
         }
-        if (lane == 0) { S.total = total32; S.status = st; __threadfence_block(); S.done = 1; }
+        if (lane == 0) { S.total = total32; S.status = st; __threadfence_block(); S.done = 1; if (FILTER) Fl.pops[q] = dbg_pops; }
+    } else if (FILTER) {
+        // copier warps, filtered: the 32-row slices of all published leaves, numbered in publishing order, go round-robin to the
+        // warps (so leaves of 32 rows or fewer spread over all of them); a warp appends the rows whose filter bit is set at the
+        // leaf's cursor (lq_dst, bumped atomically), and reads `produced` / `done` once, through lane 0
+        const uint32_t cw = warp - 1, ncw = W1_THREADS / 32 - 1;
+        uint32_t e = 0, slice0 = 0;   // slice0: number of the first slice of leaf e
+        for (;;) {
+            int dn = 0;
+            uint32_t p = 0;
+            if (lane == 0) { dn = S.done; __threadfence_block(); p = S.produced; }
+            dn = __shfl_sync(0xffffffffu, dn, 0);
+            p = __shfl_sync(0xffffffffu, p, 0);
+            if (e < p) {
+                for (; e < p; ++e) {
+                    const uint32_t off = S.lq_off[e], len = S.lq_len[e];
+                    const uint32_t first = (cw + ncw - slice0 % ncw) % ncw;   // this warp's first slice of the leaf
+                    slice0 += (len + 31) / 32;
+                    for (uint32_t i0 = first * 32; i0 < len; i0 += ncw * 32) {
+                        const uint32_t i = i0 + lane;
+                        uint32_t row = 0;
+                        bool pass = false;
+                        if (i < len) { row = F.desc_rows[off + i]; pass = (Fl.bits[row >> 5] >> (row & 31)) & 1u; }
+                        const unsigned m = __ballot_sync(0xffffffffu, pass);
+                        uint32_t base = 0;
+                        if (lane == 0 && m) base = atomicAdd(const_cast<uint32_t*>(&S.lq_dst[e]), (uint32_t)__popc(m));
+                        base = __shfl_sync(0xffffffffu, base, 0);
+                        if (pass) S.cand[base + __popc(m & ((1u << lane) - 1u))] = row;
+                    }
+                }
+            } else if (dn) break;
+            else __nanosleep(100);
+        }
     } else {
         // copier warps: Descendants nodes as they are published
         const int t = tid - 32, nt = W1_THREADS - 32;
@@ -373,7 +491,10 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
     uint32_t* out = out_cand + (size_t)q * cand_cap;
     for (uint32_t i = b0; i < e0; ++i) if (i == 0 || S.cand[i] != S.cand[i - 1]) out[o++] = S.cand[i];
     if (tid == 0) { out_count[q] = uniq; status[q] = 0; }
-    if (debug && tid == 0) printf("[walk1] q %u: %u pops (%u leaves), walk %lld cycles, sort + unique %lld cycles, %u candidates (%u unique)\n", q, dbg_pops, dbg_leaves, dbg_t1 - dbg_t0, clock64() - dbg_t1, n, uniq);
+    if (debug && tid == 0) {
+        if (FILTER) printf("[walk1] q %u: %u pops (%u leaves), largest frontier %u, walk %lld cycles, sort + unique %lld cycles, %u candidates (%u unique)\n", q, dbg_pops, dbg_leaves, dbg_front, dbg_t1 - dbg_t0, clock64() - dbg_t1, n, uniq);
+        else printf("[walk1] q %u: %u pops (%u leaves), walk %lld cycles, sort + unique %lld cycles, %u candidates (%u unique)\n", q, dbg_pops, dbg_leaves, dbg_t1 - dbg_t0, clock64() - dbg_t1, n, uniq);
+    }
 }
 
 }  // namespace ab

@@ -268,6 +268,20 @@ int32_t arroy_b200_search_batch(arroy_ctx* ctx, uint32_t nq, const uint32_t* que
                                 const float* qhdr0, uint64_t count, uint64_t search_k,
                                 uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status);
 
+/* arroy_b200_search_batch with one QueryBuilder::candidates filter shared by every query of the call (reader.rs:350-357):
+ * filter_bits holds ceil(n / 32) words, bit r (word r / 32, bit r % 32) set when staged row r passes. A walk keeps only the
+ * filtered rows of each Descendants node and counts only those towards search_k, as the reference does; it never enters a
+ * subtree without a filtered row (or a missing node). When the filtered rows of the whole forest number at most search_k, the
+ * walk is skipped and they are re-ranked directly. Results and out_status as arroy_b200_search_batch. */
+int32_t arroy_b200_search_batch_filtered(arroy_ctx* ctx, uint32_t nq, const uint32_t* query_rows, const float* queries,
+                                         const float* qhdr0, uint64_t count, uint64_t search_k, const uint32_t* filter_bits,
+                                         uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status);
+
+/* Filtered-search counters since create: out[0] = filtered queries completed on the device, out[1] = of those, answered
+ * without a walk (the filter's rows in the forest numbered at most search_k), out[2] = filtered queries returned with a
+ * nonzero status (the caller falls back to its own walk), out[3] = nodes popped by filtered walks. */
+int32_t arroy_b200_search_stats(arroy_ctx* ctx, uint64_t out[4]);
+
 /* ---- synthetic data + timing helpers (bench / tests; not part of the reference seam) ---- */
 
 /* Fill a device matrix (rows x dim f32, dense) with element (i,j) = n-th gen::<f32>() of

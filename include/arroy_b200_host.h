@@ -121,8 +121,16 @@ int32_t arroy_reader_nns_by_item(arroy_reader* r, uint32_t item, uint64_t count,
 int32_t arroy_reader_nns_by_vector(arroy_reader* r, const float* vector, uint32_t len, uint64_t count, uint64_t search_k,
                                    uint64_t oversampling, const uint32_t* candidates, int64_t n_candidates,
                                    uint32_t* out_ids, float* out_dist, uint64_t* out_len);
-/* Many by_item queries in one call (not in the reference, which has no batching API): tree walks
- * run on host threads, the re-rank of all queries is one device launch. out_* are nq x count. */
+/* Many queries in one call (not in the reference, which has no batching API): exactly one of items (by_item, nq ids) and
+ * vectors (by_vector, nq x dimensions) is given, and one optional candidates filter (NULL / n_candidates < 0 = none) applies to
+ * every query. The walks, candidate sort and re-rank run on the device (arroy_b200_search_batch / _filtered); queries the
+ * device walk gives up on, count > 2048 or ARROY_B200_HOST_WALK=1 take the host walk and one batched device re-rank.
+ * out_* are nq x count; each row equals the single query with the same settings. */
+int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count,
+                               uint64_t search_k, uint64_t oversampling, const uint32_t* candidates, int64_t n_candidates,
+                               uint32_t* out_ids, float* out_dist, uint32_t* out_len,
+                               double* out_ms /* [0] tree walk [1] re-rank, may be NULL */);
+/* arroy_reader_nns_batch with items and no filter */
 int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint32_t* items, uint64_t count, uint64_t search_k,
                                        uint64_t oversampling, uint32_t* out_ids, float* out_dist, uint32_t* out_len,
                                        double* out_ms /* [0] tree walk [1] re-rank, may be NULL */);
