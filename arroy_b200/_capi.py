@@ -52,6 +52,9 @@ SIGNATURES = [
     ("arroy_b200_search_batch", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, _f32p, C.c_uint64, C.c_uint64, _u32p, _f32p, _u32p, C.POINTER(C.c_int32)]),
     ("arroy_b200_search_batch_filtered", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, _f32p, C.c_uint64, C.c_uint64, _u32p, _u32p, _f32p, _u32p, C.POINTER(C.c_int32)]),
     ("arroy_b200_search_stats", C.c_int32, [C.c_void_p, _u64p]),
+    ("arroy_b200_search_batch_multi_filtered", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, _f32p, C.c_uint64, C.c_uint64, C.c_uint32, _u64p, _u32p, _u32p,
+                                                           _u32p, _f32p, _u32p, C.POINTER(C.c_int32)]),
+    ("arroy_b200_multi_filter_stats", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_synth_device", C.c_int32, [C.c_void_p, _u8p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_float, C.c_void_p]),
     ("arroy_b200_time_scan", C.c_int32, [C.c_void_p, _f32p, C.c_float, C.c_float, _u32p, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, _f32p, _u64p]),
     ("arroy_b200_arena_new", C.c_void_p, []),
@@ -407,7 +410,17 @@ class Context:
             raise ValueError("filter_bits must hold ceil(n / 32) = %d words" % ((self.n + 31) // 32))
         return self._search(count, query_rows, queries, qhdr0, search_k, bits)
 
-    def _search(self, count, query_rows, queries, qhdr0, search_k, bits):
+    def search_batch_multi_filtered(self, count, filters, query_filter, query_rows=None, queries=None, qhdr0=None, search_k=0):
+        """search_batch with one row filter per query: query q uses filters[query_filter[q]], a list of ascending, unique row
+        indices. Several queries may share a filter; unused filters are allowed."""
+        lists = [np.ascontiguousarray(f, dtype=np.uint32).ravel() for f in filters]
+        offsets = np.zeros(len(lists) + 1, dtype=np.uint64)
+        offsets[1:] = np.cumsum([f.size for f in lists])
+        rows = np.concatenate(lists) if lists else np.zeros(0, np.uint32)
+        qf = np.ascontiguousarray(query_filter, dtype=np.uint32)
+        return self._search(count, query_rows, queries, qhdr0, search_k, None, (offsets, rows, qf))
+
+    def _search(self, count, query_rows, queries, qhdr0, search_k, bits, multi=None):
         if query_rows is not None:
             query_rows = np.ascontiguousarray(query_rows, dtype=np.uint32)
             nq = query_rows.size
@@ -420,7 +433,13 @@ class Context:
         out_len = np.zeros(nq, dtype=np.uint32)
         status = np.zeros(nq, dtype=np.int32)
         st = status.ctypes.data_as(C.POINTER(C.c_int32))
-        if bits is None:
+        if multi is not None:
+            offsets, rows, qf = multi
+            if qf.size != nq:
+                raise ValueError("query_filter must hold one filter index per query (%d)" % nq)
+            self._ck(self.lib.arroy_b200_search_batch_multi_filtered(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, offsets.size - 1,
+                                                                     offsets.ctypes.data_as(_u64p), _up(rows), _up(qf), _up(out_rows), _fp(out_dist), _up(out_len), st))
+        elif bits is None:
             self._ck(self.lib.arroy_b200_search_batch(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, _up(out_rows), _fp(out_dist), _up(out_len), st))
         else:
             self._ck(self.lib.arroy_b200_search_batch_filtered(self.h, nq, _up(query_rows), _fp(queries), _fp(h0), count, search_k, _up(bits), _up(out_rows), _fp(out_dist),
@@ -431,6 +450,11 @@ class Context:
         out = (C.c_uint64 * 4)()
         self._ck(self.lib.arroy_b200_search_stats(self.h, out))
         return {"filtered_queries": int(out[0]), "shortcut_queries": int(out[1]), "failed_queries": int(out[2]), "nodes_popped": int(out[3])}
+
+    def multi_filter_stats(self):
+        out = (C.c_uint64 * 2)()
+        self._ck(self.lib.arroy_b200_multi_filter_stats(self.h, out))
+        return {"summary_passes": int(out[0]), "filters_summarised": int(out[1])}
 
     # -- helpers ---------------------------------------------------------------------------------
     def synth_device(self, seed, dim, row0, rows, centre, device_ptr):

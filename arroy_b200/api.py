@@ -53,6 +53,8 @@ HOST_SIGNATURES = [
     ("arroy_reader_nns_batch_by_item", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, _f32p, _u32p, C.POINTER(C.c_double)]),
     ("arroy_reader_nns_batch", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, C.c_uint64, C.c_uint64, C.c_uint64, _u32p, C.c_int64, _u32p, _f32p, _u32p,
                                            C.POINTER(C.c_double)]),
+    ("arroy_reader_nns_batch_multi", C.c_int32, [C.c_void_p, C.c_uint32, _u32p, _f32p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, _u64p, _u32p, _u32p,
+                                                 _u32p, _f32p, _u32p, C.POINTER(C.c_double)]),
 ]
 
 _BOUND = False
@@ -68,6 +70,17 @@ def _lib():
             fn.argtypes = args
         _BOUND = True
     return lib
+
+
+def _id_array(ids):
+    """A collection of item ids as a uint32 array (any order; the library sorts)."""
+    a = ids if isinstance(ids, np.ndarray) else np.fromiter(ids, dtype=np.int64)
+    a = a.ravel()
+    if a.dtype != np.uint32:
+        if a.size and (a.min() < 0 or a.max() > 0xffffffff):
+            raise ValueError("item ids are u32")
+        a = a.astype(np.uint32)
+    return a
 
 
 class ArroyError(RuntimeError):
@@ -430,26 +443,45 @@ class Reader:
     def nns(self, count):
         return QueryBuilder(self, count)
 
-    def nns_batch_by_item(self, items, count, search_k=None, oversampling=None, candidates=None):
+    def nns_batch_by_item(self, items, count, search_k=None, oversampling=None, candidates=None, filters=None, filter_of_query=None):
         """One nns(count).search_k(..).oversampling(..).candidates(..).by_item(it) per item, in one call; candidates (optional)
-        is shared by every query. Returns (ids nq x count, distances nq x count, lengths nq, timings)."""
+        is shared by every query. Or one filter per query: filters is a list of id collections and query i uses
+        filters[filter_of_query[i]] (not together with candidates). Returns (ids nq x count, distances nq x count, lengths nq,
+        timings)."""
         items = np.ascontiguousarray(items, dtype=np.uint32)
-        return self._nns_batch(items.size, items.ctypes.data_as(_u32p), None, count, search_k, oversampling, candidates, items)
+        return self._nns_batch(items.size, items.ctypes.data_as(_u32p), None, count, search_k, oversampling, candidates, filters, filter_of_query, items)
 
-    def nns_batch_by_vector(self, vectors, count, search_k=None, oversampling=None, candidates=None):
+    def nns_batch_by_vector(self, vectors, count, search_k=None, oversampling=None, candidates=None, filters=None, filter_of_query=None):
         """nns_batch_by_item for query vectors (nq x dimensions), as QueryBuilder::by_vector."""
         vectors = np.ascontiguousarray(vectors, dtype=np.float32)
         if vectors.ndim != 2 or vectors.shape[1] != self.dimensions():
             raise ArroyError(100, "Invalid vector dimensions. Got %s but expected %d" % (vectors.shape[1:] or vectors.shape, self.dimensions()))
-        return self._nns_batch(vectors.shape[0], None, vectors.ctypes.data_as(_f32p), count, search_k, oversampling, candidates, vectors)
+        return self._nns_batch(vectors.shape[0], None, vectors.ctypes.data_as(_f32p), count, search_k, oversampling, candidates, filters, filter_of_query,
+                               vectors)
 
-    def _nns_batch(self, nq, items_p, vectors_p, count, search_k, oversampling, candidates, _keep):
+    def _nns_batch(self, nq, items_p, vectors_p, count, search_k, oversampling, candidates, filters, filter_of_query, _keep):
         out_ids = np.zeros((nq, max(count, 1)), dtype=np.uint32)
         out_dist = np.zeros((nq, max(count, 1)), dtype=np.float32)
         out_len = np.zeros(nq, dtype=np.uint32)
         ms = (C.c_double * 2)()
-        cand = None if candidates is None else np.ascontiguousarray(sorted(candidates), dtype=np.uint32)
-        _ck(_lib().arroy_reader_nns_batch(self.h, nq, items_p, vectors_p, count, min(search_k or 0, 2**64 - 1), oversampling or 0,
-                                          None if cand is None else cand.ctypes.data_as(_u32p), -1 if cand is None else cand.size,
-                                          out_ids.ctypes.data_as(_u32p), out_dist.ctypes.data_as(_f32p), out_len.ctypes.data_as(_u32p), ms))
+        sk, os_ = min(search_k or 0, 2**64 - 1), oversampling or 0
+        outs = (out_ids.ctypes.data_as(_u32p), out_dist.ctypes.data_as(_f32p), out_len.ctypes.data_as(_u32p), ms)
+        if filters is not None or filter_of_query is not None:
+            if candidates is not None:
+                raise ValueError("candidates= is one filter for every query; filters= / filter_of_query= give each query its own: pass one or the other")
+            if filters is None or filter_of_query is None:
+                raise ValueError("filters= and filter_of_query= go together")
+            lists = [_id_array(f) for f in filters]
+            offsets = np.zeros(len(lists) + 1, dtype=np.uint64)
+            offsets[1:] = np.cumsum([f.size for f in lists])
+            ids = np.concatenate(lists) if lists else np.zeros(0, np.uint32)
+            fq = np.ascontiguousarray(filter_of_query, dtype=np.uint32)
+            if fq.size != nq:
+                raise ValueError("filter_of_query must hold one filter index per query (%d)" % nq)
+            _ck(_lib().arroy_reader_nns_batch_multi(self.h, nq, items_p, vectors_p, count, sk, os_, len(lists), offsets.ctypes.data_as(_u64p),
+                                                    ids.ctypes.data_as(_u32p), fq.ctypes.data_as(_u32p), *outs))
+        else:
+            cand = None if candidates is None else np.ascontiguousarray(sorted(candidates), dtype=np.uint32)
+            _ck(_lib().arroy_reader_nns_batch(self.h, nq, items_p, vectors_p, count, sk, os_, None if cand is None else cand.ctypes.data_as(_u32p),
+                                              -1 if cand is None else cand.size, *outs))
         return out_ids, out_dist, out_len, {"tree_walk_ms": ms[0], "rerank_ms": ms[1]}

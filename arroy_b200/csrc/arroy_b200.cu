@@ -141,6 +141,10 @@ struct arroy_ctx {
     // per-call scratch of filtered searches (arroy_b200_search_batch_filtered)
     DevBuf w_fbits, w_fcount, w_live, w_ftotal, w_pops, w_spill, w_scount, w_soff;
     uint64_t filter_stats[4] = {0, 0, 0, 0};   // arroy_b200_search_stats
+    // per-call scratch of multi-filter searches (arroy_b200_search_batch_multi_filtered): the filters' row lists and offsets, the
+    // group summaries (search.cuh GroupSummaries), each query's filter (w_ftotal / w_pops are shared with the one-filter path)
+    DevBuf w_mrows, w_moffs, w_msum, w_mqf;
+    uint64_t multi_stats[2] = {0, 0};          // arroy_b200_multi_filter_stats
     // results of the last build_trees_begin, waiting for build_trees_emit
     std::vector<std::vector<struct BuiltTreeView>> pending_waves;
     std::vector<uint32_t> pending_wave_t0;
@@ -1830,28 +1834,36 @@ int32_t arroy_b200_load_forest(arroy_ctx* c, uint32_t n_nodes, const uint8_t* ki
 extern "C++" {
 namespace {
 
-template <bool FILTER> void configure_walk_kernels() {
+template <bool FILTER, bool MULTI = false> void configure_walk_kernels() {
     static bool configured = false;
     if (configured) return;
-    CK(cudaFuncSetAttribute(walk_kernel<FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)WALK_WARPS * WALK_SHEAP * 8)));
-    CK(cudaFuncSetAttribute(walk1_kernel<FILTER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk1_smem<FILTER>(W1_MAX_LD)));
+    CK(cudaFuncSetAttribute(walk_kernel<FILTER, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)WALK_WARPS * WALK_SHEAP * 8)));
+    CK(cudaFuncSetAttribute(walk1_kernel<FILTER, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk1_smem<FILTER>(W1_MAX_LD)));
     configured = true;
 }
 
-// arroy_b200_search_batch, and with filter_bits != NULL arroy_b200_search_batch_filtered: one row filter for every query
-void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
-                       uint64_t count, uint64_t search_k, const uint32_t* filter_bits, uint32_t* out_rows, float* out_dist, uint32_t* out_len,
-                       int32_t* out_status) {
+// The checks every batched search starts with. false: nothing to search (nq == 0, or count == 0 and the results are empty).
+bool batch_begin(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, uint64_t count, uint32_t* out_rows, float* out_dist,
+                 uint32_t* out_len, int32_t* out_status) {
         require_staged(c); set_device(c);
         if (!c->forest_loaded || c->forest_n != c->n) throw NotStaged("no forest loaded on this context for the staged items (arroy_b200_load_forest)");
-        if (nq == 0) return;
+        if (nq == 0) return false;
         if ((!query_rows && !queries) || !out_rows || !out_dist || !out_len) throw ArgError("null argument");
-        if (count == 0) { for (uint32_t q = 0; q < nq; ++q) { out_len[q] = 0; if (out_status) out_status[q] = 0; } return; }
+        if (count == 0) { for (uint32_t q = 0; q < nq; ++q) { out_len[q] = 0; if (out_status) out_status[q] = 0; } return false; }
         if (count > TOPK_CAP / 2) throw ArgError("count larger than the top-k buffer (TOPK_CAP/2 = 2048)");
         if (query_rows) for (uint32_t q = 0; q < nq; ++q) if (query_rows[q] >= c->n) throw ArgError("query row out of range");
-        const uint32_t ld = c->ld, k = (uint32_t)count;
+        return true;
+}
+
+// The per-query buffer sizes of a call's walks.
+struct BatchShape {
+    uint32_t k;
+    uint64_t search_k, cand_cap64;
+    uint32_t cand_cap, heap_cap, bm_words;
+};
+
+BatchShape batch_shape(arroy_ctx* c, uint64_t count, uint64_t search_k, bool filtered) {
         const DevForest& F = c->forest;
-        const bool filtered = filter_bits != nullptr;
         if (search_k == 0) search_k = count * F.n_roots;  // reader.rs:330
         // (filtered: saturating, so that search_k near 2^64 still leaves room for every filtered row the shortcut may take)
         const uint64_t sk_plus = filtered && search_k > UINT64_MAX - c->forest_max_desc ? UINT64_MAX : search_k + c->forest_max_desc;
@@ -1859,66 +1871,64 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
         // a filtered walk may push every node once (a filter can keep it going through the whole forest)
         const uint64_t heap_cap64 = (uint64_t)F.n_roots + (filtered ? (uint64_t)F.n_nodes : std::min<uint64_t>(F.n_nodes, 2 * std::min<uint64_t>(search_k, c->n) + 1024));
         if (cand_cap64 > 0x7fffffffull || heap_cap64 > 0x7fffffffull) throw ArgError("search_k too large for the device walk");
-        const uint32_t cand_cap = (uint32_t)std::max<uint64_t>(cand_cap64, 1), heap_cap = (uint32_t)heap_cap64;
-        const uint32_t bm_words = (uint32_t)((c->n + 31) / 32);
+        BatchShape S{};
+        S.k = (uint32_t)count; S.search_k = search_k; S.cand_cap64 = cand_cap64;
+        S.cand_cap = (uint32_t)std::max<uint64_t>(cand_cap64, 1); S.heap_cap = (uint32_t)heap_cap64;
+        S.bm_words = (uint32_t)((c->n + 31) / 32);
+        return S;
+}
+
+enum FilterMode { FM_NONE, FM_SHARED, FM_MULTI };
+
+// How the walks of one run_batch call are filtered. Queries [0, n_walk) walk; the others take the small-filter shortcut: with
+// FM_SHARED every query or none (the shared filter's rows from w_fbits / w_soff), with FM_MULTI per filter (the rows of the
+// query's filter f, rows[offs[f] .. offs[f + 1])).
+struct BatchFilter {
+    FilterMode mode = FM_NONE;
+    WalkFilter Fl{};
+    uint32_t n_walk = 0;
+    const uint32_t* rows = nullptr;
+    const uint64_t* offs = nullptr;
+};
+
+// The stages every batched search shares once its filters are summarised: the walks (or the shortcut), the candidate sort, the
+// re-rank and top-k, bq_normalize and the results, in the order of the nq queries given.
+void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0, const BatchShape& S,
+               const BatchFilter& bf, uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status) {
+        const uint32_t ld = c->ld, k = S.k, cand_cap = S.cand_cap, heap_cap = S.heap_cap, bm_words = S.bm_words;
+        const uint64_t search_k = S.search_k, cand_cap64 = S.cand_cap64;
+        const DevForest& F = c->forest;
+        const bool filtered = bf.mode != FM_NONE, multi = bf.mode == FM_MULTI;
+        const WalkFilter& Fl0 = bf.Fl;
         const size_t walk_smem = (size_t)WALK_WARPS * WALK_SHEAP * 8;
-        if (filtered) configure_walk_kernels<true>(); else configure_walk_kernels<false>();
-        for (double& x : c->sbreak) x = 0;
         int nte = 0;
         auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
-        // ---- the filter's summary: fcount / live per node and ftotal (search.cuh filter_count_kernel). When ftotal <= search_k
-        //      the reference's walk only ends with an empty queue, so its candidates are every filtered row of a reachable leaf:
-        //      the shortcut takes those without a walk (only where no reachable node is missing and pruning is exact).
-        WalkFilter Fl{};
-        bool shortcut = false;
         std::vector<int32_t> h_status;
         std::vector<uint32_t> h_pops;
-        auto filter_tally = [&](uint32_t m, bool walked) {   // after the stream is idle: statistics of m filtered queries
+        auto filter_tally = [&](uint32_t m, uint32_t m_walk) {   // after the stream is idle: statistics of m filtered queries, the first m_walk walked
             if (!filtered) return;
             h_status.resize(m); h_pops.resize(m);
             CK(cudaMemcpy(h_status.data(), c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost));
-            if (walked) CK(cudaMemcpy(h_pops.data(), c->w_pops.p, 4ull * m, cudaMemcpyDeviceToHost));
+            if (m_walk) CK(cudaMemcpy(h_pops.data(), c->w_pops.p, 4ull * m_walk, cudaMemcpyDeviceToHost));
             for (uint32_t q = 0; q < m; ++q) {
-                if (h_status[q] == 0) { c->filter_stats[0] += 1; c->filter_stats[1] += walked ? 0 : 1; }
+                if (h_status[q] == 0) { c->filter_stats[0] += 1; c->filter_stats[1] += q < m_walk ? 0 : 1; }
                 else c->filter_stats[2] += 1;
-                if (walked) c->filter_stats[3] += h_pops[q];
+                if (q < m_walk) c->filter_stats[3] += h_pops[q];
             }
         };
-        if (filtered) {
-            c->w_fbits.ensure(4ull * bm_words); c->w_fcount.ensure(std::max<size_t>(16, 4ull * F.n_nodes)); c->w_live.ensure(std::max<size_t>(16, F.n_nodes));
-            c->w_ftotal.ensure(16); c->w_pops.ensure(4ull * std::max<uint32_t>(nq, 1));
-            CK(cudaMemcpyAsync(c->w_fbits.p, filter_bits, 4ull * bm_words, cudaMemcpyHostToDevice, c->stream));
-            if (c->f_tree) CK(cudaMemcpyAsync(c->w_live.p, c->f_pin.p, F.n_nodes, cudaMemcpyDeviceToDevice, c->stream));
-            else CK(cudaMemsetAsync(c->w_live.p, 1, F.n_nodes, c->stream));
-            CK(cudaMemsetAsync(c->w_ftotal.p, 0, 8, c->stream));
-            if (F.n_nodes) {
-                filter_count_kernel<<<(uint32_t)(((uint64_t)F.n_nodes * 32 + 255) / 256), 256, 0, c->stream>>>(F, c->w_fbits.as<uint32_t>(), c->f_reach.as<uint8_t>(),
-                                                                                                              c->f_tree ? c->f_parent.as<uint32_t>() : nullptr, c->w_fcount.as<uint32_t>(),
-                                                                                                              c->w_live.as<uint8_t>(), c->w_ftotal.as<unsigned long long>());
-                CK(cudaGetLastError());
-                c->n_launches += 1;
-            }
-            unsigned long long ftotal = 0;
-            CK(cudaMemcpyAsync(&ftotal, c->w_ftotal.p, 8, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaStreamSynchronize(c->stream));
-            c->h2d_bytes += 4ull * bm_words;
-            Fl.bits = c->w_fbits.as<uint32_t>(); Fl.fcount = c->w_fcount.as<uint32_t>(); Fl.live = c->w_live.as<uint8_t>(); Fl.pops = c->w_pops.as<uint32_t>();
-            shortcut = c->f_tree && c->f_complete && ftotal <= search_k && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
-            if (shortcut) {   // the rows, ascending: popcounts per word, an exclusive scan, then every query's segment is written
-                c->w_scount.ensure(4ull * bm_words); c->w_soff.ensure(4ull * bm_words);
-                filter_select_count_kernel<<<(bm_words + 255) / 256, 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), bm_words, c->w_scount.as<uint32_t>());
-                CK(cudaGetLastError());
-                size_t tmp_bytes = 0;
-                CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
-                c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
-                CK(cub::DeviceScan::ExclusiveSum(c->w_tmp.p, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
-                c->n_launches += 2;
-            }
-        }
+        // the shortcut for queries q0 + [m_walk, m) of the call, their candidate segments [m_walk, m) of `cand`
+        auto shortcut = [&](uint32_t q0, uint32_t m_walk, uint32_t m, uint32_t* cand) {
+            if (multi) multi_filter_select_kernel<<<(m - m_walk + 7) / 8, 256, 0, c->stream>>>(bf.rows, bf.offs, Fl0.qfilter + q0 + m_walk, c->f_inleaf.as<uint32_t>(), m - m_walk,
+                                                                                              cand + (size_t)m_walk * cand_cap, cand_cap, c->w_count.as<uint32_t>() + m_walk,
+                                                                                              c->w_status.as<int32_t>() + m_walk);
+            else filter_select_scatter_kernel<<<dim3((bm_words + 255) / 256, m), 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), c->w_soff.as<uint32_t>(), bm_words,
+                                                                                                      cand, cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>());
+            CK(cudaGetLastError());
+        };
         // ---- a few queries: latency path, one CTA per query (search.cuh walk1_kernel), then the plain distance + top-k kernels on
         //      all SMs. Any query it cannot hold (heap / candidate overflow) sends the call through the general path below.
-        if (!shortcut && nq <= 16 && cand_cap64 <= (uint64_t)W1_CAND && getenv("ARROY_B200_NO_WALK1") == nullptr) {
-            const uint32_t m = nq;
+        if (bf.n_walk > 0 && nq <= 16 && cand_cap64 <= (uint64_t)W1_CAND && getenv("ARROY_B200_NO_WALK1") == nullptr) {
+            const uint32_t m = nq, m_walk = bf.n_walk;
             const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
             if (ld <= W1_MAX_LD) {
                 c->w_cand2.ensure(4ull * cand_cap * m); c->w_count.ensure(4ull * m); c->w_status.ensure(4ull * m);
@@ -1940,7 +1950,6 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
                 if (qhdr0) CK(cudaMemcpyAsync(c->s_qh0.p, qhdr0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
                 else if (query_rows) { gather_f32_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->s_qh0.as<float>(), c->h0.as<float>(), d_qrows, m); CK(cudaGetLastError()); }
                 else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
-                for (double& x : c->sbreak) x = 0;
                 int nte1 = 0;
                 auto mark1 = [&]() { if (!c->xev[nte1]) CK(cudaEventCreate(&c->xev[nte1])); CK(cudaEventRecord(c->xev[nte1], c->stream)); ++nte1; };
                 mark1();
@@ -1961,15 +1970,21 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
                     }
                 }
                 const int w1debug = getenv("ARROY_B200_WALK1_DEBUG") ? 1 : 0;
+                if (m_walk < m) shortcut(0, m_walk, m, c->w_cand2.as<uint32_t>());   // (multi only: a shared filter walks every query or none)
                 if (filtered) {
+                    WalkFilter Fl = Fl0;
                     Fl.spill_cap = F.n_roots + F.n_nodes;
-                    c->w_spill.ensure(8ull * Fl.spill_cap * m);
+                    c->w_spill.ensure(8ull * Fl.spill_cap * m_walk);
                     Fl.spill = c->w_spill.as<unsigned long long>();
-                    walk1_kernel<true><<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
-                                                                            c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
+                    if (multi)
+                        walk1_kernel<true, true><<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug,
+                                                                                           search_k, c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
+                    else
+                        walk1_kernel<true><<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
+                                                                                 c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
                 } else
                     walk1_kernel<false><<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
-                                                                             c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
+                                                                             c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl0);
                 CK(cudaGetLastError());
                 mark1();
                 walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
@@ -2000,7 +2015,7 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
                 for (uint32_t q = 0; q < m; ++q) all_ok = all_ok && h_st[q] == 0;
                 if (all_ok) {
                     if (out_status) for (uint32_t q = 0; q < m; ++q) out_status[q] = 0;
-                    filter_tally(m, true);
+                    filter_tally(m, m_walk);
                     c->d2h_bytes += 8ull * m * k + 8ull * m;
                     return;
                 }
@@ -2011,6 +2026,7 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
         uint32_t chunk = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>({(uint64_t)nq, (1ull << 30) / per_q, 65535ull}));
         for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
             const uint32_t m = std::min(chunk, nq - q0);
+            const uint32_t m_walk = q0 < bf.n_walk ? std::min(m, bf.n_walk - q0) : 0u;   // the chunk's first m_walk queries walk
             c->w_heaps.ensure(8ull * heap_cap * m); c->w_cand.ensure(4ull * cand_cap * m); c->w_cand2.ensure(4ull * cand_cap * m);
             c->w_count.ensure(4ull * m); c->w_bitmap.ensure(4ull * bm_words * m); c->w_status.ensure(4ull * m);
             c->w_beg.ensure(8ull * (m + 1)); c->w_end.ensure(8ull * (m + 1));
@@ -2034,23 +2050,29 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
                 CK(cudaGetLastError());
             } else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
             nte = 0; mark();
-            if (shortcut) {
-                filter_select_scatter_kernel<<<dim3((bm_words + 255) / 256, m), 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), c->w_soff.as<uint32_t>(), bm_words,
-                                                                                                    c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>());
-                CK(cudaGetLastError());
+            if (m_walk == 0) {   // every query of the chunk takes the shortcut: its segments are already sorted
+                shortcut(q0, 0, m, c->w_cand2.as<uint32_t>());
                 mark();
                 walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
                 CK(cudaGetLastError());
             } else {
-            CK(cudaMemsetAsync(c->w_bitmap.p, 0, 4ull * bm_words * m, c->stream));
-            if (filtered)
-                walk_kernel<true><<<(m + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(),
-                                                                                             search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
-                                                                                             c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
+            if (m_walk < m) shortcut(q0, m_walk, m, c->w_cand.as<uint32_t>());   // (multi only) sorted with the walked segments below
+            CK(cudaMemsetAsync(c->w_bitmap.p, 0, 4ull * bm_words * m_walk, c->stream));
+            if (multi) {
+                WalkFilter Fl = Fl0;
+                Fl.qfilter += q0;
+                walk_kernel<true, true><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q,
+                                                                                                        c->s_qh0.as<float>(), search_k, c->w_heaps.as<unsigned long long>(), heap_cap,
+                                                                                                        c->w_cand.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(),
+                                                                                                        bm_words, c->w_status.as<int32_t>(), Fl);
+            } else if (filtered)
+                walk_kernel<true><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(),
+                                                                                                  search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
+                                                                                                  c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl0);
             else
-                walk_kernel<false><<<(m + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(),
-                                                                                              search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
-                                                                                              c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
+                walk_kernel<false><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(),
+                                                                                                   search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
+                                                                                                   c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl0);
             CK(cudaGetLastError());
             mark();
             walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
@@ -2090,8 +2112,191 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
             if (out_status) CK(cudaMemcpyAsync(out_status + q0, c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
             CK(cudaStreamSynchronize(c->stream));
             for (int i = 0; i + 1 < nte; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); c->sbreak[i] += ms; }
-            filter_tally(m, !shortcut);
+            filter_tally(m, m_walk);
             c->d2h_bytes += 8ull * m * k + 8ull * m;
+        }
+}
+
+// arroy_b200_search_batch, and with filter_bits != NULL arroy_b200_search_batch_filtered: one row filter for every query
+void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
+                       uint64_t count, uint64_t search_k, const uint32_t* filter_bits, uint32_t* out_rows, float* out_dist, uint32_t* out_len,
+                       int32_t* out_status) {
+        if (!batch_begin(c, nq, query_rows, queries, count, out_rows, out_dist, out_len, out_status)) return;
+        const DevForest& F = c->forest;
+        const bool filtered = filter_bits != nullptr;
+        const BatchShape S = batch_shape(c, count, search_k, filtered);
+        const uint32_t bm_words = S.bm_words;
+        if (filtered) configure_walk_kernels<true>(); else configure_walk_kernels<false>();
+        for (double& x : c->sbreak) x = 0;
+        // ---- the filter's summary: fcount / live per node and ftotal (search.cuh filter_count_kernel). When ftotal <= search_k
+        //      the reference's walk only ends with an empty queue, so its candidates are every filtered row of a reachable leaf:
+        //      the shortcut takes those without a walk (only where no reachable node is missing and pruning is exact).
+        BatchFilter bf;
+        bf.mode = filtered ? FM_SHARED : FM_NONE;
+        bf.n_walk = nq;
+        if (filtered) {
+            c->w_fbits.ensure(4ull * bm_words); c->w_fcount.ensure(std::max<size_t>(16, 4ull * F.n_nodes)); c->w_live.ensure(std::max<size_t>(16, F.n_nodes));
+            c->w_ftotal.ensure(16); c->w_pops.ensure(4ull * std::max<uint32_t>(nq, 1));
+            CK(cudaMemcpyAsync(c->w_fbits.p, filter_bits, 4ull * bm_words, cudaMemcpyHostToDevice, c->stream));
+            if (c->f_tree) CK(cudaMemcpyAsync(c->w_live.p, c->f_pin.p, F.n_nodes, cudaMemcpyDeviceToDevice, c->stream));
+            else CK(cudaMemsetAsync(c->w_live.p, 1, F.n_nodes, c->stream));
+            CK(cudaMemsetAsync(c->w_ftotal.p, 0, 8, c->stream));
+            if (F.n_nodes) {
+                filter_count_kernel<<<(uint32_t)(((uint64_t)F.n_nodes * 32 + 255) / 256), 256, 0, c->stream>>>(F, c->w_fbits.as<uint32_t>(), c->f_reach.as<uint8_t>(),
+                                                                                                              c->f_tree ? c->f_parent.as<uint32_t>() : nullptr, c->w_fcount.as<uint32_t>(),
+                                                                                                              c->w_live.as<uint8_t>(), c->w_ftotal.as<unsigned long long>());
+                CK(cudaGetLastError());
+                c->n_launches += 1;
+            }
+            unsigned long long ftotal = 0;
+            CK(cudaMemcpyAsync(&ftotal, c->w_ftotal.p, 8, cudaMemcpyDeviceToHost, c->stream));
+            CK(cudaStreamSynchronize(c->stream));
+            c->h2d_bytes += 4ull * bm_words;
+            WalkFilter& Fl = bf.Fl;
+            Fl.bits = c->w_fbits.as<uint32_t>(); Fl.fcount = c->w_fcount.as<uint32_t>(); Fl.live = c->w_live.as<uint8_t>(); Fl.pops = c->w_pops.as<uint32_t>();
+            const bool shortcut = c->f_tree && c->f_complete && ftotal <= S.search_k && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
+            if (shortcut) {   // the rows, ascending: popcounts per word, an exclusive scan, then every query's segment is written
+                bf.n_walk = 0;
+                c->w_scount.ensure(4ull * bm_words); c->w_soff.ensure(4ull * bm_words);
+                filter_select_count_kernel<<<(bm_words + 255) / 256, 256, 0, c->stream>>>(c->w_fbits.as<uint32_t>(), c->f_inleaf.as<uint32_t>(), bm_words, c->w_scount.as<uint32_t>());
+                CK(cudaGetLastError());
+                size_t tmp_bytes = 0;
+                CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
+                c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
+                CK(cub::DeviceScan::ExclusiveSum(c->w_tmp.p, tmp_bytes, c->w_scount.as<uint32_t>(), c->w_soff.as<uint32_t>(), (int)bm_words, c->stream));
+                c->n_launches += 2;
+            }
+        }
+        run_batch(c, nq, query_rows, queries, qhdr0, S, bf, out_rows, out_dist, out_len, out_status);
+}
+
+// arroy_b200_search_batch_multi_filtered. The distinct filters the queries use are summarised 32 to a group (one row-mask
+// scatter and one multi_filter_count_kernel pass per group), as many groups at a time as fit the scratch bound of the summaries
+// (1 GiB); each such set of filters then runs its queries through run_batch, those whose filter takes the shortcut after the
+// ones that walk, and their results go back to the caller's query order.
+void multi_filter_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0, uint64_t count,
+                       uint64_t search_k, uint32_t n_filters, const uint64_t* filter_offsets, const uint32_t* filter_rows, const uint32_t* query_filter,
+                       uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status) {
+        require_staged(c);
+        if (nq > 0) {
+            if (n_filters == 0) throw ArgError("no filters for the queries");
+            if (!filter_offsets || !query_filter) throw ArgError("null filter argument");
+            for (uint32_t q = 0; q < nq; ++q) if (query_filter[q] >= n_filters) throw ArgError("query_filter out of range");
+            for (uint32_t f = 0; f < n_filters; ++f) {
+                const uint64_t b = filter_offsets[f], e = filter_offsets[f + 1];
+                if (e < b) throw ArgError("filter offsets must not decrease");
+                if (e > b && !filter_rows) throw ArgError("null filter rows");
+                for (uint64_t i = b; i < e; ++i) {
+                    if (filter_rows[i] >= c->n) throw ArgError("filter row out of range");
+                    if (i > b && filter_rows[i] <= filter_rows[i - 1]) throw ArgError("filter rows must be strictly ascending");
+                }
+            }
+        }
+        if (!batch_begin(c, nq, query_rows, queries, count, out_rows, out_dist, out_len, out_status)) return;
+        const DevForest& F = c->forest;
+        const BatchShape S = batch_shape(c, count, search_k, true);
+        const uint32_t k = S.k, d = c->dim;
+        configure_walk_kernels<true, true>();
+        for (double& x : c->sbreak) x = 0;
+        // the used filters in order of first use: filter used[u] is bit u % 32 of group u / 32
+        std::vector<uint32_t> used, slot(n_filters, UINT32_MAX);
+        for (uint32_t q = 0; q < nq; ++q) {
+            const uint32_t f = query_filter[q];
+            if (slot[f] == UINT32_MAX) { slot[f] = (uint32_t)used.size(); used.push_back(f); }
+        }
+        const uint32_t n_used = (uint32_t)used.size();
+        // per group (search.cuh GroupSummaries): a row mask per row, a live mask and 32 counts per node, plus 32 totals
+        GroupSummaries G{};
+        G.live_off = (c->n + 31) / 32 * 32;
+        G.count_off = G.live_off + ((uint64_t)F.n_nodes + 31) / 32 * 32;
+        G.group_words = G.count_off + 32ull * F.n_nodes;
+        const uint64_t group_bytes = 4ull * G.group_words + 256;
+        const uint32_t set_groups = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((1ull << 30) / group_bytes, 65535 / 32));
+        const bool shortcut_ok = c->f_tree && c->f_complete && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
+        std::vector<uint32_t> h_rows, h_qf, order, s_qrows, o_rows, o_len;
+        std::vector<uint64_t> h_offs;
+        std::vector<unsigned long long> ftotal;
+        std::vector<float> s_q, s_qh0, o_dist;
+        std::vector<int32_t> o_status;
+        for (uint32_t u0 = 0; u0 < n_used; u0 += 32 * set_groups) {
+            const uint32_t nf = std::min(32 * set_groups, n_used - u0), groups = (nf + 31) / 32;
+            h_offs.assign(1, 0); h_rows.clear();
+            uint64_t longest = 0;
+            for (uint32_t u = u0; u < u0 + nf; ++u) {
+                const uint64_t b = filter_offsets[used[u]], e = filter_offsets[used[u] + 1];
+                h_rows.insert(h_rows.end(), filter_rows + b, filter_rows + e);
+                h_offs.push_back(h_rows.size());
+                longest = std::max(longest, e - b);
+            }
+            int nte = 0;
+            auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
+            mark();
+            c->w_mrows.ensure(std::max<size_t>(16, 4ull * h_rows.size())); c->w_moffs.ensure(8ull * (nf + 1));
+            c->w_msum.ensure(4ull * G.group_words * groups); c->w_ftotal.ensure(256ull * groups);
+            G.sum = c->w_msum.as<uint32_t>();
+            c->w_pops.ensure(4ull * nq);
+            if (!h_rows.empty()) CK(cudaMemcpyAsync(c->w_mrows.p, h_rows.data(), 4ull * h_rows.size(), cudaMemcpyHostToDevice, c->stream));
+            CK(cudaMemcpyAsync(c->w_moffs.p, h_offs.data(), 8ull * (nf + 1), cudaMemcpyHostToDevice, c->stream));
+            CK(cudaMemset2DAsync(c->w_msum.p, 4ull * G.group_words, 0, 4ull * c->n, groups, c->stream));   // the row masks
+            if (longest) {
+                const uint32_t gx = (uint32_t)std::min<uint64_t>((longest + 255) / 256, (uint64_t)c->sm_count * 4);
+                multi_filter_mask_kernel<<<dim3(gx, nf), 256, 0, c->stream>>>(c->w_mrows.as<uint32_t>(), c->w_moffs.as<uint64_t>(), G);
+                CK(cudaGetLastError());
+                c->n_launches += 1;
+            }
+            mark();
+            CK(cudaMemsetAsync(c->w_ftotal.p, 0, 256ull * groups, c->stream));
+            if (F.n_nodes) {
+                multi_filter_live_init_kernel<<<dim3((F.n_nodes + 255) / 256, groups), 256, 0, c->stream>>>(c->f_tree ? c->f_pin.as<uint8_t>() : nullptr, F.n_nodes, G);
+                CK(cudaGetLastError());
+                multi_filter_count_kernel<<<dim3((uint32_t)(((uint64_t)F.n_nodes * 32 + 255) / 256), groups), 256, 0, c->stream>>>(F, G, c->f_reach.as<uint8_t>(),
+                                                                                                                                  c->f_tree ? c->f_parent.as<uint32_t>() : nullptr,
+                                                                                                                                  c->w_ftotal.as<unsigned long long>());
+                CK(cudaGetLastError());
+                c->n_launches += 2;
+            }
+            ftotal.resize(32ull * groups);
+            CK(cudaMemcpyAsync(ftotal.data(), c->w_ftotal.p, 256ull * groups, cudaMemcpyDeviceToHost, c->stream));
+            mark();
+            CK(cudaStreamSynchronize(c->stream));
+            { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[0], c->xev[1])); c->sbreak[5] += ms; CK(cudaEventElapsedTime(&ms, c->xev[1], c->xev[2])); c->sbreak[6] += ms; }
+            c->h2d_bytes += 4ull * h_rows.size() + 8ull * (nf + 1);
+            c->multi_stats[0] += groups; c->multi_stats[1] += nf;
+            // this set's queries: those that walk, then those whose filter takes the shortcut, each in call order
+            order.clear();
+            for (int pass = 0; pass < 2; ++pass)
+                for (uint32_t q = 0; q < nq; ++q) {
+                    const uint32_t u = slot[query_filter[q]];
+                    if (u < u0 || u >= u0 + nf) continue;
+                    const bool sc = shortcut_ok && ftotal[u - u0] <= S.search_k;
+                    if (sc == (pass == 1)) order.push_back(q);
+                }
+            const uint32_t m = (uint32_t)order.size();
+            BatchFilter bf;
+            bf.mode = FM_MULTI;
+            bf.n_walk = 0;
+            for (uint32_t q : order) bf.n_walk += !(shortcut_ok && ftotal[slot[query_filter[q]] - u0] <= S.search_k);
+            h_qf.resize(m);
+            for (uint32_t i = 0; i < m; ++i) h_qf[i] = slot[query_filter[order[i]]] - u0;
+            c->w_mqf.ensure(4ull * m);
+            CK(cudaMemcpyAsync(c->w_mqf.p, h_qf.data(), 4ull * m, cudaMemcpyHostToDevice, c->stream));
+            if (query_rows) { s_qrows.resize(m); for (uint32_t i = 0; i < m; ++i) s_qrows[i] = query_rows[order[i]]; }
+            else { s_q.resize((size_t)m * d); for (uint32_t i = 0; i < m; ++i) memcpy(&s_q[(size_t)i * d], queries + (size_t)order[i] * d, 4ull * d); }
+            if (qhdr0) { s_qh0.resize(m); for (uint32_t i = 0; i < m; ++i) s_qh0[i] = qhdr0[order[i]]; }
+            bf.rows = c->w_mrows.as<uint32_t>(); bf.offs = c->w_moffs.as<uint64_t>();
+            WalkFilter& Fl = bf.Fl;
+            Fl.pops = c->w_pops.as<uint32_t>(); Fl.qfilter = c->w_mqf.as<uint32_t>();
+            Fl.summary = G.sum; Fl.group_words = G.group_words; Fl.live_off = G.live_off; Fl.count_off = G.count_off;
+            o_rows.resize((size_t)m * k); o_dist.resize((size_t)m * k); o_len.resize(m); o_status.resize(m);
+            run_batch(c, m, query_rows ? s_qrows.data() : nullptr, query_rows ? nullptr : s_q.data(), qhdr0 ? s_qh0.data() : nullptr, S, bf,
+                      o_rows.data(), o_dist.data(), o_len.data(), o_status.data());
+            for (uint32_t i = 0; i < m; ++i) {
+                const uint32_t q = order[i];
+                memcpy(out_rows + (size_t)q * k, &o_rows[(size_t)i * k], 4ull * k);
+                memcpy(out_dist + (size_t)q * k, &o_dist[(size_t)i * k], 4ull * k);
+                out_len[q] = o_len[i];
+                if (out_status) out_status[q] = o_status[i];
+            }
         }
 }
 
@@ -2109,6 +2314,23 @@ int32_t arroy_b200_search_batch_filtered(arroy_ctx* c, uint32_t nq, const uint32
     return guarded(c, [&] {
         if (!filter_bits) throw ArgError("null filter");
         search_batch_body(c, nq, query_rows, queries, qhdr0, count, search_k, filter_bits, out_rows, out_dist, out_len, out_status);
+    });
+}
+
+int32_t arroy_b200_search_batch_multi_filtered(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, const float* qhdr0,
+                                               uint64_t count, uint64_t search_k, uint32_t n_filters, const uint64_t* filter_offsets,
+                                               const uint32_t* filter_rows, const uint32_t* query_filter, uint32_t* out_rows, float* out_dist,
+                                               uint32_t* out_len, int32_t* out_status) {
+    return guarded(c, [&] {
+        multi_filter_body(c, nq, query_rows, queries, qhdr0, count, search_k, n_filters, filter_offsets, filter_rows, query_filter, out_rows, out_dist,
+                          out_len, out_status);
+    });
+}
+
+int32_t arroy_b200_multi_filter_stats(arroy_ctx* c, uint64_t out[2]) {
+    return guarded(c, [&] {
+        if (!out) throw ArgError("null argument");
+        out[0] = c->multi_stats[0]; out[1] = c->multi_stats[1];
     });
 }
 

@@ -1201,6 +1201,23 @@ inline std::vector<uint32_t> candidate_row_bits(const arroy_reader* r, const std
     return bits;
 }
 
+// The same filter as ascending, unique rows (arroy_b200_search_batch_multi_filtered takes row lists).
+inline std::vector<uint32_t> candidate_rows(const arroy_reader* r, const std::vector<uint32_t>& sorted_ids) {
+    const size_t n = r->items.size();
+    std::vector<uint32_t> rows;
+    if (n && r->items.front() == 0 && r->items.back() == n - 1) {   // ids 0..n-1: row = id
+        for (uint32_t id : sorted_ids) { if (id >= n) break; if (rows.empty() || rows.back() != id) rows.push_back(id); }
+        return rows;
+    }
+    size_t j = 0;
+    for (uint32_t id : sorted_ids) {
+        while (j < n && r->items[j] < id) ++j;
+        if (j == n) break;
+        if (r->items[j] == id && (rows.empty() || rows.back() != j)) rows.push_back((uint32_t)j);
+    }
+    return rows;
+}
+
 // Where the host walk of one filtered query beats the device on an H100 (tools/bench_filtered_search.py on C2, DESIGN §7.1):
 //   - the filter holds at least 1/20 of the items: few leaves reach search_k, so the host walk is short and the device's fixed
 //     cost per filtered call (the bitmap upload and the summary pass over every leaf) dominates;
@@ -1471,18 +1488,29 @@ int32_t arroy_reader_nns_by_vector(arroy_reader* r, const float* vector, uint32_
         nns_by_leaf(r, vector, h0, h1, count, search_k, oversampling, cand, n_cand, out_ids, out_dist, out_len);
     });
 }
-int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count, uint64_t search_k,
-                               uint64_t oversampling, const uint32_t* cand, int64_t n_cand, uint32_t* out_ids, float* out_dist, uint32_t* out_len,
-                               double* out_ms) {
-    return hguard([&] {
+}  // extern "C"
+
+namespace arroy_host {
+
+// The filters of a batched call, as id lists sorted ascending: none (`sorted` empty), one for every query, or one per query
+// (`of_query`: the query's index into `sorted`).
+struct BatchFilters {
+    std::vector<std::vector<uint32_t>> sorted;
+    std::vector<uint32_t> of_query;
+    bool per_query() const { return !of_query.empty(); }
+    const std::vector<uint32_t>* of(uint32_t q) const { return sorted.empty() ? nullptr : &sorted[per_query() ? of_query[q] : 0]; }
+};
+
+// arroy_reader_nns_batch and arroy_reader_nns_batch_multi
+inline void nns_batch_body(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count, uint64_t search_k,
+                           uint64_t oversampling, const BatchFilters& bf, uint32_t* out_ids, float* out_dist, uint32_t* out_len, double* out_ms) {
         const uint32_t d = r->dims;
         const int hf = header_floats(r->metric);
         if ((items == nullptr) == (vectors == nullptr)) throw HostError(ARROY_ERR_PANIC, "exactly one of items / vectors must be given");
         check_fresh(r);
         std::vector<float> q, qh0, qh1;
         std::vector<std::vector<uint32_t>> rows;
-        std::vector<uint32_t> cv, fbits;
-        if (n_cand >= 0) { cv.assign(cand, cand + n_cand); std::sort(cv.begin(), cv.end()); }
+        std::vector<uint32_t> fbits;
         if (items)
             for (uint32_t i = 0; i < nq; ++i)
                 if (row_of(r, items[i]) < 0) throw HostError(ARROY_ERR_MISSING_KEY, "Internal error: Item(" + std::to_string(items[i]) + ") is missing in index `" + std::to_string(r->index) + "`");
@@ -1520,8 +1548,19 @@ int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* ite
             const uint32_t* qrp = items ? qrows.data() : nullptr;
             const float* qvp = items ? nullptr : q.data();
             const float* qhp = items ? nullptr : qh0.data();
-            if (n_cand >= 0) {
-                fbits = candidate_row_bits(r, cv);
+            if (bf.per_query()) {   // each used filter as ascending rows, CSR (unused ones empty)
+                std::vector<uint64_t> offs(bf.sorted.size() + 1, 0);
+                std::vector<uint32_t> frows;
+                std::vector<uint8_t> used(bf.sorted.size(), 0);
+                for (uint32_t f : bf.of_query) used[f] = 1;
+                for (size_t f = 0; f < bf.sorted.size(); ++f) {
+                    if (used[f]) { const std::vector<uint32_t> fr = candidate_rows(r, bf.sorted[f]); frows.insert(frows.end(), fr.begin(), fr.end()); }
+                    offs[f + 1] = frows.size();
+                }
+                dev_ck(r->ctx, arroy_b200_search_batch_multi_filtered(r->ctx, nq, qrp, qvp, qhp, count, eff_search_k, (uint32_t)bf.sorted.size(), offs.data(), frows.data(),
+                                                                      bf.of_query.data(), orow_dev.data(), out_dist, out_len, status.data()));
+            } else if (bf.of(0)) {
+                fbits = candidate_row_bits(r, *bf.of(0));
                 dev_ck(r->ctx, arroy_b200_search_batch_filtered(r->ctx, nq, qrp, qvp, qhp, count, eff_search_k, fbits.data(), orow_dev.data(), out_dist, out_len, status.data()));
             } else
                 dev_ck(r->ctx, arroy_b200_search_batch(r->ctx, nq, qrp, qvp, qhp, count, eff_search_k, orow_dev.data(), out_dist, out_len, status.data()));
@@ -1540,7 +1579,7 @@ int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* ite
         std::string err; std::mutex emu;
         const bool only_failed = !host_walk;
         auto worker = [&] {
-            try { for (;;) { uint32_t i = next.fetch_add(1); if (i >= nq) return; if (only_failed && status[i] == 0) continue; tree_walk(r, &q[(size_t)i * d], qh0[i], count, search_k, oversampling, n_cand >= 0 ? &cv : nullptr, rows[i]); } }
+            try { for (;;) { uint32_t i = next.fetch_add(1); if (i >= nq) return; if (only_failed && status[i] == 0) continue; tree_walk(r, &q[(size_t)i * d], qh0[i], count, search_k, oversampling, bf.of(i), rows[i]); } }
             catch (const std::exception& e) { std::lock_guard<std::mutex> lk(emu); err = e.what(); }
         };
         unsigned nt = std::max(1u, std::min<unsigned>(nq, std::thread::hardware_concurrency()));
@@ -1579,6 +1618,41 @@ int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* ite
                 memcpy(out_ids + (size_t)i * k, keep_ids.data() + (size_t)i * k, 4ull * k);
             }
         if (out_ms) out_ms[1] += ms_since(t0);
+}
+
+}  // namespace arroy_host
+
+extern "C" {
+
+int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count, uint64_t search_k,
+                               uint64_t oversampling, const uint32_t* cand, int64_t n_cand, uint32_t* out_ids, float* out_dist, uint32_t* out_len,
+                               double* out_ms) {
+    return hguard([&] {
+        BatchFilters bf;
+        if (n_cand >= 0) { bf.sorted.emplace_back(cand, cand + n_cand); std::sort(bf.sorted[0].begin(), bf.sorted[0].end()); }
+        nns_batch_body(r, nq, items, vectors, count, search_k, oversampling, bf, out_ids, out_dist, out_len, out_ms);
+    });
+}
+int32_t arroy_reader_nns_batch_multi(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count, uint64_t search_k,
+                                     uint64_t oversampling, uint32_t n_filters, const uint64_t* cand_offsets, const uint32_t* cand_ids,
+                                     const uint32_t* query_filter, uint32_t* out_ids, float* out_dist, uint32_t* out_len, double* out_ms) {
+    return hguard([&] {
+        if (nq > 0 && n_filters == 0) throw HostError(ARROY_ERR_PANIC, "no filters for the queries");
+        if (nq > 0 && (!cand_offsets || !query_filter)) throw HostError(ARROY_ERR_PANIC, "null filter argument");
+        for (uint32_t f = 0; f < n_filters; ++f) if (cand_offsets[f + 1] < cand_offsets[f]) throw HostError(ARROY_ERR_PANIC, "filter offsets must not decrease");
+        for (uint32_t i = 0; i < nq; ++i) if (query_filter[i] >= n_filters) throw HostError(ARROY_ERR_PANIC, "query_filter out of range");
+        BatchFilters bf;
+        bf.sorted.resize(n_filters);
+        bf.of_query.assign(query_filter, query_filter + nq);
+        std::vector<uint8_t> used(n_filters, 0);
+        for (uint32_t f : bf.of_query) used[f] = 1;
+        for (uint32_t f = 0; f < n_filters; ++f)   // (an unused filter stays empty: nothing reads it)
+            if (used[f]) {
+                std::vector<uint32_t>& v = bf.sorted[f];
+                v.assign(cand_ids + cand_offsets[f], cand_ids + cand_offsets[f + 1]);
+                if (!std::is_sorted(v.begin(), v.end())) std::sort(v.begin(), v.end());
+            }
+        nns_batch_body(r, nq, items, vectors, count, search_k, oversampling, bf, out_ids, out_dist, out_len, out_ms);
     });
 }
 int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint32_t* items, uint64_t count, uint64_t search_k, uint64_t oversampling,

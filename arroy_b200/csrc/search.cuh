@@ -101,7 +101,96 @@ struct WalkFilter {
     uint32_t* pops;             // per query: nodes popped
     unsigned long long* spill;  // walk1_kernel: per query, frontier entries past the shared-memory slots (spill_cap each)
     uint32_t spill_cap;
+    // MULTI walks (one filter per query, arroy_b200_search_batch_multi_filtered): query q reads bit qfilter[q] % 32 of the
+    // summaries of group qfilter[q] / 32 (GroupSummaries) in place of bits / fcount / live
+    const uint32_t* qfilter;
+    const uint32_t* summary;
+    unsigned long long group_words, live_off, count_off;
 };
+
+// The summaries of up to 32 filters (a group), group_words words per group in one buffer:
+//   [0, n_rows)             row masks: bit b of word r = row r passes filter b of the group
+//   [live_off, + n_nodes)   live masks: bit b = the node's subtree holds a row of filter b (or a missing node)
+//   [count_off, + 32 n_nodes) fcount: word 32 node + b = |desc(node) & filter b| (Descendants nodes)
+// One block per group keeps a walker's filter state at one pointer and one bit.
+struct GroupSummaries {
+    uint32_t* sum;
+    unsigned long long group_words, live_off, count_off;
+};
+
+// ---- many filters per call: one summary pass per group of 32 ----------------------------------------------------------
+// Each filter sets its bit in its group's row masks (one block row per filter of the call).
+__global__ void multi_filter_mask_kernel(const uint32_t* __restrict__ rows, const uint64_t* __restrict__ offs, GroupSummaries G) {
+    const uint32_t f = blockIdx.y;
+    const uint64_t e = offs[f + 1];
+    uint32_t* m = G.sum + (f >> 5) * G.group_words;
+    const uint32_t bit = 1u << (f & 31);
+    for (uint64_t i = offs[f] + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (uint64_t)gridDim.x * blockDim.x) atomicOr(&m[rows[i]], bit);
+}
+
+// live masks before the summary pass: all bits on pinned nodes (a missing node and its ancestors), or on every node when the
+// forest is not tree-shaped (no pruning)
+__global__ void multi_filter_live_init_kernel(const uint8_t* __restrict__ pin, uint32_t n_nodes, GroupSummaries G) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_nodes) G.sum[blockIdx.y * G.group_words + G.live_off + i] = (!pin || pin[i]) ? 0xffffffffu : 0u;
+}
+
+// filter_count_kernel for the 32 filters of group blockIdx.y at once: one warp per Descendants node reads its rows' masks once;
+// lane b ends with fcount of filter b, and the OR of the masks is ORed into the live masks of the node and its ancestors
+// (`parent`: tree-shaped forests), stopping at the first that already holds those bits.
+__global__ void multi_filter_count_kernel(DevForest F, GroupSummaries G, const uint8_t* __restrict__ reach, const uint32_t* __restrict__ parent,
+                                          unsigned long long* __restrict__ ftotal) {
+    const uint32_t node = (uint32_t)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    const uint32_t g = blockIdx.y;
+    if (node >= F.n_nodes || F.kind[node] != 1) return;
+    uint32_t* gs = G.sum + g * G.group_words;
+    const uint32_t* m = gs;
+    const uint32_t off = F.desc_off[node], len = F.desc_len[node];
+    uint32_t cnt = 0, any = 0;
+    for (uint32_t i0 = 0; i0 < len; i0 += 32) {
+        const uint32_t x = i0 + lane < len ? m[F.desc_rows[off + i0 + lane]] : 0u;
+        uint32_t u = __reduce_or_sync(0xffffffffu, x);
+        any |= u;
+        for (; u; u &= u - 1) {   // only the filters present in these 32 rows
+            const int b = __ffs((int)u) - 1;
+            const unsigned v = __ballot_sync(0xffffffffu, (x >> b) & 1u);
+            if (lane == b) cnt += __popc(v);
+        }
+    }
+    gs[G.count_off + (size_t)node * 32 + lane] = cnt;
+    if (cnt && reach[node]) atomicAdd(&ftotal[g * 32 + lane], (unsigned long long)cnt);
+    if (lane == 0 && any && parent) {
+        uint32_t* lv = gs + G.live_off;
+        for (uint32_t x = node; x != NO_PARENT; x = parent[x]) if ((atomicOr(&lv[x], any) & any) == any) break;
+    }
+}
+
+// The small-filter shortcut of a multi-filter call, one warp per query: the query's filter rows that some reachable leaf
+// holds, already ascending (a compaction of the filter's row list).
+__global__ void multi_filter_select_kernel(const uint32_t* __restrict__ rows, const uint64_t* __restrict__ offs, const uint32_t* __restrict__ qfilter,
+                                           const uint32_t* __restrict__ inleaf, uint32_t nq, uint32_t* __restrict__ cand, uint32_t cand_cap,
+                                           uint32_t* __restrict__ cand_count, int32_t* __restrict__ status) {
+    const uint32_t q = (uint32_t)(((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;
+    const uint32_t f = qfilter[q];
+    const uint64_t b = offs[f], e = offs[f + 1];
+    uint32_t* out = cand + (size_t)q * cand_cap;
+    uint32_t o = 0;
+    int st = 0;
+    for (uint64_t i0 = b; i0 < e; i0 += 32) {
+        const uint64_t i = i0 + lane;
+        uint32_t row = 0;
+        bool keep = false;
+        if (i < e) { row = rows[i]; keep = (inleaf[row >> 5] >> (row & 31)) & 1u; }
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        if (keep) { const uint32_t p = o + __popc(m & ((1u << lane) - 1u)); if (p < cand_cap) out[p] = row; else st = 1; }
+        o += __popc(m);
+    }
+    st = __reduce_max_sync(0xffffffffu, st);
+    if (lane == 0) { cand_count[q] = o < cand_cap ? o : cand_cap; status[q] = st; }
+}
 
 // fcount for every Descendants node (one warp per node) and ftotal = their sum over the nodes reachable from the roots. With
 // `parent` (a tree-shaped forest), a node with a filtered row flags itself and its ancestors live, stopping at the first one
@@ -146,19 +235,25 @@ __global__ void filter_select_scatter_kernel(const uint32_t* __restrict__ bits, 
     if (w == words - 1) { cand_count[q] = o; status[q] = 0; }
 }
 
-// query q: vector = qrows ? items[qrows[q]] : queries[q] (ld floats); qh0 = extra_dim for DotProduct margins
-template <bool FILTER>
+// query q: vector = qrows ? items[qrows[q]] : queries[q] (ld floats); qh0 = extra_dim for DotProduct margins.
+// FILTER: one filter for every query (Fl.bits / fcount / live); with MULTI, each query's own (Fl.qfilter, the group summaries).
+template <bool FILTER, bool MULTI = false>
 __global__ void __launch_bounds__(WALK_WARPS * 32)
 walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t ld, int metric, uint32_t nq,
             const uint32_t* __restrict__ qrows, const float* __restrict__ queries, const float* __restrict__ qh0,
             unsigned long long search_k, unsigned long long* __restrict__ heaps, uint32_t heap_cap,
             uint32_t* __restrict__ cand, uint32_t cand_cap, uint32_t* __restrict__ cand_count,
             uint32_t* __restrict__ bitmap, uint32_t bitmap_words, int32_t* __restrict__ status, WalkFilter Fl) {
+    static_assert(FILTER || !MULTI, "MULTI is a filtered walk");
     const int lane = threadIdx.x & 31;
     const uint32_t q = blockIdx.x * WALK_WARPS + (threadIdx.x >> 5);
     if (q >= nq) return;
     const float* qv = qrows ? items + (size_t)qrows[q] * ld : queries + (size_t)q * ld;
     const float qhdr = qh0 ? qh0[q] : 0.f;
+    // MULTI: this query's filter is bit fb of the group summaries at gs
+    const uint32_t qf = MULTI ? Fl.qfilter[q] : 0u, fb = qf & 31u;
+    const uint32_t* gs = MULTI ? Fl.summary + (qf >> 5) * Fl.group_words : nullptr;
+    auto live = [&](uint32_t node) -> bool { return MULTI ? (gs[Fl.live_off + node] >> fb) & 1u : Fl.live[node]; };
     // The heap lives in shared memory (a walk pushes two entries per pop: a few hundred in practice) and moves to
     // its global-memory slot only if it outgrows WALK_SHEAP: every pop / push is a chain of dependent accesses.
     extern __shared__ unsigned long long walk_sheap[];
@@ -171,7 +266,7 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
     if (F.n_roots > cap) { heap = gheap; cap = heap_cap; }
     if (lane == 0) {
         const unsigned long long inf_key = (unsigned long long)ordered_key(__uint_as_float(0x7f800000u)) << 32;
-        for (uint32_t r = 0; r < F.n_roots && size < cap; ++r) if (!FILTER || Fl.live[F.roots[r]]) heap_push(heap, size, inf_key | F.roots[r]);
+        for (uint32_t r = 0; r < F.n_roots && size < cap; ++r) if (!FILTER || live(F.roots[r])) heap_push(heap, size, inf_key | F.roots[r]);
     }
     unsigned long long total = 0;   // nns.len() of the reference (duplicates included)
     uint32_t unique = 0, pops = 0;
@@ -195,7 +290,7 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
                 if (i < len) {
                     row = F.desc_rows[off + i];
                     uint32_t bit = 1u << (row & 31);
-                    fresh = (!FILTER || (Fl.bits[row >> 5] & bit)) && (atomicOr(&bm[row >> 5], bit) & bit) == 0;
+                    fresh = (!FILTER || (MULTI ? ((gs[row] >> fb) & 1u) : (Fl.bits[row >> 5] & bit))) && (atomicOr(&bm[row >> 5], bit) & bit) == 0;
                 }
                 unsigned m = __ballot_sync(0xffffffffu, fresh);
                 if (fresh) {
@@ -204,11 +299,11 @@ walk_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t l
                 }
                 unique += __popc(m);
             }
-            total += FILTER ? Fl.fcount[node] : len;
+            total += FILTER ? (MULTI ? gs[Fl.count_off + (size_t)node * 32 + fb] : Fl.fcount[node]) : len;
         } else if (kind == 2) {
             const uint32_t ni = F.normal_idx[node];
             bool push_l = true, push_r = true;
-            if (FILTER && lane == 0) { push_l = Fl.live[F.left[node]]; push_r = Fl.live[F.right[node]]; }
+            if (FILTER && lane == 0) { push_l = live(F.left[node]); push_r = live(F.right[node]); }
             float mg = 0.0f;
             if (ni != 0xffffffffu) {
                 const float* nv = F.normals + (size_t)ni * ld;
@@ -304,8 +399,8 @@ forest_dots_kernel(DevForest F, uint32_t n_normals, const float* __restrict__ it
 
 // FILTER: the frontier may outgrow the W1_HEAP shared-memory slots (a selective filter keeps the walk going through many more
 // splits); entries past them continue the same unsorted array in the query's global spill slot, so the arg-max, and with it
-// the pop order, is unchanged.
-template <bool FILTER>
+// the pop order, is unchanged. MULTI: each query reads its own filter's bit, as in walk_kernel.
+template <bool FILTER, bool MULTI = false>
 __global__ void __launch_bounds__(W1_THREADS)
 walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t ld, int metric, uint32_t nq,
              const uint32_t* __restrict__ qrows, const float* __restrict__ queries, const float* __restrict__ qh0,
@@ -319,6 +414,9 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* qv = qrows ? items + (size_t)qrows[q] * ld : queries + (size_t)q * ld;
     const float qhdr = qh0 ? qh0[q] : 0.f;
+    static_assert(FILTER || !MULTI, "MULTI is a filtered walk");
+    const uint32_t qf = MULTI ? Fl.qfilter[q] : 0u, fb = qf & 31u;
+    const uint32_t* gs = MULTI ? Fl.summary + (qf >> 5) * Fl.group_words : nullptr;
     unsigned long long* spill = FILTER ? Fl.spill + (size_t)q * Fl.spill_cap : nullptr;
     const uint32_t hcap = FILTER ? W1_HEAP + Fl.spill_cap : W1_HEAP;
     auto hget = [&](uint32_t i) -> unsigned long long { return (!FILTER || i < W1_HEAP) ? S.heap[i] : spill[i - W1_HEAP]; };
@@ -335,7 +433,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
         if (lane == 0) {
             const unsigned long long inf_key = (unsigned long long)ordered_key(__uint_as_float(0x7f800000u)) << 32;
             uint32_t r = 0;
-            for (; r < F.n_roots && size < hcap; ++r) if (!FILTER || Fl.live[F.roots[r]]) hset(size++, inf_key | F.roots[r]);
+            for (; r < F.n_roots && size < hcap; ++r) if (!FILTER || (MULTI ? (gs[Fl.live_off + F.roots[r]] >> fb) & 1u : Fl.live[F.roots[r]])) hset(size++, inf_key | F.roots[r]);
             if (FILTER ? r < F.n_roots : F.n_roots > W1_HEAP) st = 2;
         }
         st = __shfl_sync(0xffffffffu, st, 0);
@@ -370,7 +468,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
             const int kind = (int)r0.x;
             if (kind == 1) {
                 const uint32_t off = r1.y, len = r1.z;
-                const uint32_t cnt = FILTER ? Fl.fcount[node] : len;   // slots this leaf fills
+                const uint32_t cnt = FILTER ? (MULTI ? gs[Fl.count_off + (size_t)node * 32 + fb] : Fl.fcount[node]) : len;   // slots this leaf fills
                 if (total32 + cnt > W1_CAND || produced >= LEAFQ) { st = 1; break; }
                 if (!FILTER || cnt) {
                     if (lane == 0) { S.lq_off[produced] = off; S.lq_len[produced] = len; S.lq_dst[produced] = total32; __threadfence_block(); S.produced = produced + 1; }
@@ -387,7 +485,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
                     if (ch < F.n_nodes) {
                         asm volatile("prefetch.global.L1 [%0];" :: "l"(F.rec + 2 * (size_t)ch));
                         if (pre_dots) asm volatile("prefetch.global.L1 [%0];" :: "l"(pre_dots + (size_t)q * F.n_nodes + ch));
-                        if (FILTER) { asm volatile("prefetch.global.L1 [%0];" :: "l"(Fl.fcount + ch)); lv = Fl.live[ch]; }
+                        if (FILTER) { asm volatile("prefetch.global.L1 [%0];" :: "l"(MULTI ? gs + Fl.count_off + (size_t)ch * 32 + fb : Fl.fcount + ch)); lv = MULTI ? (gs[Fl.live_off + ch] >> fb) & 1u : Fl.live[ch]; }
                     }
                 }
                 float mg = 0.0f;
@@ -430,7 +528,7 @@ walk1_kernel(DevForest F, const float* __restrict__ items, uint32_t d, uint32_t 
                         const uint32_t i = i0 + lane;
                         uint32_t row = 0;
                         bool pass = false;
-                        if (i < len) { row = F.desc_rows[off + i]; pass = (Fl.bits[row >> 5] >> (row & 31)) & 1u; }
+                        if (i < len) { row = F.desc_rows[off + i]; pass = MULTI ? (gs[row] >> fb) & 1u : (Fl.bits[row >> 5] >> (row & 31)) & 1u; }
                         const unsigned m = __ballot_sync(0xffffffffu, pass);
                         uint32_t base = 0;
                         if (lane == 0 && m) base = atomicAdd(const_cast<uint32_t*>(&S.lq_dst[e]), (uint32_t)__popc(m));

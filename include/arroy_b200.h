@@ -282,6 +282,21 @@ int32_t arroy_b200_search_batch_filtered(arroy_ctx* ctx, uint32_t nq, const uint
  * nonzero status (the caller falls back to its own walk), out[3] = nodes popped by filtered walks. */
 int32_t arroy_b200_search_stats(arroy_ctx* ctx, uint64_t out[4]);
 
+/* arroy_b200_search_batch_filtered with one filter per query: query q uses filter query_filter[q] (< n_filters).
+ * Filter f is the ascending, unique staged rows filter_rows[filter_offsets[f] .. filter_offsets[f+1]).
+ * Several queries may share a filter; unused filters are allowed. Row q of the outputs equals
+ * arroy_b200_search_batch_filtered(..., bitmap of filter query_filter[q], ...) for that query alone, and out_status keeps
+ * its meaning. The filters the queries use are summarised 32 per pass over the forest's descendant lists; a filter whose rows
+ * in the forest number at most search_k answers its queries without a walk. Counted in arroy_b200_search_stats like the
+ * one-filter queries. A query_filter >= n_filters, n_filters == 0 with nq > 0, decreasing offsets, a row >= n or rows not
+ * strictly ascending within a filter are argument errors. */
+int32_t arroy_b200_search_batch_multi_filtered(arroy_ctx* ctx, uint32_t nq, const uint32_t* query_rows, const float* queries,
+                                               const float* qhdr0, uint64_t count, uint64_t search_k, uint32_t n_filters,
+                                               const uint64_t* filter_offsets, const uint32_t* filter_rows, const uint32_t* query_filter,
+                                               uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status);
+/* out[0] = filter-summary passes run by multi-filter calls since create, out[1] = filters summarised */
+int32_t arroy_b200_multi_filter_stats(arroy_ctx* ctx, uint64_t out[2]);
+
 /* ---- synthetic data + timing helpers (bench / tests; not part of the reference seam) ---- */
 
 /* Fill a device matrix (rows x dim f32, dense) with element (i,j) = n-th gen::<f32>() of
@@ -333,7 +348,8 @@ int32_t arroy_b200_prefilter_scores(arroy_ctx* ctx, uint32_t nq, const float* qu
 int32_t arroy_b200_rerank_stats(arroy_ctx* ctx, uint64_t out[4]);
 
 /* CUDA-event breakdown of the last arroy_b200_search_batch call (ms, summed over its query chunks):
- * [0] bitmap clear + tree walk, [1] candidate sort, [2] distances, [3] top-k, [4..7] reserved. */
+ * [0] bitmap clear + tree walk, [1] candidate sort, [2] distances, [3] top-k, [4] reserved; after a multi-filter call also
+ * [5] filter upload + row masks, [6] filter summaries (both summed over its filter sets); [7] reserved. */
 int32_t arroy_b200_search_breakdown(arroy_ctx* ctx, double out[8]);
 
 /* CUDA-event breakdown of the last arroy_b200_rerank_shared call (ms, summed over its query chunks):

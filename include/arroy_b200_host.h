@@ -130,6 +130,15 @@ int32_t arroy_reader_nns_batch(arroy_reader* r, uint32_t nq, const uint32_t* ite
                                uint64_t search_k, uint64_t oversampling, const uint32_t* candidates, int64_t n_candidates,
                                uint32_t* out_ids, float* out_dist, uint32_t* out_len,
                                double* out_ms /* [0] tree walk [1] re-rank, may be NULL */);
+/* arroy_reader_nns_batch with one candidates filter per query: query i uses filter query_filter[i] (< n_filters), the item ids
+ * cand_ids[cand_offsets[f] .. cand_offsets[f+1]) (any order; duplicates and ids outside the index drop out, as in
+ * QueryBuilder::candidates). Several queries may share a filter and unused filters are allowed. The device walks every query
+ * with its own filter (arroy_b200_search_batch_multi_filtered); the host walk takes over as in arroy_reader_nns_batch, each query
+ * with its own filter. Each row equals the single query with that filter. */
+int32_t arroy_reader_nns_batch_multi(arroy_reader* r, uint32_t nq, const uint32_t* items, const float* vectors, uint64_t count,
+                                     uint64_t search_k, uint64_t oversampling, uint32_t n_filters, const uint64_t* cand_offsets,
+                                     const uint32_t* cand_ids, const uint32_t* query_filter, uint32_t* out_ids, float* out_dist,
+                                     uint32_t* out_len, double* out_ms /* [0] tree walk [1] re-rank, may be NULL */);
 /* arroy_reader_nns_batch with items and no filter */
 int32_t arroy_reader_nns_batch_by_item(arroy_reader* r, uint32_t nq, const uint32_t* items, uint64_t count, uint64_t search_k,
                                        uint64_t oversampling, uint32_t* out_ids, float* out_dist, uint32_t* out_len,
