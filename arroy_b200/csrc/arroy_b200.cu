@@ -1083,7 +1083,7 @@ void frerank_launch(arroy_ctx* c, uint32_t m, const float* d_q, const uint32_t* 
     P.d = c->dim; P.ld = c->ld; P.metric = c->metric;
     P.queries = d_q; P.qrows = d_qrows; P.qh0 = d_qh0;
     P.rows = d_rows; P.seg_beg = d_beg; P.seg_end = d_end;
-    P.k = k; P.rel = fr_rel(c->dim); P.gmax_bits = c->fr_gmax.as<uint32_t>();
+    P.k = k; P.rel = fr_rel(c->dim); P.sub = fr_sub(c->dim); P.hmin = cos_header_min(c->dim); P.gmax_bits = c->fr_gmax.as<uint32_t>();
     P.out_rows = c->s_orows.as<uint32_t>(); P.out_dist = c->s_odist.as<float>(); P.out_len = c->s_olen.as<uint32_t>(); P.status = c->fr_status.as<int32_t>();
     const size_t smem = frerank_smem(c->ld);
     static std::atomic<size_t> configured{0};
@@ -1674,7 +1674,7 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
               norms_kernel<<<g, 256, 0, c->stream>>>(cand, nc, c->dim, ld, c->x_cnorm.as<float>(), nullptr); CK(cudaGetLastError()); }
             c->x_ca.ensure(4ull * nc); c->x_cb.ensure(4ull * nc); c->x_gmax.ensure(4);
             CK(cudaMemsetAsync(c->x_gmax.p, 0, 4, c->stream));
-            xf_cand_prep_kernel<<<(nc + 255) / 256, 256, 0, c->stream>>>(c->x_cnorm.as<float>(), c->h0.as<float>(), c->s_rows.as<uint32_t>(), nc, c->metric,
+            xf_cand_prep_kernel<<<(nc + 255) / 256, 256, 0, c->stream>>>(c->x_cnorm.as<float>(), c->h0.as<float>(), c->s_rows.as<uint32_t>(), nc, c->metric, cos_header_min(c->dim),
                                                                          c->x_ca.as<float>(), c->x_cb.as<float>(), c->x_gmax.as<uint32_t>());
             CK(cudaGetLastError());
             c->n_launches += 2;

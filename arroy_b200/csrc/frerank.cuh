@@ -7,10 +7,36 @@
 // top-k, and re-scores only those from the fp32 rows in the reference's exact summation order — so
 // ids and distances stay bit-identical while the bytes per query drop ~1.9x.
 //
-//   shadow[c][i] = bf16_rn(item[c][i])  ->  | dot(q, shadow_c) - dot_ref(q, item_c) | <= rel |q| |c|,
-//   rel = 2^-9 (rounding of one operand) + d 2^-22 (fp32 accumulation, any order, and the reference's own
-//   rounding) with slack; the estimate a(q, c) of built_distance and E(q) follow xrerank.cuh
-//   (same formulas as the tensor-core pre-filter: TgEpilogue / xf_query_prep_kernel).
+//   shadow[c][i] = bf16_rn(item[c][i])  ->  | s - dot_ref(q, item_c) | <= rel (qn + sub) (gmax + sub),   s = phase 1's fp32 dot,
+//   rel = 1.0625 2^-8 + d 2^-22,   sub = sqrt(d + 64) 2^-74,   qn >= |q| and gmax >= |c| as computed in fp32.
+// The terms, with u = 2^-24 (fp32) and the bf16 rounding e_i = shadow_i - c_i:
+//   * bf16 keeps 8 significant bits: round to nearest even gives |e_i| <= 2^-8 |c_i| for |c_i| >= 2^-126 (an element just below
+//     the midpoint 1 + 2^-8 loses almost 2^-8 of itself), and |e_i| <= 2^-134 below it (the subnormal step is 2^-133), so
+//     |sum q_i e_i| <= 2^-8 |q| |c| + sqrt(d) 2^-134 |q|. The errors of all elements line up when the row's rounding
+//     directions follow the query's signs: tests/test_frerank_bound_cpu.py builds such rows and reaches 0.996 of 2^-8 |q| |c|.
+//   * fp32 accumulation of s: a product passes through at most d/8 + 11 roundings (its lane's FMA chain over the non-zero
+//     elements, then the xor 4, 2, 1 adds). The reference's dot_ref: at most d/32 + 37 (an AVX chain, hsum256, the three adds,
+//     a tail of up to 31 elements; SSE and scalar paths are shorter). Both sums run over |q_i| |c_i| (1 + 2^-8), so together
+//     they stay below (0.16 d + 48) u |q| |c| <= d 2^-22 |q| |c| for d >= 13, and below 4 d u by counting the non-zero terms
+//     for smaller d.
+//   * underflow: |q| (the kernel's qq) and |c| (norms_kernel) are fp32 sums of squares. A square below 2^-150 rounds to zero and
+//     each of the at most d + 40 roundings loses at most 2^-150 in the subnormal range, so |c| <= gmax + sqrt(d + 40) 2^-75 and
+//     |q| <= qn + sqrt(d + 40) 2^-75; `sub` is twice that. It also covers the subnormal term above, sqrt(d) 2^-134 |q| <=
+//     2^-8 sub |q|. Without it an index of rows whose squared norm underflows has gmax = 0 and an E far below its error.
+//     Cosine divides by the headers instead: gmax is cnorm / header, the ratio of two equal fp32 sums, so sub does not bound
+//     a row's |c| / header, which underflow makes unbounded (a row of one element 2^-72 and a tail of 2^-76 has header 2^-72
+//     and |c| = 2.2 2^-72 at d = 1024). A row whose header is at least cos_header_min(d) = sqrt(d + 64) 2^-70 (xrerank.cuh)
+//     loses at most 2^-10 of its squared norm, so |c| <= header (1 + 2^-11) (1 + small), inside the 1.0625 factor; a row
+//     below it gets an unknown estimate and always survives. The query's side is covered by qn + sub over its header.
+//   * the 1.0625 factor covers the roundings of the bound itself: qn = sqrt(qq) * 1.000001 and gmax (|c| by norms_kernel,
+//     Cosine |c| / header) are within (d/32 + 10) u of the true norms, and eps, e and 2e take a few more roundings and the
+//     1.001 factor; all of them are multiplicative, far below 2^-4.
+//   The estimate a(q, c) of built_distance and E(q) follow xrerank.cuh (same formulas as the tensor-core pre-filter:
+//   TgEpilogue / xf_query_prep_kernel), with eps = rel (qn + sub) (gmax + sub) + 1e-30: DotProduct E = eps; Euclidean
+//   E = 2 eps + (d/32 + 16) 2^-22 (|q|^2 + gmax^2) for the roundings of |q|^2, |c|^2 and the reference's own sum of squares;
+//   Cosine E = eps / (2 |q|) + 2^-19 for the roundings of the division and of the clamp formula (a row whose header is below
+//   cos_header_min(d) has an unknown estimate and always survives). For ordinary data sub vanishes next to the norms and eps
+//   is rel qn gmax.
 //
 // One CTA per query, everything in shared memory:
 //   1. estimates of all candidates (8 lanes per row, 16-byte loads of 8 bf16)
@@ -32,7 +58,8 @@ constexpr int FR_CAP = 8192;      // candidates per query held in shared memory
 constexpr int FR_SURV = 2048;     // survivors per query
 constexpr int FR_BINS = 2048;
 
-inline float fr_rel(uint32_t d) { return 0.00244140625f + (float)d * 2.384185791015625e-07f; }   // 1.25 * 2^-9 + d 2^-22
+inline float fr_rel(uint32_t d) { return 0.004150390625f + (float)d * 2.384185791015625e-07f; }   // 1.0625 * 2^-8 + d 2^-22
+inline float fr_sub(uint32_t d) { return sqrtf((float)d + 64.0f) * 5.293955920339377e-23f; }  // sqrt(d + 64) 2^-74
 
 // shadow copy: n x ld bf16, round to nearest even (padding stays zero)
 __global__ void fr_shadow_kernel(const float4* __restrict__ items, uint2* __restrict__ shadow, uint64_t total4) {
@@ -65,7 +92,7 @@ struct FrParams {
     uint32_t d, ld; int metric;
     const float* queries; const uint32_t* qrows; const float* qh0;                            // like distance_kernel
     const uint32_t* rows; const uint64_t* seg_beg; const uint64_t* seg_end;                   // sorted candidate rows per query
-    uint32_t k; float rel; const uint32_t* gmax_bits;
+    uint32_t k; float rel, sub, hmin; const uint32_t* gmax_bits;   // hmin: cos_header_min(d)
     uint32_t* out_rows; float* out_dist; uint32_t* out_len; int32_t* status;
 };
 
@@ -108,7 +135,7 @@ frerank_kernel(FrParams P) {
     for (int i = 0; i < FR_THREADS / 32; ++i) qq += sm_f[i];
     const float qn = sqrtf(qq) * 1.000001f;
     const float gmax = __uint_as_float(*P.gmax_bits);
-    const float eps = fmaf(P.rel, qn * gmax, 1e-30f);
+    const float eps = fmaf(P.rel, (qn + P.sub) * (gmax + P.sub), 1e-30f);
     float qa = 0.f, e;
     if (metric == DOT_PRODUCT) e = eps;
     else if (metric == EUCLIDEAN) { qa = qq; e = fmaf(((float)(P.d / 32u) + 16.0f) * 2.384185791015625e-07f, qq + gmax * gmax, 2.0f * eps); }
@@ -143,7 +170,7 @@ frerank_kernel(FrParams P) {
                 const float ch = P.ih0[r];
                 const float pnqn = __fmul_rn(qh, ch);
                 if (pnqn > 1.1920928955078125e-07f) {
-                    float cs = ch >= 1e-30f ? acc * (qa * (1.0f / ch)) : __uint_as_float(0x7fc00000u);
+                    float cs = ch >= P.hmin ? acc * (qa * (1.0f / ch)) : __uint_as_float(0x7fc00000u);
                     cs = cs < -1.0f ? -1.0f : (cs > 1.0f ? 1.0f : cs);
                     a = 0.5f * (1.0f - cs);
                 } else a = pnqn == pnqn ? 0.0f : pnqn;

@@ -209,7 +209,10 @@ topk_dense_kernel(const float* __restrict__ dist, const uint32_t* __restrict__ r
 // operands truncated to TF32 (10-bit mantissa) and FP32 accumulation the contraction s satisfies
 //     | s - dot_ref(q, c) |  <=  rel * |q| * |c|,      rel = 2^-8 + d * 2^-22
 // (Cauchy-Schwarz over the per-element relative errors 2 * 2^-10, the accumulation error, and the
-// reference's own FP32 rounding of dot_ref; about 2x slack). tcgemm.cuh turns s into an estimate
+// reference's own FP32 rounding of dot_ref; about 2x slack). E(q) charges rel (qn + sub) (gmax + sub),
+// sub = sqrt(d + 64) 2^-74: the fp32 norms qn and gmax may have underflowed (frerank.cuh derives sub),
+// and sub also covers operands below 2^-126, which the conversion may flush to zero (a loss of at most
+// sqrt(d) 2^-126 (|q| + |c|) over the row, far below 2^-8 sub (|q| + |c|)). tcgemm.cuh turns s into an estimate
 // a(q, c) of built_distance in its epilogue; for a query q every pair then satisfies
 //     | a(q, c) - built_distance_ref(q, c) |  <=  E(q)
 // where E(q) uses the largest candidate norm (xf_query_prep_kernel). Let a_(k) be the k-th smallest
@@ -226,6 +229,10 @@ constexpr int XF_STAGE = 2048;
 constexpr uint32_t XF_SAMPLE = 4;
 
 inline float xf_rel(uint32_t d) { return 0.00390625f + (float)d * 2.384185791015625e-07f; }   // 2^-8 + d 2^-22
+// Cosine: the smallest header norm whose row gets a known estimate. A row's fp32 sum of squares may lose up to (d + 40) 2^-150
+// to underflow, so its true |c| can be many times its header; from sqrt(d + 64) 2^-70 on, |c| <= header (1 + 2^-11) (1 + small).
+// Rows below it have an unknown estimate (NaN) and always survive; the reference still sees pnqn > EPSILON for them.
+inline float cos_header_min(uint32_t d) { return sqrtf((float)d + 64.0f) * 8.470329472543003e-22f; }   // sqrt(d + 64) 2^-70
 
 // dst[c] = items[rows[c]] (ld floats per row), float4 granularity
 __global__ void xf_gather_kernel(float4* __restrict__ dst, const float4* __restrict__ items, const uint32_t* __restrict__ rows, uint32_t nc, uint32_t ld4) {
@@ -239,7 +246,7 @@ __global__ void xf_gather_kernel(float4* __restrict__ dst, const float4* __restr
 // per-candidate epilogue constants (see TgEpilogue) and gmax = max over candidates of the factor
 // the error bound grows with: |c| (Euclidean, DotProduct) or |c| / header norm (Cosine, normally 1)
 __global__ void xf_cand_prep_kernel(const float* __restrict__ cnorm, const float* __restrict__ ih0, const uint32_t* __restrict__ rows, uint32_t nc, int metric,
-                                    float* __restrict__ ca, float* __restrict__ cb, uint32_t* __restrict__ gmax_bits) {
+                                    float hmin, float* __restrict__ ca, float* __restrict__ cb, uint32_t* __restrict__ gmax_bits) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     float g = 0.f;
     if (i < nc) {
@@ -249,8 +256,8 @@ __global__ void xf_cand_prep_kernel(const float* __restrict__ cnorm, const float
         if (metric == EUCLIDEAN) a = __fmul_rn(cn, cn);
         else if (metric == COSINE) {
             b = ih0[rows[i]];
-            if (b >= 1e-30f) { a = __fdiv_rn(1.0f, b); g = __fmul_rn(cn, a); }
-            else { a = __uint_as_float(0x7fc00000u); g = 0.f; }   // only reachable when pnqn <= EPSILON (estimate exactly 0) or the pair is unknown
+            if (b >= hmin) { a = __fdiv_rn(1.0f, b); g = __fmul_rn(cn, a); }   // hmin = cos_header_min(d)
+            else { a = __uint_as_float(0x7fc00000u); g = 0.f; }   // the estimate is exactly 0 (pnqn <= EPSILON) or unknown
         }
         ca[i] = a; cb[i] = b;
         if (!(g == g)) g = __uint_as_float(0x7f800000u);
@@ -266,7 +273,8 @@ __global__ void xf_query_prep_kernel(const float* __restrict__ qnorm, const floa
     uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= m) return;
     const float qn = qnorm[q], gmax = __uint_as_float(*gmax_bits);
-    const float eps = __fmaf_rn(rel, __fmul_rn(qn, gmax), 1e-30f);
+    const float sub = __fmul_rn(sqrtf((float)d + 64.0f), 5.293955920339377e-23f);   // sqrt(d + 64) 2^-74: underflowed norms, flushed operands
+    const float eps = __fmaf_rn(rel, __fmul_rn(__fadd_rn(qn, sub), __fadd_rn(gmax, sub)), 1e-30f);
     float a = 0.f, b = 0.f, e;
     if (metric == DOT_PRODUCT) e = eps;
     else if (metric == EUCLIDEAN) {

@@ -1,10 +1,12 @@
 """Fused re-rank (bf16 shadow pre-filter + exact re-score, frerank.cuh) must return exactly what the
-plain distance + top-k kernels and the oracle (reader.rs:381-399) return."""
+plain distance + top-k kernels and the oracle (reader.rs:381-399) return, also on rows built to put the bf16 rounding at its
+worst, and through the filtered searches that use it."""
 import numpy as np
 import pytest
 
 import arroy_b200 as ab
 import oracle
+from helpers import ADVERSARIAL_KINDS, adversarial_set
 
 pytestmark = pytest.mark.gpu
 SEED = bytes([42] * 32)
@@ -73,3 +75,98 @@ def test_fused_rerank_with_ties_and_degenerate_rows(ctx, monkeypatch):
         ctx.stage_items_flat(metric, np.arange(n, dtype=np.uint32), data)
         qh = np.sqrt((q.astype(np.float64) ** 2).sum(1)).astype(np.float32) if metric == "cosine" else None
         _both(ctx, monkeypatch, q, qh, lists, 50)   # too many survivors -> falls back inside, results still identical
+
+
+ADV_DIMS = [20, 32, 33, 64, 96, 100, 200, 768, 1536, 4096]   # 20: d < 32; 32, 96, 200: a trailing 32-element chunk (ld % 64 == 32)
+
+
+def _adversarial_matrix(kind, metric, d, n_random=2000):
+    """the adversarial set of helpers.adversarial_set in rows 0 .. nc-1, then random rows no longer than its shortest row, so
+    the largest norm of the staged items (gmax) is the construction's"""
+    q, adv = adversarial_set(kind, metric, d, seed=d)
+    rng = np.random.default_rng(d + 1)
+    fill = rng.standard_normal((n_random, d))
+    shortest = np.linalg.norm(adv.astype(np.float64), axis=1).min()
+    fill *= rng.uniform(0.2, 0.95, (n_random, 1)) * shortest / np.linalg.norm(fill, axis=1, keepdims=True)
+    return q, adv.shape[0], np.concatenate([adv, fill.astype(np.float32)])
+
+
+def _cos_header(v):
+    return oracle.new_header(oracle.COSINE, v)[0]
+
+
+@pytest.mark.parametrize("d", ADV_DIMS)
+@pytest.mark.parametrize("metric", ["euclidean", "cosine", "dot-product"])
+def test_fused_rerank_on_adversarial_rows(ctx, monkeypatch, metric, d):
+    # rows whose bf16 rounding errors all line up with the query (tests/test_frerank_bound_cpu.py restates the kernel's rule on
+    # them): A is the true nearest row and its shadow looks farther than the k rows B. The fused kernel must keep A, with no
+    # fallback, and return what the plain kernels and the oracle return; random queries share the batch.
+    m = oracle.METRICS[metric]
+    for kind in ADVERSARIAL_KINDS:
+        q, nc, data = _adversarial_matrix(kind, metric, d)
+        n = data.shape[0]
+        ctx.stage_items_flat(metric, np.arange(n, dtype=np.uint32), data)
+        hdr = np.array([_cos_header(r) for r in data], np.float32) if metric == "cosine" else np.zeros(n, np.float32)
+        rng = np.random.default_rng(d + 2)
+        rq = (rng.standard_normal((2, d)) * (np.linalg.norm(q.astype(np.float64)) / np.sqrt(d))).astype(np.float32)
+        queries = np.concatenate([q[None, :], rq])
+        qh = np.array([_cos_header(v) for v in queries], np.float32) if metric == "cosine" else None
+        lists = [np.arange(nc)] + [np.sort(rng.choice(n, 1500, replace=False)) for _ in range(2)]
+        for k in (1, 10, nc - 1):
+            (rows, dist, lens), fallbacks = _both(ctx, monkeypatch, queries, qh, lists, k)
+            assert fallbacks == 0, (kind, k)
+            for i in range(queries.shape[0]):
+                wr, wd = oracle.rerank(m, queries[i], (float(qh[i]) if qh is not None else 0.0, 0.0), data, hdr, None,
+                                       lists[i].astype(np.uint32), k)
+                assert rows[i, :lens[i]].tolist() == wr.tolist() and dist[i, :lens[i]].tobytes() == wd.tobytes(), (kind, k, i)
+
+
+def _env(ctx):
+    e = ab.Env(0)
+    e._ctx = ctx
+    return e
+
+
+@pytest.mark.parametrize("metric,d", [("dot-product", 33), ("euclidean", 200), ("cosine", 768), ("dot-product", 768)])
+def test_adversarial_rows_through_filtered_queries(ctx, monkeypatch, metric, d):
+    # the same sets through QueryBuilder::candidates: a filter of exactly {A, B_1 .. B_k} (the small-filter shortcut, or a
+    # walk with search_k below the filter's rows in the forest), single queries and batches (walk1_kernel, walk_kernel), one
+    # shared filter and one filter per query, against the oracle's Reader
+    n_trees, count = 8, 10
+    q, nc, data = _adversarial_matrix("ones", metric, d)
+    n = data.shape[0]
+    ids = np.arange(n, dtype=np.uint32)
+    odb = oracle.Db(metric, d)
+    odb.set_items(ids, data)
+    odb.build(oracle.StdRng(SEED), n_trees=n_trees, threads=8)
+    env = _env(ctx)
+    try:
+        w = ab.Writer(env, 0, d, metric)
+        w.add_items(ids, data)
+        w.builder(ab.StdRng.from_seed(SEED)).n_trees(n_trees).build()
+        r = ab.Reader.open(env, 0, metric)
+        F = list(range(nc))
+        rng = np.random.default_rng(4)
+        G = np.sort(rng.choice(n, 40, replace=False)).tolist()
+        c0 = ctx.counters()
+        for sk in (None, 2**64 - 1, 30):
+            got = r.nns(count).search_k(sk).candidates(F).by_vector(q) if sk else r.nns(count).candidates(F).by_vector(q)
+            want = odb.nns_by_vector(q, count, search_k=sk, candidates=F)
+            assert sk == 30 or want[0][0] == 0            # every row of the filter is a candidate: A comes first
+            assert got == want, sk
+            for nq in (3, 40):
+                vecs = np.repeat(q[None, :], nq, axis=0)
+                vecs[1::2] = (rng.standard_normal((nq // 2, d)) * np.abs(q).mean()).astype(np.float32)
+                bi, bd, bl, _ = r.nns_batch_by_vector(vecs, count, search_k=sk, candidates=F)
+                fq = np.arange(nq) % 2
+                mi, md, ml, _ = r.nns_batch_by_vector(vecs, count, search_k=sk, filters=[F, G], filter_of_query=fq)
+                for i in range(nq):
+                    wv = odb.nns_by_vector(vecs[i], count, search_k=sk, candidates=F)
+                    assert list(zip(bi[i, :bl[i]].tolist(), bd[i, :bl[i]].tolist())) == wv, (sk, nq, i)
+                    wm = wv if fq[i] == 0 else odb.nns_by_vector(vecs[i], count, search_k=sk, candidates=G)
+                    assert list(zip(mi[i, :ml[i]].tolist(), md[i, :ml[i]].tolist())) == wm, (sk, nq, i)
+        c1 = ctx.counters()
+        assert c1["fused_rerank_batches"] > c0["fused_rerank_batches"]
+        assert c1["fused_rerank_fallbacks"] == c0["fused_rerank_fallbacks"]
+    finally:
+        env._ctx = None
