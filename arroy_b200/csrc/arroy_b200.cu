@@ -71,9 +71,9 @@ struct PinBuf {
 };
 
 struct Wave {  // device buffers of one wave of trees; kept across builds
-    DevBuf st, frames, recs, perm0, perm1, flags, unit_left, pool, pool_counter, jobs, scratch, active, error, final_ids, keys, sub_rows, sub_off, timing, slots, abort, cur_normal, start_pos, root, shadow_stats;
+    DevBuf st, frames, recs, perm0, perm1, flags, unit_left, pool, pool_counter, jobs, scratch, active, error, final_ids, keys, sub_rows, sub_off, slots, abort, cur_normal, start_pos, root, shadow_stats;
     void release() {
-        sub_rows.release(); sub_off.release(); timing.release(); slots.release(); abort.release(); cur_normal.release(); start_pos.release(); root.release(); shadow_stats.release();
+        sub_rows.release(); sub_off.release(); slots.release(); abort.release(); cur_normal.release(); start_pos.release(); root.release(); shadow_stats.release();
         st.release(); frames.release(); recs.release(); perm0.release(); perm1.release(); flags.release(); unit_left.release();
         pool.release(); pool_counter.release(); jobs.release(); scratch.release(); active.release(); error.release(); final_ids.release(); keys.release();
     }
@@ -192,7 +192,7 @@ void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
         CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         configured = smem;
     }
-    work_kernel<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric, 0);
+    work_kernel<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric);
     CK(cudaGetLastError());
     c->n_launches += 1;
 }
@@ -246,12 +246,9 @@ template <class RowSrc>
 void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t ld, RowSrc row_src, float* dst_override = nullptr, size_t chunk_mb_override = 0, bool count_bytes = true,
                          int mode = 0, uint32_t src_dim = 0) {
     if (n == 0) return;
-    unsigned W = 8;   // 8 lanes x 4 MB chunks: decode of one chunk overlaps the PCIe copies of the others
-    if (const char* e = getenv("ARROY_B200_STAGE_THREADS")) W = (unsigned)std::max(1, atoi(e));
-    W = std::max(1u, std::min(W, std::max(1u, std::thread::hardware_concurrency())));
-    size_t chunk_mb = 4;
-    if (const char* e = getenv("ARROY_B200_STAGE_CHUNK_MB")) chunk_mb = (size_t)std::max(1, atoi(e));
-    if (chunk_mb_override) chunk_mb = chunk_mb_override;
+    // 8 lanes x 4 MB chunks: decode of one chunk overlaps the PCIe copies of the others
+    unsigned W = std::min(8u, std::max(1u, std::thread::hardware_concurrency()));
+    const size_t chunk_mb = chunk_mb_override ? chunk_mb_override : 4;
     const uint64_t chunk_rows = std::max<uint64_t>(1, (chunk_mb << 20) / ((size_t)ld * 4));
     const uint64_t n_chunks = (n + chunk_rows - 1) / chunk_rows;
     W = (unsigned)std::min<uint64_t>(W, n_chunks);
@@ -424,8 +421,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     size_t ws_bytes = (size_t)WS_VECS * ld * 4;
     int use_smem = ws_bytes <= 200 * 1024 ? 1 : 0;
     if (!use_smem) W.scratch.ensure(ws_bytes * tw);
-    // speculative two_means (build.cuh): needs the 24-vector workspace in shared memory; ARROY_B200_SPEC=0 keeps the sequential loop
-    const int spec = (use_smem && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024 && !(getenv("ARROY_B200_SPEC") && atoi(getenv("ARROY_B200_SPEC")) == 0)) ? 1 : 0;
+    // speculative two_means (build.cuh): needs the 24-vector workspace in shared memory
+    const int spec = (use_smem && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024) ? 1 : 0;
     if (spec) ws_bytes = (size_t)WS_VECS_SPEC * ld * 4;
 
     BuildParams P{};
@@ -439,11 +436,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     P.active = W.active.as<uint32_t>(); P.error = W.error.as<int32_t>();
     P.sub_rows = nullptr; P.sub_off = nullptr;
     // cluster-resident nodes: up to ~6 MB of item rows per scan (2048 rows at d = 768, every node of a 10k x 64 index)
-    P.lat_mask = getenv("ARROY_B200_LATMASK") ? (uint32_t)atoi(getenv("ARROY_B200_LATMASK")) : 3u;
-    P.small_max = getenv("ARROY_B200_SMALL_MAX") ? (uint32_t)atoi(getenv("ARROY_B200_SMALL_MAX")) : (uint32_t)std::max<uint64_t>(2048, (6ull << 20) / (4ull * ld));
+    P.small_max = (uint32_t)std::max<uint64_t>(2048, (6ull << 20) / (4ull * ld));
     P.max_inner = 1024u;   // attempts per launch; `cancel` is polled between launches
-    P.timing = nullptr;
-    if (getenv("ARROY_B200_CTRL_TIMING")) { W.timing.ensure(24 * 8); CK(cudaMemsetAsync(W.timing.p, 0, 24 * 8, c->stream)); P.timing = W.timing.as<unsigned long long>(); }
     if (sub.rows) {   // this wave's subsets, offsets rebased to the wave
         const uint64_t b = sub.off[t0], e = sub.off[t0 + tw];
         std::vector<uint64_t> off(tw + 1);
@@ -484,50 +478,39 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     if (wsmem + perm_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + perm_smem)));
     const int work_grid = c->sm_count * 3;
 
-    // Two schedules over the same kernels:
-    //  * async (default): every tree is its own chain control -> work -> control -> ... on its own
-    //    stream; all chains of the wave are branches of ONE CUDA graph, so the two_means latency of
-    //    one tree overlaps the scans of the others (trees only share the read-only item matrix).
-    //  * lockstep (ARROY_B200_LOCKSTEP=1, also used by ARROY_B200_PROFILE=1): one control launch
-    //    for all trees, then one work launch for all posted jobs; every kernel runs alone, which is
-    //    what the per-launch roofline measurement needs.
+    // Three schedules over the same kernels:
+    //  * persistent (below): one cooperative launch for the whole wave.
+    //  * async: every tree is its own chain control -> work -> control -> ... on its own stream; all chains of the wave are
+    //    branches of ONE CUDA graph of ASYNC_BATCH steps each, so the two_means latency of one tree overlaps the scans of the
+    //    others (trees only share the read-only item matrix).
+    //  * lockstep (ARROY_B200_LOCKSTEP=1, also used by ARROY_B200_PROFILE=1): one control launch for all trees, then one work
+    //    launch for all posted jobs, launched directly; every kernel runs alone, which is what the per-launch roofline
+    //    measurement needs. It is the reference the other two schedules are tested against.
+    constexpr int ASYNC_BATCH = 64, LOCKSTEP_BATCH = 32;   // steps per graph launch / per batch of direct launches
     const bool profile = getenv("ARROY_B200_PROFILE") != nullptr && atoi(getenv("ARROY_B200_PROFILE")) != 0;
     const bool lockstep = profile || (getenv("ARROY_B200_LOCKSTEP") != nullptr && atoi(getenv("ARROY_B200_LOCKSTEP")) != 0);
-    const bool use_graph = getenv("ARROY_B200_NO_GRAPH") == nullptr && !profile;
-    const int steps_per_batch = lockstep ? 32 : (getenv("ARROY_B200_BATCH") ? std::max(1, atoi(getenv("ARROY_B200_BATCH"))) : 64);
-    const int tree_grid = c->sm_count;  // work CTAs per tree launch in async mode
-    const int interleave = (getenv("ARROY_B200_INTERLEAVE") != nullptr && atoi(getenv("ARROY_B200_INTERLEAVE")) != 0) ? 1 : 0;
-    const size_t wsmem1 = work_smem(ld, 1);
-    // Few trees on this GPU = the chain of attempts of each tree is the critical path: run the control
-    // kernel as a thread-block cluster that scans small nodes itself (build.cuh). ARROY_B200_CLUSTER = 0 | 8 | 16.
-    int cluster = 1;
-    if (!lockstep && use_smem) {
-        const char* e = getenv("ARROY_B200_CLUSTER");
-        if (e) { int v = atoi(e); cluster = (v == 8 || v == 16) ? v : 1; }
-        // measured: d = 64, 1-10 trees: 24 -> 20 us per attempt; d = 768: 38 -> 37 us for one tree but slower from ~6 trees on
-        else if (c->dim <= 256) cluster = tw <= 8 ? 16 : (tw <= 16 ? 8 : 1);
-        if (is_bq(c->metric)) cluster = 1;
-    }
-    if (cluster > 1) {
-        CK(cudaFuncSetAttribute(control_fn(true, cluster, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
-        if (cluster == 16) CK(cudaFuncSetAttribute(control_fn(true, 16, c->metric), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    }
+    const int steps_per_batch = lockstep ? LOCKSTEP_BATCH : ASYNC_BATCH;
     const void* ctrl1 = control_fn(use_smem != 0, 1, c->metric);
+    // Few trees on this GPU = the chain of attempts of each tree is the critical path: the async schedule runs the control kernel
+    // as a thread-block cluster that scans small nodes itself (build.cuh control_kernel<.., CS = 8 | 16>).
+    // measured: d = 64, 1-10 trees: 24 -> 20 us per attempt; d = 768: 38 -> 37 us for one tree but slower from ~6 trees on
+    const int cluster = (!lockstep && use_smem && c->dim <= 256 && !is_bq(c->metric)) ? (tw <= 8 ? 16 : (tw <= 16 ? 8 : 1)) : 1;
     const void* ctrlc = control_fn(use_smem != 0, cluster, c->metric);
+    if (cluster > 1) {
+        CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
+        if (cluster == 16) CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    }
 
     // Persistent schedule (default): ONE cooperative launch per wave — a control CTA per tree plus worker CTAs on every SM
-    // (build.cuh control_kernel<.., CS = 0>). Needs two CTAs per SM to have enough workers next to the control CTAs; with a big
-    // workspace (d > 1152) that means giving up the speculative two_means. ARROY_B200_PERSIST=0 keeps the per-attempt launches.
+    // (build.cuh control_kernel<.., CS = 0>). Needs two CTAs per SM to have enough workers next to the control CTAs; with
+    // a big workspace (d > 1152) that means giving up the speculative two_means.
     bool persist = false;
     int pgrid = 0;
     size_t psmem = ctrl_smem;
     const void* ctrlp = nullptr;
     // It wins where the chain of attempts is the critical path (few trees per GPU, small indexes); a wave that is bandwidth-bound
     // from start to end (10M x 100 trees) runs a little faster on work_kernel's three scanning CTAs per SM.
-    // ARROY_B200_PERSIST = 0 | 1 overrides the choice.
-    const char* pe = getenv("ARROY_B200_PERSIST");
-    const bool pwant = pe ? atoi(pe) != 0 : (double)n * (double)tw <= 2.0e8;
-    if (pwant && !lockstep && use_smem && ld <= 8u * CTRL_THREADS && n < (1ull << 29)) {
+    if ((double)n * (double)tw <= 2.0e8 && !lockstep && use_smem && ld <= 8u * CTRL_THREADS && n < (1ull << 29)) {
         ctrlp = control_fn(true, 0, c->metric);
         const size_t cand[2] = {ctrl_smem, (size_t)WS_VECS * ld * 4};
         for (int k = 0; k < 2 && !persist; ++k) {
@@ -537,26 +520,18 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ctrlp, CTRL_THREADS, cand[k]));
             const int cap = nb * c->sm_count;
             if ((nb >= 2 || k == 1) && cap >= (int)tw + std::max(16, c->sm_count / 2)) { persist = true; pgrid = cap; psmem = cand[k]; if (k == 1) P.spec = 0; }
-            if (persist) if (const char* ge = getenv("ARROY_B200_PGRID")) pgrid = std::max((int)tw + 16, std::min(pgrid, atoi(ge)));   // experiments: fewer resident CTAs
         }
     }
     // scans through the 8-bit planes of the items (kernels.cuh scan_claim_planes): nodes of more than shadow_min_units units
-    {
-        const char* se = getenv("ARROY_B200_SHADOW");
-        const bool want = !(se && atoi(se) == 0) && !is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && n * (uint64_t)ld >= (1ull << 22);
-        if (want) {
-            planes_prepare(c);
-            P.planes = PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()};
-            W.shadow_stats.ensure(24);
-            CK(cudaMemsetAsync(W.shadow_stats.p, 0, 24, c->stream));
-            P.shadow_stats = W.shadow_stats.as<unsigned long long>();
-            // many trees per GPU: bandwidth decides, every node goes through the shadow; few: the chain of attempts decides and
-            // small nodes keep the one-unit claims of the exact scan (more CTAs per node)
-            P.shadow_min_units = getenv("ARROY_B200_SHADOW_MIN") ? (uint32_t)atoi(getenv("ARROY_B200_SHADOW_MIN")) : ((!persist || tw >= 32) ? 12u : (tw >= 12 ? 64u : 128u));
-            P.shadow_small_chunk = getenv("ARROY_B200_SHADOW_CHUNK") ? (uint32_t)std::min(4, std::max(1, atoi(getenv("ARROY_B200_SHADOW_CHUNK")))) : 4u;
-            P.shadow_big_units = getenv("ARROY_B200_SHADOW_BIG") ? (uint32_t)atoi(getenv("ARROY_B200_SHADOW_BIG")) : 512u;
-            P.shadow_big_chunk = getenv("ARROY_B200_SHADOW_BIGCHUNK") ? (uint32_t)std::max(4, atoi(getenv("ARROY_B200_SHADOW_BIGCHUNK"))) : 8u;
-        }
+    if (!is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && n * (uint64_t)ld >= (1ull << 22)) {
+        planes_prepare(c);
+        P.planes = PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()};
+        W.shadow_stats.ensure(24);
+        CK(cudaMemsetAsync(W.shadow_stats.p, 0, 24, c->stream));
+        P.shadow_stats = W.shadow_stats.as<unsigned long long>();
+        // many trees per GPU: bandwidth decides, every node goes through the shadow; few: the chain of attempts decides and
+        // small nodes keep the one-unit claims of the exact scan (more CTAs per node)
+        P.shadow_min_units = (!persist || tw >= 32) ? 12u : (tw >= 12 ? 64u : 128u);
     }
     if (persist) {
         W.slots.ensure(sizeof(PSlot) * tw);
@@ -569,57 +544,44 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         P.abort = W.abort.as<int>();
         // fused root scan: every tree of the wave starts at the root of the whole index (no subtree mode), rows go through the
         // 8-lanes-per-row path, and a batch of normals fits next to nothing else in the workers' shared memory
-        const char* rf = getenv("ARROY_B200_ROOT_FUSE");
-        P.root_fused = (!sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem && !(rf && atoi(rf) == 0)) ? 1 : 0;
+        P.root_fused = (!sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem) ? 1 : 0;
         W.root.ensure(8);
         CK(cudaMemsetAsync(W.root.p, 0, 8, c->stream));
         P.root_ready = W.root.as<uint32_t>(); P.root_ticket = W.root.as<uint32_t>() + 1;
     }
 
-    auto launch_step = [&](cudaStream_t s) {  // lockstep: all trees per launch
-        launch_control(ctrl1, tw, 1, ctrl_smem, s, P, 0u);
-        if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + perm_smem, s>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-        else work_kernel<<<work_grid, WORK_THREADS, wsmem, s>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric, interleave);
-    };
-    auto launch_tree_step = [&](uint32_t t, cudaStream_t s) {  // async: one tree per launch
-        launch_control(ctrlc, 1, cluster, ctrl_smem, s, P, t);
-        if (P.planes.hi) work_kernel_shadow<<<tree_grid, WORK_THREADS, wsmem1 + perm_smem, s>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-        else work_kernel<<<tree_grid, WORK_THREADS, wsmem1, s>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric, 0);
-    };
-    if (!lockstep) {
-        while (c->tree_streams.size() < tw) { cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); c->tree_streams.push_back(st); }
-        while (c->tree_events.size() < (size_t)tw + 1) { cudaEvent_t ev; CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); c->tree_events.push_back(ev); }
-    }
-
     CK(cudaStreamSynchronize(c->stream));
     c->breakdown[0] += ms_since(t_setup);
     auto t_graph = std::chrono::steady_clock::now();
-    // The captured graph only depends on the kernel arguments (BuildParams: buffer pointers are
-    // stable because the wave buffers live in the context) and the schedule, so it is reused by
-    // later builds with the same shapes.
+    // The async schedule's graph only depends on the kernel arguments (BuildParams: buffer pointers are stable because the wave
+    // buffers live in the context), the wave's size and the cluster size, so it is reused by later builds with the same shapes.
     cudaGraphExec_t gexec = nullptr;
-    if (use_graph && !persist) {
-        std::vector<uint8_t> key(sizeof(BuildParams) + 16);
+    if (!persist && !lockstep) {
+        std::vector<uint8_t> key(sizeof(BuildParams) + 12);
         memcpy(key.data(), &P, sizeof(BuildParams));
-        int32_t sched[4] = {(lockstep ? 1 : 0) | (interleave << 1) | (cluster << 8), steps_per_batch, (int32_t)tw, (int32_t)ctrl_smem};
-        memcpy(key.data() + sizeof(BuildParams), sched, 16);
+        const int32_t shape[3] = {(int32_t)tw, (int32_t)ctrl_smem, cluster};
+        memcpy(key.data() + sizeof(BuildParams), shape, 12);
         if (c->cached_exec && key == c->cached_graph_key) gexec = c->cached_exec;
         else {
             if (c->cached_exec) { cudaGraphExecDestroy(c->cached_exec); c->cached_exec = nullptr; }
             if (c->cached_graph) { cudaGraphDestroy(c->cached_graph); c->cached_graph = nullptr; }
             c->cached_graph_key.clear();
+            while (c->tree_streams.size() < tw) { cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); c->tree_streams.push_back(st); }
+            while (c->tree_events.size() < (size_t)tw + 1) { cudaEvent_t ev; CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); c->tree_events.push_back(ev); }
+            const size_t wsmem1 = work_smem(ld, 1);
             cudaGraph_t graph = nullptr;
             CK(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-            if (lockstep) { for (int i = 0; i < steps_per_batch; ++i) launch_step(c->stream); }
-            else {
-                CK(cudaEventRecord(c->tree_events[0], c->stream));
-                for (uint32_t t = 0; t < tw; ++t) {
-                    cudaStream_t st = c->tree_streams[t];
-                    CK(cudaStreamWaitEvent(st, c->tree_events[0], 0));
-                    for (int i = 0; i < steps_per_batch; ++i) launch_tree_step(t, st);
-                    CK(cudaEventRecord(c->tree_events[1 + t], st));
-                    CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
+            CK(cudaEventRecord(c->tree_events[0], c->stream));
+            for (uint32_t t = 0; t < tw; ++t) {   // one tree (one cluster) per control launch, sm_count work CTAs per work launch
+                cudaStream_t st = c->tree_streams[t];
+                CK(cudaStreamWaitEvent(st, c->tree_events[0], 0));
+                for (int i = 0; i < ASYNC_BATCH; ++i) {
+                    launch_control(ctrlc, 1, cluster, ctrl_smem, st, P, t);
+                    if (P.planes.hi) work_kernel_shadow<<<c->sm_count, WORK_THREADS, wsmem1 + perm_smem, st>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+                    else work_kernel<<<c->sm_count, WORK_THREADS, wsmem1, st>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric);
                 }
+                CK(cudaEventRecord(c->tree_events[1 + t], st));
+                CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
             }
             CK(cudaStreamEndCapture(c->stream, &graph));
             c->cached_graph = graph;
@@ -636,7 +598,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     volatile int32_t* h_error = reinterpret_cast<volatile int32_t*>(c->pin.as<uint32_t>() + 1);
     std::vector<cudaEvent_t> pev;
     struct EvGuard { std::vector<cudaEvent_t>& v; ~EvGuard() { for (auto e : v) cudaEventDestroy(e); } } evg{pev};
-    if (profile) { pev.resize(2 * steps_per_batch); for (auto& e : pev) CK(cudaEventCreate(&e)); }
+    if (profile) { pev.resize(2 * LOCKSTEP_BATCH); for (auto& e : pev) CK(cudaEventCreate(&e)); }
     uint64_t steps = 0;
     // safety net against a stuck state machine (never hit by a correct build): every step each
     // live tree completes one attempt or one partition
@@ -683,32 +645,23 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     } else
     for (;;) {
         if (steps > max_steps) throw std::runtime_error("forest build did not converge (internal state machine error)");
-        if (use_graph) CK(cudaGraphLaunch(gexec, c->stream));
-        else if (profile) {
-            for (int i = 0; i < steps_per_batch; ++i) {
+        if (!lockstep) CK(cudaGraphLaunch(gexec, c->stream));
+        else {   // all trees per launch; with `profile`, each work launch is timed by a pair of events
+            for (int i = 0; i < LOCKSTEP_BATCH; ++i) {
                 launch_control(ctrl1, tw, 1, ctrl_smem, c->stream, P, 0u);
-                CK(cudaEventRecord(pev[2 * i], c->stream));
+                if (profile) CK(cudaEventRecord(pev[2 * i], c->stream));
                 if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + perm_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-                else work_kernel<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric, interleave);
-                CK(cudaEventRecord(pev[2 * i + 1], c->stream));
-            }
-            CK(cudaStreamSynchronize(c->stream));
-            for (int i = 0; i < steps_per_batch; ++i) {
-                float ms = 0; CK(cudaEventElapsedTime(&ms, pev[2 * i], pev[2 * i + 1])); c->stats[5] += ms;
-                if (getenv("ARROY_B200_TRACE") && steps + i < 48) fprintf(stderr, "[trace] step %llu work_kernel %.3f ms\n", (unsigned long long)(steps + i), ms);
-            }
-        }
-        else if (lockstep) { for (int i = 0; i < steps_per_batch; ++i) launch_step(c->stream); CK(cudaGetLastError()); }
-        else {  // async without a graph (debugging): fork / join by events
-            CK(cudaEventRecord(c->tree_events[0], c->stream));
-            for (uint32_t t = 0; t < tw; ++t) {
-                cudaStream_t st = c->tree_streams[t];
-                CK(cudaStreamWaitEvent(st, c->tree_events[0], 0));
-                for (int i = 0; i < steps_per_batch; ++i) launch_tree_step(t, st);
-                CK(cudaEventRecord(c->tree_events[1 + t], st));
-                CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
+                else work_kernel<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric);
+                if (profile) CK(cudaEventRecord(pev[2 * i + 1], c->stream));
             }
             CK(cudaGetLastError());
+            if (profile) {
+                CK(cudaStreamSynchronize(c->stream));
+                for (int i = 0; i < LOCKSTEP_BATCH; ++i) {
+                    float ms = 0; CK(cudaEventElapsedTime(&ms, pev[2 * i], pev[2 * i + 1])); c->stats[5] += ms;
+                    if (getenv("ARROY_B200_TRACE") && steps + i < 48) fprintf(stderr, "[trace] step %llu work_kernel %.3f ms\n", (unsigned long long)(steps + i), ms);
+                }
+            }
         }
         steps += steps_per_batch;
         c->n_launches += 2ull * steps_per_batch * (lockstep ? 1 : tw);
@@ -724,15 +677,6 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     }
     c->stats[1] += (double)steps;
     c->breakdown[2] += ms_since(t_loop);
-    if (P.timing) {
-        unsigned long long tv[24]; CK(cudaMemcpy(tv, P.timing, sizeof(tv), cudaMemcpyDeviceToHost));
-        const char* nm[20] = {"decide", "rng", "gather", "norms", "two_means_rest", "finish_split", "cluster_scan", "prefix", "partition", "attempts", "inner", "total", "tm_dot_rest", "tm_update", "tm_dots", "tm_finish", "tm_recurrence", "publish_fence", "recur_it0", "recur_it1_9"};
-        const double att = (double)std::max<unsigned long long>(tv[9], 1);
-        fprintf(stderr, "[ctrl timing] attempts %llu, in-cluster %llu; cycles per attempt:", tv[9], tv[10]);
-        for (int i = 0; i < 20; ++i) if (i != 9 && i != 10) fprintf(stderr, " %s %.0f", nm[i], (double)tv[i] / att);
-        if (tv[20]) fprintf(stderr, "; fused root pass: %llu cycles on the slowest worker", tv[20]);
-        fprintf(stderr, "\n");
-    }
     c->breakdown[5] += (double)(steps / steps_per_batch);
     auto t_d2h = std::chrono::steady_clock::now();
 
@@ -926,9 +870,7 @@ void do_build_emit(arroy_ctx* c, const uint32_t* root_ids, const uint64_t* base,
             }
         } catch (const std::exception& e) { std::lock_guard<std::mutex> lk(sink_mu); worker_err = e.what(); abort_flag = 2; }
     };
-    int nthreads = (int)std::min<uint64_t>(n_blocks, std::max(1u, std::min(64u, std::thread::hardware_concurrency())));
-    if (const char* e = getenv("ARROY_B200_ENCODE_THREADS")) nthreads = std::max(1, atoi(e));
-    if (c->n < 100000) nthreads = 1;
+    const int nthreads = c->n < 100000 ? 1 : (int)std::min<uint64_t>(n_blocks, std::max(1u, std::min(64u, std::thread::hardware_concurrency())));
     if (nthreads <= 1) worker();
     else { std::vector<std::thread> th; for (int i = 0; i < nthreads; ++i) th.emplace_back(worker); for (auto& x : th) x.join(); }
     c->breakdown[4] = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_enc).count();
@@ -1516,7 +1458,7 @@ int32_t arroy_b200_create_split(arroy_ctx* c, const uint32_t rng_key[8], uint64_
         P.n = (uint32_t)c->n; P.d = c->dim; P.ld = ld; P.metric = c->metric;
         size_t ws_bytes = (size_t)WS_VECS * ld * 4;
         P.use_smem_ws = ws_bytes <= 200 * 1024;
-        P.spec = (P.use_smem_ws && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024 && !(getenv("ARROY_B200_SPEC") && atoi(getenv("ARROY_B200_SPEC")) == 0)) ? 1 : 0;
+        P.spec = (P.use_smem_ws && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024) ? 1 : 0;
         if (P.spec) ws_bytes = (size_t)WS_VECS_SPEC * ld * 4;
         P.scratch = reinterpret_cast<float*>(c->s_misc.as<uint8_t>() + 64);
         size_t smem = P.use_smem_ws ? ws_bytes : 0;
@@ -1954,13 +1896,12 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 auto mark1 = [&]() { if (!c->xev[nte1]) CK(cudaEventCreate(&c->xev[nte1])); CK(cudaEventRecord(c->xev[nte1], c->stream)); ++nte1; };
                 mark1();
                 // every split normal's dot with the query in one pass over the forest's normals, when that is cheaper than the
-                // walker's chain of per-pop reductions (ARROY_B200_WALK1_DOTS_MB: largest normals matrix it is done for; 0 = never)
+                // walker's chain of per-pop reductions (up to a 768 MB normals matrix)
                 const float* d_pre = nullptr;
                 {
-                    const char* pe = getenv("ARROY_B200_WALK1_DOTS_MB");
-                    const uint64_t cap_mb = pe ? (uint64_t)atoll(pe) : 768ull;
+                    constexpr uint64_t DOTS_MAX_BYTES = 768ull << 20;
                     const uint64_t nbytes = (uint64_t)c->f_n_normals * ld * 4;
-                    if (c->f_n_normals > 0 && m <= 4 && nbytes <= cap_mb << 20 && c->dim >= 32) {
+                    if (c->f_n_normals > 0 && m <= 4 && nbytes <= DOTS_MAX_BYTES && c->dim >= 32) {
                         c->w_pre.ensure(4ull * F.n_nodes * m);
                         const uint32_t gx = (uint32_t)std::min<uint64_t>(((uint64_t)c->f_n_normals + 7) / 8, (uint64_t)c->sm_count * 8);
                         forest_dots_kernel<<<dim3(gx, m), 256, (size_t)ld * 4, c->stream>>>(F, c->f_n_normals, c->items.as<float>(), c->dim, ld, d_qrows, d_q, c->w_pre.as<float>());
@@ -2154,7 +2095,7 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
             c->h2d_bytes += 4ull * bm_words;
             WalkFilter& Fl = bf.Fl;
             Fl.bits = c->w_fbits.as<uint32_t>(); Fl.fcount = c->w_fcount.as<uint32_t>(); Fl.live = c->w_live.as<uint8_t>(); Fl.pops = c->w_pops.as<uint32_t>();
-            const bool shortcut = c->f_tree && c->f_complete && ftotal <= S.search_k && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
+            const bool shortcut = c->f_tree && c->f_complete && ftotal <= S.search_k;
             if (shortcut) {   // the rows, ascending: popcounts per word, an exclusive scan, then every query's segment is written
                 bf.n_walk = 0;
                 c->w_scount.ensure(4ull * bm_words); c->w_soff.ensure(4ull * bm_words);
@@ -2212,7 +2153,7 @@ void multi_filter_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
         G.group_words = G.count_off + 32ull * F.n_nodes;
         const uint64_t group_bytes = 4ull * G.group_words + 256;
         const uint32_t set_groups = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((1ull << 30) / group_bytes, 65535 / 32));
-        const bool shortcut_ok = c->f_tree && c->f_complete && getenv("ARROY_B200_NO_FILTER_SHORTCUT") == nullptr;
+        const bool shortcut_ok = c->f_tree && c->f_complete;
         std::vector<uint32_t> h_rows, h_qf, order, s_qrows, o_rows, o_len;
         std::vector<uint64_t> h_offs;
         std::vector<unsigned long long> ftotal;

@@ -73,6 +73,9 @@ __device__ __forceinline__ unsigned long long pticket(uint32_t seq, uint32_t tot
 __device__ __forceinline__ uint32_t pt_seq(unsigned long long t) { return (uint32_t)(t >> 48); }
 __device__ __forceinline__ uint32_t pt_total(unsigned long long t) { return (uint32_t)(t >> 24) & 0xffffffu; }
 __device__ __forceinline__ uint32_t pt_next(unsigned long long t) { return (uint32_t)t & 0xffffffu; }
+constexpr uint32_t LAT_MASK = 3;   // worker w is a latency worker (pworker) when (w & LAT_MASK) == 0: one in four
+// units per claim of a scan through the 8-bit planes: SHADOW_CHUNK, or SHADOW_BIG_CHUNK for scans of more than SHADOW_BIG_UNITS
+constexpr uint32_t SHADOW_CHUNK = 4, SHADOW_BIG_UNITS = 512, SHADOW_BIG_CHUNK = 8;
 
 struct BuildParams {
     const float* items; const float* ih0; const float* ih1;
@@ -97,8 +100,6 @@ struct BuildParams {
     // cluster-resident small nodes (control_kernel<.., CS > 1>): nodes of at most small_max rows are
     // scanned by the control kernel's own cluster, at most max_inner attempts per launch
     uint32_t small_max, max_inner;
-    uint32_t lat_mask;      // persistent schedule: worker w is a latency worker when (w & lat_mask) == 0
-    unsigned long long* timing;   // optional: 16 cycle counters summed over all control launches (ARROY_B200_CTRL_TIMING)
     // persistent schedule
     PSlot* slots;                 // n_trees
     float* cur_normal;            // n_trees x pool_stride: the normal of each tree's open scan job, at an address workers know without the job fields
@@ -108,7 +109,7 @@ struct BuildParams {
     // the 8-bit planes of the item matrix (kernels.cuh), or NULLs: scans of more than shadow_min_units units go through them
     // (scan_claim_planes)
     PlaneRows planes;
-    uint32_t shadow_min_units, shadow_small_chunk, shadow_big_units, shadow_big_chunk;
+    uint32_t shadow_min_units;
     unsigned long long* shadow_stats;   // [0] rows scanned through the planes, [1] of them re-scored from the f32 row, [2] through stage 2
     int32_t root_fused;
     uint32_t* root_ready;         // number of trees whose root normal is published
@@ -136,8 +137,6 @@ struct TwoMeansShared {
     float res[2][2];        // di, dj, double buffered by iteration parity
     float php[2], phq[2];   // headers of p and q
     float misc[2];
-    long long tacc[24];     // cycle accumulators of the phases (thread 0; flushed to BuildParams::timing when set)
-    long long tlast;
     // speculative two_means
     float G[12][12];        // approximate dots between the 12 gathered vectors (0 = p, 1 = q after normalize, 2.. = the ten k)
     float Gp[8][16][16];    // its partial products, one 16 x 16 tile per warp
@@ -148,11 +147,6 @@ struct TwoMeansShared {
     int ready;              // iterations whose choice has been published by the speculating warp
     int mismatch;
 };
-// phase ids of BuildParams::timing
-enum { TP_DECIDE = 0, TP_RNG = 1, TP_GATHER = 2, TP_NORMS = 3, TP_TWOMEANS = 4, TP_FINISH_SPLIT = 5, TP_CLUSTER_SCAN = 6, TP_PREFIX = 7, TP_PARTITION = 8, TP_ATTEMPTS = 9, TP_INNER = 10, TP_TOTAL = 11, TP_TM_DOT = 12, TP_TM_UPD = 13 };
-// (thread 0 records; the WARPSYNC afterwards merges it with the rest of warp 0 again — without it the warp stays split behind
-// every mark and the phase that follows is measured several times slower than it runs)
-#define TP_MARK(S_, id_) do { if (P.timing != nullptr && threadIdx.x < 32) { if (threadIdx.x == 0) { long long now_ = clock64(); (S_).tacc[id_] += now_ - (S_).tlast; (S_).tlast = now_; } __syncwarp(); } } while (0)
 
 // hsum256 of the four accumulators + ((h1+h2)+h3)+h4 when lane l holds accumulator lane l (simple_avx.rs:6-13)
 __device__ __forceinline__ float warp_hsum_exact(float acc) {
@@ -275,7 +269,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
     }
     if (tid >= 32 && tid < 132) { const int it = (tid - 32) / 10, l = (tid - 32) - 10 * it; S.An[it][l] = S.G[2 + it][2 + l] * __fdividef(1.f, cosine ? S.nk[2 + it] : 1.f); }
     __syncthreads();
-    TP_MARK(S, TP_TM_DOT);
     if (warp == 0) {
         // (1b) the recurrence on SUMS: with Sp = ic * p (the sum of p0 and the k / norm assigned to it), lane l < 10 carries
         // Sp . k_l and Sq . k_l; every lane carries Sp . Sp, Sq . Sq and the counts. The warp runs alone, so what counts is the
@@ -283,8 +276,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
         // before this iteration's branch is known (and patched with one add afterwards), and everything a branch changes — the
         // new Sp . Sp, its rsqrt / reciprocal, the new count — is computed for both outcomes ahead of the comparison.
         const int li = lane < 10 ? lane : 0;
-        long long tw0 = 0;
-        if (P.timing != nullptr) tw0 = clock64();
         float spk = S.G[0][2 + li], sqk = S.G[1][2 + li];
         float spp = S.G[0][0], sqq = S.G[1][1], ic = 1.f, jc = 1.f;
         float a = __shfl_sync(full, spk, 0), b = __shfl_sync(full, sqk, 0);
@@ -318,7 +309,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
             if (lane == 0) S.choice[it] = c1 ? 1 : (c2 ? 2 : 0);
         }
         asm volatile("" :: "f"(spk), "f"(sqk), "f"(spp), "f"(sqq), "f"(a), "f"(b) : "memory");
-        if (P.timing != nullptr && lane == 0) S.tacc[18] += clock64() - tw0;
     } else if (cosine) {
         // meanwhile the other warps divide the ten k by their norms (the k / norm term of update_mean, mod.rs:172-180) into the
         // slots the centroid versions will be produced in; element i belongs to thread (i mod 224) + 32 from here on
@@ -340,7 +330,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
         }
     }
     __syncthreads();
-    TP_MARK(S, 16);
     if (warp != 0) {
         // the centroid versions, element-wise and in the reference's exact operations; every thread only re-reads elements it
         // wrote itself, so the ten steps need no barrier
@@ -368,7 +357,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
         }
     }
     __syncthreads();
-    TP_MARK(S, TP_TM_UPD);
     // (2) the reference's dots: group j < 10: p_j . k_j, 10 + j: q_j . k_j (Euclidean: squared distances), 20 / 21: the D::init
     // dots of the initial p / q, 22 + j: of the centroid iteration j produced
     if (!EUCLID || warp < 5) {
@@ -388,7 +376,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
         if (g8 == 0) S.vdot[job] = r;
     }
     __syncthreads();
-    TP_MARK(S, 14);
     // (3) exact di / dj of every iteration (mod.rs:148-149) against the predicted branch
     int ps = 0, qs = 1;
     if (tid < 10) {
@@ -414,7 +401,6 @@ __device__ __forceinline__ bool spec_two_means(const BuildParams& P, float* ws, 
         if (want != S.choice[it]) S.mismatch = 1;
     }
     __syncthreads();
-    TP_MARK(S, 15);
     if (S.mismatch) return false;
     ps = 0; qs = 1;
     for (int j = 0; j < 10; ++j) { const int c = S.choice[j]; if (c == 1) ps = 14 + j; else if (c == 2) qs = 14 + j; }
@@ -464,7 +450,6 @@ __device__ __noinline__ void two_means_sequential(const BuildParams& P, float* w
             const float* a = qs ? q : p;
             float xk, xx;
             if (metric == EUCLIDEAN) exact_warp_ab_aa<true>(a, k, d, xk, xx); else exact_warp_ab_aa<false>(a, k, d, xk, xx);
-            TP_MARK(S, 14);
             if (lane == 0) {
                 float* hdr = qs ? S.phq : S.php;
                 float h0v = hdr[0], h1v = hdr[1];
@@ -479,7 +464,6 @@ __device__ __noinline__ void two_means_sequential(const BuildParams& P, float* w
                 }
                 S.res[it & 1][qs ? 1 : 0] = __fmul_rn(qs ? jc : ic, dv);
             }
-            TP_MARK(S, 15);
         } else if (cosine) {
             // meanwhile the other warps form k / norm for update_mean (mod.rs:86-94): it does not depend on
             // the centroids, so the division leaves the critical path
@@ -488,7 +472,6 @@ __device__ __noinline__ void two_means_sequential(const BuildParams& P, float* w
         }
         p_dirty = false; q_dirty = false;
         __syncthreads();
-        TP_MARK(S, TP_TM_DOT);
         const float di = S.res[it & 1][0], dj = S.res[it & 1][1];
         const float norm = cosine ? S.nk[2 + it] : 1.0f;
         if (norm != norm || norm <= 0.0f) continue;
@@ -506,7 +489,6 @@ __device__ __noinline__ void two_means_sequential(const BuildParams& P, float* w
             }
             if (up) { ic = c1; p_dirty = cosine; } else { jc = c1; q_dirty = cosine; }
             __syncthreads();
-            TP_MARK(S, TP_TM_UPD);
         }
     }
 }
@@ -582,7 +564,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
             for (int it = 0; it < 10; ++it) S.rows[2 + it] = rng.gen_range_incl(0, len - 1);
         }
     }
-    TP_MARK(S, TP_RNG);
     __syncthreads();
     uint32_t my_row = 0;
     if (tid < 12) my_row = __ldcg(seg + S.rows[tid]);  // RoaringBitmap::select(rank) on the ascending id list
@@ -605,7 +586,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
         }
     }
     __syncthreads();
-    TP_MARK(S, TP_GATHER);
     if (tid == 0) { S.php[0] = S.h0[0]; S.php[1] = S.h1[0]; S.phq[0] = S.h0[1]; S.phq[1] = S.h1[1]; }
     float* p = ws; float* q = ws + ld;
     float* sc0 = ws + (size_t)12 * ld; float* sc1 = ws + (size_t)13 * ld;
@@ -627,7 +607,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
         }
     }
     __syncthreads();
-    TP_MARK(S, TP_NORMS);
     bool spec_done = false;
     if constexpr (metric != MANHATTAN) {
         if (P.spec && d >= 32) {
@@ -638,7 +617,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
     }
     if (!spec_done) two_means_sequential<metric>(P, ws, S);
     __syncthreads();
-    TP_MARK(S, TP_TWOMEANS);
     // normal = normalize(p - q) (+ bias / extra_dim) — euclidean.rs:59-75, manhattan.rs:62-78,
     // cosine.rs:77-83, dot_product.rs:102-111. (A D::init still pending after the last update only
     // touches the centroid's norm header, which create_split does not read.)
@@ -667,7 +645,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
             if (mirror != nullptr) mirror[0] = bias;
         }
         __syncthreads();
-        TP_MARK(S, TP_FINISH_SPLIT);
     } else {
     for (int i = tid; i < ld; i += blockDim.x) nv[i] = i < d ? __fsub_rn(p[i], q[i]) : 0.f;
     float extra = (metric == DOT_PRODUCT) ? __fsub_rn(S.php[0], S.phq[0]) : 0.f;
@@ -701,7 +678,6 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
         if (mirror != nullptr) mirror[0] = (metric == DOT_PRODUCT) ? extra : 0.f;
     }
     __syncthreads();
-    TP_MARK(S, TP_FINISH_SPLIT);
     }
 }
 
@@ -933,8 +909,6 @@ __device__ __noinline__ void proot(const BuildParams& P, float* smN) {
     __syncthreads();
     if (!r_ok) return;
     __threadfence();
-    long long rt0 = 0;
-    if (P.timing != nullptr && tid == 0) rt0 = clock64();
     const uint32_t units = (n + SCAN_UNIT - 1) / SCAN_UNIT;
     // claims are taken one ahead, so that the first unit of the next claim can be prefetched during the last unit of this one
     if (tid == 0) r_claim = atomicAdd(P.root_ticket, 1u);
@@ -983,7 +957,6 @@ __device__ __noinline__ void proot(const BuildParams& P, float* smN) {
         for (uint32_t t = tid; t < T; t += CTRL_THREADS) atomicAdd(&P.slots[t].done, (unsigned long long)(u1 - u0));
         u0 = nu0;
     }
-    if (P.timing != nullptr && tid == 0) atomicMax(P.timing + 20, (unsigned long long)(clock64() - rt0));   // the slowest worker's pass
 }
 
 // A worker CTA: claims units of whatever the control CTAs have published and runs the same scan / partition code as work_kernel.
@@ -999,7 +972,7 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     const uint32_t T = P.n_trees;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t rot = (blockIdx.x - T) * 7u;
-    const bool latency_class = ((blockIdx.x - T) & P.lat_mask) == 0u;
+    const bool latency_class = ((blockIdx.x - T) & LAT_MASK) == 0u;
     uint32_t loaded_t = 0xffffffffu, loaded_seq = 0xffffffffu;
     float nh0 = 0.f;
     float2 wf = make_float2(0.f, 0.f);   // the loaded normal's bound factors (scan_claim_planes)
@@ -1179,7 +1152,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
     // job.kind is already JOB_NONE and job.pad 0 for a finished tree / after an error
     if (P.st[t].phase == PH_DONE || *P.error != ERR_NONE) { if (CS > 1) cooperative_groups::this_cluster().sync(); return; }
     uint32_t inner = 0;
-    if (P.timing != nullptr && threadIdx.x == 0) { for (int i = 0; i < 24; ++i) TM.tacc[i] = 0; TM.tlast = clock64(); TM.tacc[TP_TOTAL] = -TM.tlast; }
     Frame* gframes = P.frames + (size_t)t * MAX_DEPTH;
     if (threadIdx.x == 0) S = P.st[t];
     __syncthreads();
@@ -1200,7 +1172,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
         total_left = cta_exclusive_scan(unit_left, (f.len + SCAN_UNIT - 1) / SCAN_UNIT, sm_tmp);
     }
     __syncthreads();
-    TP_MARK(TM, TP_PREFIX);
 
     uint64_t pref_base = ~0ull;   // block number held in s_pref[0] (every thread tracks the same value)
     for (;;) {
@@ -1294,7 +1265,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
             s_rng.pref = &s_pref[0][0]; s_rng.pref_base = pref_base; s_rng.pref_n = 8;
         }
         __syncthreads();
-        TP_MARK(TM, TP_DECIDE);
         const int action = s_action;
         if (action == ACT_EXIT) break;
         const Frame f = FR(S.sp);
@@ -1307,7 +1277,7 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
             else create_split_cta<METRIC>(P, s_rng, src, f.len, P.scratch + (size_t)t * WS_VECS * P.ld, TM, slot_ptr, mirror);
             if (tid == 0) {
                 if (TM.mismatch) { S.n_misspec += 1; TM.mismatch = 0; }
-                S.n_splits_tried += 1; if (P.timing) TM.tacc[TP_ATTEMPTS] += 1;
+                S.n_splits_tried += 1;
                 job.kind = JOB_SCAN; job.len = f.len; job.rows = src; job.normal = slot_ptr;
                 job.flags = flags + f.start; job.margins = nullptr; job.unit_left = unit_left; job.dst = nullptr; job.total_left = 0;
                 S.phase = PH_AWAIT_SCAN;
@@ -1318,7 +1288,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
                 // flight) and the job fields must be visible device-wide before the job opens
                 __threadfence();
                 __syncthreads();
-                TP_MARK(TM, 17);
                 const uint32_t units = (f.len + SCAN_UNIT - 1) / SCAN_UNIT;
                 if (tid == 0) {
                     s_pseq += 1;
@@ -1335,18 +1304,15 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
                     } else {
                     // a claim = `chunk` units: four for the big scans (and for everything that goes through the 8-bit planes)
                     const bool via_shadow = P.planes.hi != nullptr && units > P.shadow_min_units;
-                    const uint32_t chunk = via_shadow ? (units > P.shadow_big_units ? P.shadow_big_chunk : (units > 128u ? 4u : P.shadow_small_chunk)) : (units > 1024u ? 4u : 1u), groups = (units + chunk - 1) / chunk;
+                    const uint32_t chunk = via_shadow ? (units > SHADOW_BIG_UNITS ? SHADOW_BIG_CHUNK : SHADOW_CHUNK) : (units > 1024u ? 4u : 1u), groups = (units + chunk - 1) / chunk;
                     ppublish(P.slots[t], job, s_pseq, groups, chunk);
                     s_wait_ok = pwait(P, P.slots[t], s_pseq, groups) ? 1 : 0;
                     }
-                    if (P.timing) TM.tacc[TP_INNER] += 1;
                 }
                 __syncthreads();
-                TP_MARK(TM, TP_CLUSTER_SCAN);
                 if (!s_wait_ok) break;
                 total_left = cta_exclusive_scan(unit_left, units, sm_tmp);
                 __syncthreads();
-                TP_MARK(TM, TP_PREFIX);
                 continue;
             }
             if (CS > 1 && f.len <= P.small_max && inner < P.max_inner) {
@@ -1355,12 +1321,10 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
                 Job jb = job;
                 cluster_scan_share<CS>(P, jb, reinterpret_cast<float*>(ctrl_smem) + (size_t)12 * P.ld, &s_scan_count, 0);
                 cooperative_groups::this_cluster().sync();                       // [B] flags / unit counts visible to this CTA
-                TP_MARK(TM, TP_CLUSTER_SCAN);
-                if (tid == 0) { job.kind = JOB_NONE; job.pad = 0; if (P.timing) TM.tacc[TP_INNER] += 1; }
+                if (tid == 0) { job.kind = JOB_NONE; job.pad = 0; }
                 total_left = cta_exclusive_scan(unit_left, (f.len + SCAN_UNIT - 1) / SCAN_UNIT, sm_tmp);
                 ++inner;
                 __syncthreads();
-                TP_MARK(TM, TP_PREFIX);
                 continue;
             }
             break;
@@ -1405,7 +1369,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
             if (tid == 0) { FR(S.sp).stage = 1; S.phase = PH_AWAIT_PART; }
             total_left = 0;
             __syncthreads();
-            TP_MARK(TM, TP_PARTITION);
             continue;
         }
         if (action == ACT_PART_INLINE) {
@@ -1414,7 +1377,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
             if (tid == 0) { FR(S.sp).stage = 1; S.phase = PH_AWAIT_PART; }
             total_left = 0;
             __syncthreads();
-            TP_MARK(TM, TP_PARTITION);
             continue;
         }
     }
@@ -1422,10 +1384,6 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
     if (CS > 1) cooperative_groups::this_cluster().sync();   // releases the helpers (job.pad == 0)
     for (int i = tid; i <= S.sp && i < SMF; i += blockDim.x) gframes[i] = sm_frames[i];
     if (tid == 0) { S.pos = s_rng.pos; P.st[t] = S; }
-    if (tid == 0 && P.timing) {
-        TM.tacc[TP_TOTAL] += clock64();
-        for (int i = 0; i < 20; ++i) atomicAdd(P.timing + i, (unsigned long long)TM.tacc[i]);
-    }
 }
 
 // Merge the two ping-pong id buffers into `final_ids` following each leaf's parity.

@@ -452,7 +452,7 @@ __device__ __forceinline__ void partition_block(const uint32_t* __restrict__ src
 // Dynamic shared memory: ld floats (normal) + (njobs + 1) uint32 (unit prefix).
 __global__ void __launch_bounds__(WORK_THREADS, 3)
 work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const float* __restrict__ ih0,
-            uint32_t d, uint32_t ld, int metric, int interleave) {
+            uint32_t d, uint32_t ld, int metric) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sm_normal = reinterpret_cast<float*>(smem_raw);
     uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_normal + ld);
@@ -480,34 +480,6 @@ work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ i
     const uint32_t total = sm_prefix[njobs];
     int loaded_job = -1;
     float nh0 = 0.f;
-    if (interleave && njobs > 1) {
-        // Unit u of every job before unit u+1 of any job: CTAs that run at the same time read the same
-        // region of the item matrix for different trees, so all but the first reader hit in L2
-        // (every tree's node at a given depth is a uniform sample of all rows, in ascending order).
-        __shared__ uint32_t sm_maxu;
-        if (threadIdx.x == 0) { uint32_t m = 0; for (int j = 0; j < njobs; ++j) m = max(m, sm_prefix[j + 1] - sm_prefix[j]); sm_maxu = m; }
-        __syncthreads();
-        const uint64_t total_il = (uint64_t)sm_maxu * (uint64_t)njobs;
-        for (uint64_t g = blockIdx.x; g < total_il; g += gridDim.x) {
-            const uint32_t unit = (uint32_t)(g / (uint64_t)njobs);
-            const int j = (int)(g % (uint64_t)njobs);
-            if (unit >= sm_prefix[j + 1] - sm_prefix[j]) continue;
-            const Job jb = jobs[j];
-            if (jb.kind == JOB_SCAN) {
-                if (loaded_job != j) {
-                    __syncthreads();
-                    for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) sm_normal[i] = jb.normal[NORMAL_HDR + i];
-                    nh0 = jb.normal[0];
-                    loaded_job = j;
-                    __syncthreads();
-                }
-                scan_unit(jb, unit, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
-            } else {
-                partition_block(jb.rows, jb.flags, jb.dst, unit * PART_UNIT, jb.len, jb.unit_left[unit * (PART_UNIT / SCAN_UNIT)], jb.total_left, sm_w);
-            }
-        }
-        return;
-    }
     for (uint32_t u = blockIdx.x; u < total; u += gridDim.x) {
         int lo = 0, hi = njobs;  // last j with prefix[j] <= u
         while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (sm_prefix[mid] <= u) lo = mid; else hi = mid; }
