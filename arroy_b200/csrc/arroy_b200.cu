@@ -1051,14 +1051,98 @@ void bq_normalize(arroy_ctx* c, float* d_dist, uint64_t count) {
     c->n_launches += 1;
 }
 
-void do_rerank_batch(arroy_ctx* c, uint32_t nq, const float* queries, const float* qh0, const float* /*qh1*/, const uint32_t* rows,
-                     const uint64_t* offsets, uint32_t k, uint32_t* out_rows, float* out_dist, uint32_t* out_len) {
+// Event marks on the stream, in c->xev. Once the stream is idle, add_to(b) adds the time from mark i to mark i + 1 to b[i].
+struct Marks {
+    arroy_ctx* c;
+    int n = 0;
+    void operator()() { if (!c->xev[n]) CK(cudaEventCreate(&c->xev[n])); CK(cudaEventRecord(c->xev[n], c->stream)); ++n; }
+    void add_to(double* b) const { for (int i = 0; i + 1 < n; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); b[i] += ms; } }
+};
+
+// A call's queries on the device: by item their rows (vecs == nullptr), by vector their vectors (rows == nullptr), and their
+// first header.
+struct DevQueries {
+    const float* vecs = nullptr;
+    const uint32_t* rows = nullptr;
+    const float* h0 = nullptr;
+};
+
+// Uploads queries q0 .. q0 + m of a call: by item their rows into w_qrows, by vector their vectors into s_q (rows padded to ld
+// with zeros). Their headers go to s_qh0: the caller's, else by item the stored header of the item, else zero.
+DevQueries upload_queries(arroy_ctx* c, uint32_t q0, uint32_t m, const uint32_t* query_rows, const float* queries, const float* qhdr0) {
+    const uint32_t ld = c->ld, d = c->dim;
+    DevQueries Q;
+    c->s_qh0.ensure(4ull * m);
+    if (query_rows) {
+        c->w_qrows.ensure(4ull * m);
+        CK(cudaMemcpyAsync(c->w_qrows.p, query_rows + q0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
+        Q.rows = c->w_qrows.as<uint32_t>();
+    } else {
+        c->s_q.ensure((size_t)m * ld * 4);
+        if (ld != d) CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)m * ld * 4, c->stream));
+        CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries + (size_t)q0 * d, (size_t)d * 4, (size_t)d * 4, m, cudaMemcpyHostToDevice, c->stream));
+        Q.vecs = c->s_q.as<float>();
+    }
+    if (qhdr0) CK(cudaMemcpyAsync(c->s_qh0.p, qhdr0 + q0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
+    else if (query_rows) { gather_f32_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->s_qh0.as<float>(), c->h0.as<float>(), Q.rows, m); CK(cudaGetLastError()); }
+    else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
+    Q.h0 = c->s_qh0.as<float>();
+    return Q;
+}
+
+// The re-rank of m queries whose sorted candidate rows are rows[beg[q] .. end[q]): at most max_len rows per query, n_keys rows
+// in the whole array (s_keys / s_dists hold as many). Results in s_orows / s_odist / s_olen. With try_fused the fused kernel
+// goes first, and the plain kernels run only if a query needs them: distance_kernel, then topk_kernel, or for k beyond the
+// top-k buffer a full segmented sort of the keys and take_sorted_kernel. `mark`, when given, is recorded after the distances.
+// (beg / end are not const: the key sort stays the CUB instantiation with uint64_t* offsets, as the walk's candidate sort)
+void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32_t* rows, uint64_t* beg, uint64_t* end,
+                     uint64_t n_keys, uint64_t max_len, uint32_t k, bool try_fused, Marks* mark) {
+    if (try_fused && frerank_enabled(c, k)) {   // one fused kernel per query: bf16 pre-filter + exact re-score + top-k (frerank.cuh)
+        frerank_launch(c, m, Q.vecs, Q.rows, Q.h0, rows, beg, end, k);
+        CK(cudaStreamSynchronize(c->stream));
+        if (frerank_ok(c, m)) { if (mark) (*mark)(); return; }
+    }
+    if (max_len) {   // Manhattan sums one row per lane, the other metrics four rows per warp
+        const uint64_t per = (c->metric == MANHATTAN || c->metric == BQ_MANHATTAN) ? 32 : 4;
+        const uint64_t warps = (max_len + per - 1) / per;
+        const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / std::min<uint32_t>(m, c->sm_count * 8u))));
+        distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric, Q.vecs, Q.rows, Q.h0, m,
+                                                           rows, beg, end, c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
+        CK(cudaGetLastError());
+    }
+    if (mark) (*mark)();
+    if (k > TOPK_CAP / 2) {
+        c->s_keys2.ensure(std::max<uint64_t>(n_keys, 1) * 8);
+        size_t tmp_bytes = 0;
+        CK(cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, c->s_keys.as<unsigned long long>(), c->s_keys2.as<unsigned long long>(), (int64_t)n_keys, (int64_t)m,
+                                              beg, end, c->stream));
+        c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
+        CK(cub::DeviceSegmentedSort::SortKeys(c->w_tmp.p, tmp_bytes, c->s_keys.as<unsigned long long>(), c->s_keys2.as<unsigned long long>(), (int64_t)n_keys, (int64_t)m,
+                                              beg, end, c->stream));
+        take_sorted_kernel<<<m, 256, 0, c->stream>>>(c->s_keys2.as<unsigned long long>(), c->s_dists.as<float>(), rows, beg, end, k, c->metric,
+                                                     c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
+    } else
+        topk_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), rows, beg, end, k, c->metric,
+                                                       c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
+    CK(cudaGetLastError());
+}
+
+// The results of queries q0 .. q0 + m (k slots each) to the caller's arrays, with the walk status when out_status is given.
+void copy_results(arroy_ctx* c, uint32_t q0, uint32_t m, uint32_t k, uint32_t* out_rows, float* out_dist, uint32_t* out_len, int32_t* out_status = nullptr) {
+    CK(cudaMemcpyAsync(out_rows + (size_t)q0 * k, c->s_orows.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(out_dist + (size_t)q0 * k, c->s_odist.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(out_len + q0, c->s_olen.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
+    if (out_status) CK(cudaMemcpyAsync(out_status + q0, c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+}
+
+void do_rerank_batch(arroy_ctx* c, uint32_t nq, const float* queries, const float* qh0, const uint32_t* rows, const uint64_t* offsets, uint32_t k,
+                     uint32_t* out_rows, float* out_dist, uint32_t* out_len) {
     require_staged(c);
     set_device(c);
     if (nq == 0) return;
     if (k == 0) { for (uint32_t q = 0; q < nq; ++q) out_len[q] = 0; return; }
     if (nq > 65535) throw ArgError("at most 65535 queries per rerank_batch call");
-    const bool big_k = k > TOPK_CAP / 2;   // beyond the streaming top-k buffer: full segmented sort of the keys
     const uint64_t total = offsets[nq];
     if (total && !rows) throw ArgError("null rows");
     for (uint32_t q = 0; q < nq; ++q) {
@@ -1066,9 +1150,6 @@ void do_rerank_batch(arroy_ctx* c, uint32_t nq, const float* queries, const floa
         if (offsets[q + 1] - offsets[q] > 0xffffffffull) throw ArgError("too many candidates for one query");
     }
     for (uint64_t i = 0; i < total; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
-    const uint32_t ld = c->ld;
-    c->s_q.ensure((size_t)nq * ld * 4);
-    c->s_qh0.ensure((size_t)nq * 4);
     c->s_off.ensure((size_t)(nq + 1) * 8);
     c->s_rows.ensure(std::max<uint64_t>(total, 1) * 4);
     c->s_keys.ensure(std::max<uint64_t>(total, 1) * 8);
@@ -1076,54 +1157,19 @@ void do_rerank_batch(arroy_ctx* c, uint32_t nq, const float* queries, const floa
     c->s_orows.ensure((size_t)nq * k * 4);
     c->s_odist.ensure((size_t)nq * k * 4);
     c->s_olen.ensure((size_t)nq * 4);
-    CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)nq * ld * 4, c->stream));
-    CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries, (size_t)c->dim * 4, (size_t)c->dim * 4, nq, cudaMemcpyHostToDevice, c->stream));
-    if (qh0) CK(cudaMemcpyAsync(c->s_qh0.p, qh0, (size_t)nq * 4, cudaMemcpyHostToDevice, c->stream));
-    else CK(cudaMemsetAsync(c->s_qh0.p, 0, (size_t)nq * 4, c->stream));
+    const DevQueries Q = upload_queries(c, 0, nq, nullptr, queries, qh0);
     CK(cudaMemcpyAsync(c->s_off.p, offsets, (size_t)(nq + 1) * 8, cudaMemcpyHostToDevice, c->stream));
     if (total) CK(cudaMemcpyAsync(c->s_rows.p, rows, total * 4, cudaMemcpyHostToDevice, c->stream));
     uint64_t max_c = 0;
     for (uint32_t q = 0; q < nq; ++q) max_c = std::max<uint64_t>(max_c, offsets[q + 1] - offsets[q]);
-    bool fused = false;
-    if (!big_k && total >= 512ull * nq && max_c <= (uint64_t)FR_CAP && frerank_enabled(c, k)) {
-        // rows of each query must be ascending for the (distance, id) tie-break; the callers of this path pass sorted lists
-        frerank_launch(c, nq, c->s_q.as<float>(), nullptr, c->s_qh0.as<float>(), c->s_rows.as<uint32_t>(), c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, k);
-        CK(cudaStreamSynchronize(c->stream));
-        fused = frerank_ok(c, nq);
-    }
-    if (!fused) {
-    if (total) {
-        uint64_t per = (c->metric == MANHATTAN || c->metric == BQ_MANHATTAN) ? 32 : 4;
-        uint64_t warps = (max_c + per - 1) / per;
-        uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / std::min<uint32_t>(nq, c->sm_count * 8u))));
-        dim3 grid(gx, nq);
-        distance_kernel<<<grid, 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, c->s_q.as<float>(), nullptr, c->s_qh0.as<float>(), nq,
-                                                     c->s_rows.as<uint32_t>(), c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
-        CK(cudaGetLastError());
-    }
-    if (big_k) {
-        c->s_keys2.ensure(std::max<uint64_t>(total, 1) * 8);
-        size_t tmp_bytes = 0;
-        CK(cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, c->s_keys.as<unsigned long long>(), c->s_keys2.as<unsigned long long>(), (int64_t)total, (int64_t)nq,
-                                              c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, c->stream));
-        c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
-        CK(cub::DeviceSegmentedSort::SortKeys(c->w_tmp.p, tmp_bytes, c->s_keys.as<unsigned long long>(), c->s_keys2.as<unsigned long long>(), (int64_t)total, (int64_t)nq,
-                                              c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, c->stream));
-        take_sorted_kernel<<<nq, 256, 0, c->stream>>>(c->s_keys2.as<unsigned long long>(), c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, k, c->metric,
-                                                      c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
-    } else
-    topk_kernel<<<nq, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, k, c->metric,
-                                                    c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
-    CK(cudaGetLastError());
-    }
+    // (the fused kernel's (distance, id) tie-break needs each query's rows ascending; the callers of this path pass sorted lists)
+    rerank_segments(c, nq, Q, c->s_rows.as<uint32_t>(), c->s_off.as<uint64_t>(), c->s_off.as<uint64_t>() + 1, total, max_c, k,
+                    total >= 512ull * nq && max_c <= (uint64_t)FR_CAP, nullptr);
     c->n_launches += total ? 2 : 1;
     bq_normalize(c, c->s_odist.as<float>(), (uint64_t)nq * k);
     c->h2d_bytes += (uint64_t)nq * c->dim * 4 + (uint64_t)nq * 4 + (uint64_t)(nq + 1) * 8 + total * 4;
     c->d2h_bytes += (uint64_t)nq * k * 8 + (uint64_t)nq * 4;
-    CK(cudaMemcpyAsync(out_rows, c->s_orows.p, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(out_dist, c->s_odist.p, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(out_len, c->s_olen.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
+    copy_results(c, 0, nq, k, out_rows, out_dist, out_len);
 }
 
 // single-CTA create_split over a host row list (exposes D::create_split for parity tests and for
@@ -1568,7 +1614,7 @@ int32_t arroy_b200_rerank(arroy_ctx* c, const float* query, float qhdr0, float q
     return guarded(c, [&] {
         if (!query || (n_rows && !rows) || !out_len) throw ArgError("null argument");
         uint64_t offs[2] = {0, n_rows};
-        do_rerank_batch(c, 1, query, &qhdr0, &qhdr1, rows, offs, k, out_rows, out_dist, out_len);
+        do_rerank_batch(c, 1, query, &qhdr0, rows, offs, k, out_rows, out_dist, out_len);
     });
 }
 
@@ -1576,7 +1622,7 @@ int32_t arroy_b200_rerank_batch(arroy_ctx* c, uint32_t nq, const float* queries,
                                 const uint64_t* row_offsets, uint32_t k, uint32_t* out_rows, float* out_dist, uint32_t* out_len) {
     return guarded(c, [&] {
         if (nq && (!queries || !row_offsets || !out_len)) throw ArgError("null argument");
-        do_rerank_batch(c, nq, queries, qhdr0, qhdr1, rows, row_offsets, k, out_rows, out_dist, out_len);
+        do_rerank_batch(c, nq, queries, qhdr0, rows, row_offsets, k, out_rows, out_dist, out_len);
     });
 }
 
@@ -1596,7 +1642,7 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
             std::vector<uint64_t> offs(nq + 1);
             for (uint32_t q = 0; q <= nq; ++q) offs[q] = (uint64_t)q * n_rows;
             for (uint32_t q = 0; q < nq; ++q) memcpy(rep.data() + (size_t)q * n_rows, rows, 4 * n_rows);
-            do_rerank_batch(c, nq, queries, qhdr0, nullptr, rep.data(), offs.data(), k, out_rows, out_dist, out_len);
+            do_rerank_batch(c, nq, queries, qhdr0, rep.data(), offs.data(), k, out_rows, out_dist, out_len);
             return;
         }
         const uint32_t ld = c->ld, nc = (uint32_t)n_rows;
@@ -1626,16 +1672,11 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
         const uint32_t chunk = (uint32_t)std::max<uint64_t>(XQB, std::min<uint64_t>(nq, ((2ull << 30) / (4ull * lds)) / XQB * XQB));
         for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
             const uint32_t m = std::min(chunk, nq - q0);
-            c->s_q.ensure((size_t)m * ld * 4); c->s_qh0.ensure(4ull * m);
             c->s_orows.ensure(4ull * m * k); c->s_odist.ensure(4ull * m * k); c->s_olen.ensure(4ull * m);
             // (a pinned multi-thread bounce of the 12.6 MB of config 5 was measured: not faster than the driver's own staging)
-            if (ld != c->dim) CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)m * ld * 4, c->stream));
-            CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries + (size_t)q0 * c->dim, (size_t)c->dim * 4, (size_t)c->dim * 4, m, cudaMemcpyHostToDevice, c->stream));
-            if (qhdr0) CK(cudaMemcpyAsync(c->s_qh0.p, qhdr0 + q0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
-            else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
+            const DevQueries Q = upload_queries(c, q0, m, nullptr, queries, qhdr0);
             bool done = false;
-            int nte = 0;
-            auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
+            Marks mark{c};
             if (filter) {
                 c->xf_calls += 1;
                 mark();
@@ -1643,14 +1684,14 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
                 c->x_sel.ensure(4ull * m * cap); c->x_beg.ensure(8ull * m); c->x_end.ensure(8ull * m);
                 c->s_dists.ensure(4ull * m * cap); c->s_keys.ensure(8ull * m * cap);
                 { uint64_t warps = ((uint64_t)m + 3) / 4; int g = (int)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16));
-                  norms_kernel<<<g, 256, 0, c->stream>>>(c->s_q.as<float>(), m, c->dim, ld, c->x_qnorm.as<float>(), nullptr); CK(cudaGetLastError()); }
-                xf_query_prep_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->x_qnorm.as<float>(), c->s_qh0.as<float>(), m, c->metric, xf_rel(c->dim), c->dim, c->x_gmax.as<uint32_t>(),
+                  norms_kernel<<<g, 256, 0, c->stream>>>(Q.vecs, m, c->dim, ld, c->x_qnorm.as<float>(), nullptr); CK(cudaGetLastError()); }
+                xf_query_prep_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->x_qnorm.as<float>(), Q.h0, m, c->metric, xf_rel(c->dim), c->dim, c->x_gmax.as<uint32_t>(),
                                                                              c->x_qa.as<float>(), c->x_qb.as<float>(), c->x_twoe.as<float>());
                 CK(cudaGetLastError());
                 mark();
                 // A (m x nc, row-major) = distance estimates: Q . cand^T on the tensor cores (TF32 inputs, FP32 accumulate) + fused epilogue
                 TgEpilogue ep{c->metric == EUCLIDEAN ? TG_EUCLID : (c->metric == COSINE ? TG_COSINE : TG_NEG), c->x_qa.as<float>(), c->x_qb.as<float>(), c->x_ca.as<float>(), c->x_cb.as<float>()};
-                xf_scores(c, c->s_q.as<float>(), m, cand, nc, c->x_S.as<float>(), lds, ep, xf_engine());
+                xf_scores(c, Q.vecs, m, cand, nc, c->x_S.as<float>(), lds, ep, xf_engine());
                 mark();
                 CK(cudaMemsetAsync(c->x_flag.p, 0, 4, c->stream));
                 xf_select_kernel<<<m, XF_THREADS, 0, c->stream>>>(c->x_S.as<float>(), lds, nc, k, c->x_twoe.as<float>(), c->s_rows.as<uint32_t>(), cap,
@@ -1658,22 +1699,13 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
                 CK(cudaGetLastError());
                 mark();
                 // exact re-score of the survivors, in the reference's summation order
-                { uint64_t warps = ((uint64_t)cap + 3) / 4;
-                  uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / std::min<uint32_t>(m, c->sm_count * 8u))));
-                  dim3 grid(gx, m);
-                  distance_kernel<<<grid, 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, c->s_q.as<float>(), nullptr, c->s_qh0.as<float>(), m,
-                                                               c->x_sel.as<uint32_t>(), c->x_beg.as<uint64_t>(), c->x_end.as<uint64_t>(), c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
-                  CK(cudaGetLastError()); }
-                mark();
-                topk_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), c->x_sel.as<uint32_t>(), c->x_beg.as<uint64_t>(), c->x_end.as<uint64_t>(), k, c->metric,
-                                                                c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
-                CK(cudaGetLastError());
+                rerank_segments(c, m, Q, c->x_sel.as<uint32_t>(), c->x_beg.as<uint64_t>(), c->x_end.as<uint64_t>(), (uint64_t)m * cap, cap, k, false, &mark);
                 c->n_launches += 6;
                 mark();
                 int flag = 0;
                 CK(cudaMemcpyAsync(&flag, c->x_flag.p, 4, cudaMemcpyDeviceToHost, c->stream));
                 CK(cudaStreamSynchronize(c->stream));
-                for (int i = 0; i + 1 < nte; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); c->xbreak[i] += ms; }
+                mark.add_to(c->xbreak);
                 done = flag == 0;
                 { std::vector<uint64_t> ends(m); CK(cudaMemcpy(ends.data(), c->x_end.p, 8ull * m, cudaMemcpyDeviceToHost));
                   for (uint32_t q = 0; q < m; ++q) c->xf_selected += ends[q] - (uint64_t)q * cap; c->xf_queries += m; }
@@ -1681,13 +1713,13 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
             }
             if (!done) {
                 c->s_dists.ensure(4ull * m * nc);
-                nte = 0; mark();
+                mark.n = 0; mark();
                 dim3 grid((nc + XCB - 1) / XCB, (m + XQB - 1) / XQB);
                 if (c->metric == EUCLIDEAN)
-                    xrerank_kernel<true><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, c->s_q.as<float>(), c->s_qh0.as<float>(), m,
+                    xrerank_kernel<true><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, Q.vecs, Q.h0, m,
                                                                           c->s_rows.as<uint32_t>(), nc, c->s_dists.as<float>());
                 else
-                    xrerank_kernel<false><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, c->s_q.as<float>(), c->s_qh0.as<float>(), m,
+                    xrerank_kernel<false><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, Q.vecs, Q.h0, m,
                                                                            c->s_rows.as<uint32_t>(), nc, c->s_dists.as<float>());
                 CK(cudaGetLastError());
                 topk_dense_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), nc, k, c->metric,
@@ -1696,12 +1728,9 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
                 c->n_launches += 2;
                 mark();
                 CK(cudaStreamSynchronize(c->stream));
-                { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[0], c->xev[1])); c->xbreak[5] += ms; }
+                mark.add_to(c->xbreak + 5);
             }
-            CK(cudaMemcpyAsync(out_rows + (size_t)q0 * k, c->s_orows.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaMemcpyAsync(out_dist + (size_t)q0 * k, c->s_odist.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaMemcpyAsync(out_len + q0, c->s_olen.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaStreamSynchronize(c->stream));
+            copy_results(c, q0, m, k, out_rows, out_dist, out_len);
         }
         c->h2d_bytes += (uint64_t)nq * c->dim * 4 + 4ull * nc;
         c->d2h_bytes += 8ull * nq * k + 4ull * nq;
@@ -1843,8 +1872,6 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
         const bool filtered = bf.mode != FM_NONE, multi = bf.mode == FM_MULTI;
         const WalkFilter& Fl0 = bf.Fl;
         const size_t walk_smem = (size_t)WALK_WARPS * WALK_SHEAP * 8;
-        int nte = 0;
-        auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
         std::vector<int32_t> h_status;
         std::vector<uint32_t> h_pops;
         auto filter_tally = [&](uint32_t m, uint32_t m_walk) {   // after the stream is idle: statistics of m filtered queries, the first m_walk walked
@@ -1871,30 +1898,14 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
         //      all SMs. Any query it cannot hold (heap / candidate overflow) sends the call through the general path below.
         if (bf.n_walk > 0 && nq <= 16 && cand_cap64 <= (uint64_t)W1_CAND && getenv("ARROY_B200_NO_WALK1") == nullptr) {
             const uint32_t m = nq, m_walk = bf.n_walk;
-            const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
             if (ld <= W1_MAX_LD) {
                 c->w_cand2.ensure(4ull * cand_cap * m); c->w_count.ensure(4ull * m); c->w_status.ensure(4ull * m);
                 c->w_beg.ensure(8ull * (m + 1)); c->w_end.ensure(8ull * (m + 1));
                 c->s_keys.ensure(8ull * cand_cap * m); c->s_dists.ensure(4ull * cand_cap * m);
-                c->s_orows.ensure(4ull * m * k); c->s_odist.ensure(4ull * m * k); c->s_olen.ensure(4ull * m); c->s_qh0.ensure(4ull * m);
-                const uint32_t* d_qrows = nullptr;
-                const float* d_q = nullptr;
-                if (query_rows) {
-                    c->w_qrows.ensure(4ull * m);
-                    CK(cudaMemcpyAsync(c->w_qrows.p, query_rows, 4ull * m, cudaMemcpyHostToDevice, c->stream));
-                    d_qrows = c->w_qrows.as<uint32_t>();
-                } else {
-                    c->s_q.ensure((size_t)m * ld * 4);
-                    if (ld != c->dim) CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)m * ld * 4, c->stream));
-                    CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries, (size_t)c->dim * 4, (size_t)c->dim * 4, m, cudaMemcpyHostToDevice, c->stream));
-                    d_q = c->s_q.as<float>();
-                }
-                if (qhdr0) CK(cudaMemcpyAsync(c->s_qh0.p, qhdr0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
-                else if (query_rows) { gather_f32_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->s_qh0.as<float>(), c->h0.as<float>(), d_qrows, m); CK(cudaGetLastError()); }
-                else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
-                int nte1 = 0;
-                auto mark1 = [&]() { if (!c->xev[nte1]) CK(cudaEventCreate(&c->xev[nte1])); CK(cudaEventRecord(c->xev[nte1], c->stream)); ++nte1; };
-                mark1();
+                c->s_orows.ensure(4ull * m * k); c->s_odist.ensure(4ull * m * k); c->s_olen.ensure(4ull * m);
+                const DevQueries Q = upload_queries(c, 0, m, query_rows, queries, qhdr0);
+                Marks mark{c};
+                mark();
                 // every split normal's dot with the query in one pass over the forest's normals, when that is cheaper than the
                 // walker's chain of per-pop reductions (up to a 768 MB normals matrix)
                 const float* d_pre = nullptr;
@@ -1904,7 +1915,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                     if (c->f_n_normals > 0 && m <= 4 && nbytes <= DOTS_MAX_BYTES && c->dim >= 32) {
                         c->w_pre.ensure(4ull * F.n_nodes * m);
                         const uint32_t gx = (uint32_t)std::min<uint64_t>(((uint64_t)c->f_n_normals + 7) / 8, (uint64_t)c->sm_count * 8);
-                        forest_dots_kernel<<<dim3(gx, m), 256, (size_t)ld * 4, c->stream>>>(F, c->f_n_normals, c->items.as<float>(), c->dim, ld, d_qrows, d_q, c->w_pre.as<float>());
+                        forest_dots_kernel<<<dim3(gx, m), 256, (size_t)ld * 4, c->stream>>>(F, c->f_n_normals, c->items.as<float>(), c->dim, ld, Q.rows, Q.vecs, c->w_pre.as<float>());
                         CK(cudaGetLastError());
                         c->n_launches += 1;
                         d_pre = c->w_pre.as<float>();
@@ -1912,46 +1923,31 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 }
                 const int w1debug = getenv("ARROY_B200_WALK1_DEBUG") ? 1 : 0;
                 if (m_walk < m) shortcut(0, m_walk, m, c->w_cand2.as<uint32_t>());   // (multi only: a shared filter walks every query or none)
+                WalkFilter Fl = Fl0;
                 if (filtered) {
-                    WalkFilter Fl = Fl0;
                     Fl.spill_cap = F.n_roots + F.n_nodes;
                     c->w_spill.ensure(8ull * Fl.spill_cap * m_walk);
                     Fl.spill = c->w_spill.as<unsigned long long>();
-                    if (multi)
-                        walk1_kernel<true, true><<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug,
-                                                                                           search_k, c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
-                    else
-                        walk1_kernel<true><<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
-                                                                                 c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
-                } else
-                    walk1_kernel<false><<<m, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m, d_qrows, d_q, c->s_qh0.as<float>(), d_pre, c->f_n_normals, w1debug, search_k,
-                                                                             c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl0);
+                }
+                const auto walk1 = multi ? &walk1_kernel<true, true> : filtered ? &walk1_kernel<true> : &walk1_kernel<false>;
+                const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
+                walk1<<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0, d_pre, c->f_n_normals, w1debug,
+                                                                 search_k, c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
                 CK(cudaGetLastError());
-                mark1();
+                mark();
                 walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
                 CK(cudaGetLastError());
-                mark1();
-                const uint64_t per = (c->metric == MANHATTAN || c->metric == BQ_MANHATTAN) ? 32 : 4;
-                const uint64_t warps = ((uint64_t)cand_cap + per - 1) / per;
-                const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / m)));
-                distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, d_q, d_qrows, c->s_qh0.as<float>(), m,
-                                                                   c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
-                CK(cudaGetLastError());
-                mark1();
-                topk_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), k, c->metric,
-                                                               c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
-                CK(cudaGetLastError());
+                mark();
+                // (no fused re-rank: its one CTA per query would leave all but <= 16 SMs idle)
+                rerank_segments(c, m, Q, c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), (uint64_t)cand_cap * m, cand_cap, k, false, &mark);
                 c->n_launches += 4;
                 bq_normalize(c, c->s_odist.as<float>(), (uint64_t)m * k);
-                mark1();
+                mark();
                 c->pin.ensure(std::max<size_t>(c->pin.cap, 4ull * m));
                 int32_t* h_st = c->pin.as<int32_t>();
                 CK(cudaMemcpyAsync(h_st, c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
-                CK(cudaMemcpyAsync(out_rows, c->s_orows.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-                CK(cudaMemcpyAsync(out_dist, c->s_odist.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-                CK(cudaMemcpyAsync(out_len, c->s_olen.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
-                CK(cudaStreamSynchronize(c->stream));
-                for (int i = 0; i + 1 < nte1; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); c->sbreak[i] += ms; }
+                copy_results(c, 0, m, k, out_rows, out_dist, out_len);
+                mark.add_to(c->sbreak);
                 bool all_ok = true;
                 for (uint32_t q = 0; q < m; ++q) all_ok = all_ok && h_st[q] == 0;
                 if (all_ok) {
@@ -1972,87 +1968,41 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
             c->w_count.ensure(4ull * m); c->w_bitmap.ensure(4ull * bm_words * m); c->w_status.ensure(4ull * m);
             c->w_beg.ensure(8ull * (m + 1)); c->w_end.ensure(8ull * (m + 1));
             c->s_keys.ensure(8ull * cand_cap * m); c->s_dists.ensure(4ull * cand_cap * m);
-            c->s_orows.ensure(4ull * m * k); c->s_odist.ensure(4ull * m * k); c->s_olen.ensure(4ull * m); c->s_qh0.ensure(4ull * m);
-            const uint32_t* d_qrows = nullptr;
-            const float* d_q = nullptr;
-            if (query_rows) {
-                c->w_qrows.ensure(4ull * m);
-                CK(cudaMemcpyAsync(c->w_qrows.p, query_rows + q0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
-                d_qrows = c->w_qrows.as<uint32_t>();
-            } else {
-                c->s_q.ensure((size_t)m * ld * 4);
-                CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)m * ld * 4, c->stream));
-                CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries + (size_t)q0 * c->dim, (size_t)c->dim * 4, (size_t)c->dim * 4, m, cudaMemcpyHostToDevice, c->stream));
-                d_q = c->s_q.as<float>();
-            }
-            if (qhdr0) CK(cudaMemcpyAsync(c->s_qh0.p, qhdr0 + q0, 4ull * m, cudaMemcpyHostToDevice, c->stream));
-            else if (query_rows) {  // by_item: the stored header of the item
-                gather_f32_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->s_qh0.as<float>(), c->h0.as<float>(), d_qrows, m);
-                CK(cudaGetLastError());
-            } else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
-            nte = 0; mark();
-            if (m_walk == 0) {   // every query of the chunk takes the shortcut: its segments are already sorted
+            c->s_orows.ensure(4ull * m * k); c->s_odist.ensure(4ull * m * k); c->s_olen.ensure(4ull * m);
+            const DevQueries Q = upload_queries(c, q0, m, query_rows, queries, qhdr0);
+            Marks mark{c};
+            mark();
+            if (m_walk == 0)   // every query of the chunk takes the shortcut: its segments are already sorted
                 shortcut(q0, 0, m, c->w_cand2.as<uint32_t>());
-                mark();
-                walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
-                CK(cudaGetLastError());
-            } else {
-            if (m_walk < m) shortcut(q0, m_walk, m, c->w_cand.as<uint32_t>());   // (multi only) sorted with the walked segments below
-            CK(cudaMemsetAsync(c->w_bitmap.p, 0, 4ull * bm_words * m_walk, c->stream));
-            if (multi) {
+            else {
+                if (m_walk < m) shortcut(q0, m_walk, m, c->w_cand.as<uint32_t>());   // (multi only) sorted with the walked segments below
+                CK(cudaMemsetAsync(c->w_bitmap.p, 0, 4ull * bm_words * m_walk, c->stream));
                 WalkFilter Fl = Fl0;
-                Fl.qfilter += q0;
-                walk_kernel<true, true><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q,
-                                                                                                        c->s_qh0.as<float>(), search_k, c->w_heaps.as<unsigned long long>(), heap_cap,
-                                                                                                        c->w_cand.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(),
-                                                                                                        bm_words, c->w_status.as<int32_t>(), Fl);
-            } else if (filtered)
-                walk_kernel<true><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(),
-                                                                                                  search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
-                                                                                                  c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl0);
-            else
-                walk_kernel<false><<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, d_qrows, d_q, c->s_qh0.as<float>(),
-                                                                                                   search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
-                                                                                                   c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl0);
-            CK(cudaGetLastError());
+                if (multi) Fl.qfilter += q0;
+                const auto walk = multi ? &walk_kernel<true, true> : filtered ? &walk_kernel<true> : &walk_kernel<false>;
+                walk<<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0,
+                                                                                                        search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
+                                                                                                        c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
+                CK(cudaGetLastError());
+            }
             mark();
             walk_segments_kernel<<<(m + 256) / 256, 256, 0, c->stream>>>(c->w_count.as<uint32_t>(), m, cand_cap, c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>());
             CK(cudaGetLastError());
-            // sort every query's unique candidates ascending (= ascending item ids): reader.rs:378
-            size_t tmp_bytes = 0;
-            CK(cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, c->w_cand.as<uint32_t>(), c->w_cand2.as<uint32_t>(), (int64_t)cand_cap * m, (int64_t)m,
-                                                  c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->stream));
-            c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
-            CK(cub::DeviceSegmentedSort::SortKeys(c->w_tmp.p, tmp_bytes, c->w_cand.as<uint32_t>(), c->w_cand2.as<uint32_t>(), (int64_t)cand_cap * m, (int64_t)m,
-                                                  c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->stream));
+            if (m_walk) {   // sort every query's unique candidates ascending (= ascending item ids): reader.rs:378
+                size_t tmp_bytes = 0;
+                CK(cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, c->w_cand.as<uint32_t>(), c->w_cand2.as<uint32_t>(), (int64_t)cand_cap * m, (int64_t)m,
+                                                      c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->stream));
+                c->w_tmp.ensure(std::max<size_t>(tmp_bytes, 16));
+                CK(cub::DeviceSegmentedSort::SortKeys(c->w_tmp.p, tmp_bytes, c->w_cand.as<uint32_t>(), c->w_cand2.as<uint32_t>(), (int64_t)cand_cap * m, (int64_t)m,
+                                                      c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->stream));
             }
             mark();
-            bool fused = frerank_enabled(c, k);
-            if (fused) {   // one fused kernel per query: bf16 pre-filter + exact re-score + top-k (frerank.cuh)
-                frerank_launch(c, m, d_q, d_qrows, c->s_qh0.as<float>(), c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), k);
-                CK(cudaStreamSynchronize(c->stream));
-                fused = frerank_ok(c, m);
-            }
-            if (!fused) {
-            uint64_t warps = ((uint64_t)cand_cap + 3) / 4;
-            uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / std::min<uint32_t>(m, c->sm_count * 8u))));
-            distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, d_q, d_qrows, c->s_qh0.as<float>(), m,
-                                                               c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
-            CK(cudaGetLastError());
-            mark();
-            topk_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), k, c->metric,
-                                                           c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
-            CK(cudaGetLastError());
-            } else mark();
+            rerank_segments(c, m, Q, c->w_cand2.as<uint32_t>(), c->w_beg.as<uint64_t>(), c->w_end.as<uint64_t>(), (uint64_t)cand_cap * m, cand_cap, k, true, &mark);
             c->n_launches += 5;
             bq_normalize(c, c->s_odist.as<float>(), (uint64_t)m * k);
             mark();
-            CK(cudaMemcpyAsync(out_rows + (size_t)q0 * k, c->s_orows.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaMemcpyAsync(out_dist + (size_t)q0 * k, c->s_odist.p, 4ull * m * k, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaMemcpyAsync(out_len + q0, c->s_olen.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
-            if (out_status) CK(cudaMemcpyAsync(out_status + q0, c->w_status.p, 4ull * m, cudaMemcpyDeviceToHost, c->stream));
-            CK(cudaStreamSynchronize(c->stream));
-            for (int i = 0; i + 1 < nte; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); c->sbreak[i] += ms; }
+            copy_results(c, q0, m, k, out_rows, out_dist, out_len, out_status);
+            mark.add_to(c->sbreak);
             filter_tally(m, m_walk);
             c->d2h_bytes += 8ull * m * k + 8ull * m;
         }
@@ -2169,8 +2119,7 @@ void multi_filter_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
                 h_offs.push_back(h_rows.size());
                 longest = std::max(longest, e - b);
             }
-            int nte = 0;
-            auto mark = [&]() { if (!c->xev[nte]) CK(cudaEventCreate(&c->xev[nte])); CK(cudaEventRecord(c->xev[nte], c->stream)); ++nte; };
+            Marks mark{c};
             mark();
             c->w_mrows.ensure(std::max<size_t>(16, 4ull * h_rows.size())); c->w_moffs.ensure(8ull * (nf + 1));
             c->w_msum.ensure(4ull * G.group_words * groups); c->w_ftotal.ensure(256ull * groups);
@@ -2200,7 +2149,7 @@ void multi_filter_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
             CK(cudaMemcpyAsync(ftotal.data(), c->w_ftotal.p, 256ull * groups, cudaMemcpyDeviceToHost, c->stream));
             mark();
             CK(cudaStreamSynchronize(c->stream));
-            { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[0], c->xev[1])); c->sbreak[5] += ms; CK(cudaEventElapsedTime(&ms, c->xev[1], c->xev[2])); c->sbreak[6] += ms; }
+            mark.add_to(c->sbreak + 5);   // the upload, the summaries
             c->h2d_bytes += 4ull * h_rows.size() + 8ull * (nf + 1);
             c->multi_stats[0] += groups; c->multi_stats[1] += nf;
             // this set's queries: those that walk, then those whose filter takes the shortcut, each in call order
@@ -2393,14 +2342,13 @@ int32_t arroy_b200_prefilter_scores(arroy_ctx* c, uint32_t nq, const float* quer
         if (c->dim < 32) throw ArgError("prefilter_scores needs dim >= 32");
         if (n_rows > 0x7fffffffull || (uint64_t)nq * n_rows > (1ull << 29)) throw ArgError("prefilter_scores: problem too large");
         for (uint64_t i = 0; i < n_rows; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
-        const uint32_t ld = c->ld, nc = (uint32_t)n_rows, lds = (nc + 3u) & ~3u;
+        const uint32_t nc = (uint32_t)n_rows, lds = (nc + 3u) & ~3u;
         c->s_rows.ensure(4ull * nc);
         CK(cudaMemcpyAsync(c->s_rows.p, rows, 4ull * nc, cudaMemcpyHostToDevice, c->stream));
         const float* cand = xf_candidates(c, rows, nc);
-        c->s_q.ensure((size_t)nq * ld * 4); c->x_S.ensure(4ull * nq * lds);
-        CK(cudaMemsetAsync(c->s_q.p, 0, (size_t)nq * ld * 4, c->stream));
-        CK(cudaMemcpy2DAsync(c->s_q.p, (size_t)ld * 4, queries, (size_t)c->dim * 4, (size_t)c->dim * 4, nq, cudaMemcpyHostToDevice, c->stream));
-        xf_scores(c, c->s_q.as<float>(), nq, cand, nc, c->x_S.as<float>(), lds, TgEpilogue{TG_RAW, nullptr, nullptr, nullptr, nullptr}, engine);
+        c->x_S.ensure(4ull * nq * lds);
+        const DevQueries Q = upload_queries(c, 0, nq, nullptr, queries, nullptr);
+        xf_scores(c, Q.vecs, nq, cand, nc, c->x_S.as<float>(), lds, TgEpilogue{TG_RAW, nullptr, nullptr, nullptr, nullptr}, engine);
         CK(cudaMemcpy2DAsync(out_scores, 4ull * nc, c->x_S.p, 4ull * lds, 4ull * nc, nq, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
     });
