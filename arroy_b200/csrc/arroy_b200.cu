@@ -474,8 +474,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     if (ctrl_smem > 48 * 1024) CK(cudaFuncSetAttribute(control_fn(true, 1, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
     const size_t wsmem = work_smem(ld, (int)tw);
     if (wsmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-    const size_t perm_smem = 4ull * planes_perm_floats(ld);   // work_kernel_shadow's second copy of the normal
-    if (wsmem + perm_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + perm_smem)));
+    const size_t limb_smem = (size_t)PLANES_LIMBS * ld;   // work_kernel_shadow's limbs of the normal
+    if (wsmem + limb_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + limb_smem)));
     const int work_grid = c->sm_count * 3;
 
     // Three schedules over the same kernels:
@@ -577,7 +577,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
                 CK(cudaStreamWaitEvent(st, c->tree_events[0], 0));
                 for (int i = 0; i < ASYNC_BATCH; ++i) {
                     launch_control(ctrlc, 1, cluster, ctrl_smem, st, P, t);
-                    if (P.planes.hi) work_kernel_shadow<<<c->sm_count, WORK_THREADS, wsmem1 + perm_smem, st>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+                    if (P.planes.hi) work_kernel_shadow<<<c->sm_count, WORK_THREADS, wsmem1 + limb_smem, st>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
                     else work_kernel<<<c->sm_count, WORK_THREADS, wsmem1, st>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric);
                 }
                 CK(cudaEventRecord(c->tree_events[1 + t], st));
@@ -650,7 +650,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             for (int i = 0; i < LOCKSTEP_BATCH; ++i) {
                 launch_control(ctrl1, tw, 1, ctrl_smem, c->stream, P, 0u);
                 if (profile) CK(cudaEventRecord(pev[2 * i], c->stream));
-                if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + perm_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
+                if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + limb_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
                 else work_kernel<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric);
                 if (profile) CK(cudaEventRecord(pev[2 * i + 1], c->stream));
             }
@@ -2251,8 +2251,10 @@ int32_t arroy_b200_time_scan(arroy_ctx* c, const float* normal, float hdr0, floa
                              int32_t flush_l2, float* out_ms_avg, uint64_t* out_left_count) {
     return guarded(c, [&] {
         require_staged(c); set_device(c);
-        (void)variant;
-        if (!normal || !out_ms_avg || n_rows == 0 || n_rows > c->n || iters <= 0) throw ArgError("bad argument");
+        if (!normal || !out_ms_avg || n_rows == 0 || n_rows > c->n || iters <= 0 || (variant != 0 && variant != 1)) throw ArgError("bad argument");
+        const bool planes = variant == 1;
+        if (planes && (is_bq(c->metric) || c->dim < 64 || c->dim > PLANES_MAX_D)) throw ArgError("time_scan variant 1 needs a float metric and 64 <= dim <= PLANES_MAX_D");
+        if (planes) planes_prepare(c);
         upload_normal(c, normal, hdr0, hdr1);
         CK(cudaStreamSynchronize(c->stream));
         c->s_flags.ensure(n_rows);
@@ -2270,14 +2272,27 @@ int32_t arroy_b200_time_scan(arroy_ctx* c, const float* normal, float hdr0, floa
         CK(cudaMemcpyAsync(c->s_job.p, &jb, sizeof(Job), cudaMemcpyHostToDevice, c->stream));
         int grid = (int)std::min<uint64_t>(units, (uint64_t)c->sm_count * 3);
         const size_t flush_bytes = 256ull << 20;
-        if (flush_l2) c->s_misc.ensure(flush_bytes);
-        launch_work(c, c->s_job.as<Job>(), 1, grid);  // warm-up
+        // variant 1: work_kernel_shadow on the one job with every unit through the 8-bit pre-filter (scan_claim_planes), two CTAs
+        // per SM as in the build; the stage counts of its last launch are what build_prefilter_stats reports afterwards
+        const size_t stats_off = flush_l2 ? flush_bytes : 0;
+        c->s_misc.ensure(stats_off + 32);
+        unsigned long long* pstats = reinterpret_cast<unsigned long long*>(c->s_misc.as<uint8_t>() + stats_off);
+        const size_t psmem = work_smem(c->ld, 1) + (size_t)PLANES_LIMBS * c->ld;
+        if (planes && psmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+        auto launch = [&] {
+            if (!planes) { launch_work(c, c->s_job.as<Job>(), 1, grid); return; }
+            work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, psmem, c->stream>>>(c->s_job.as<Job>(), 1, c->items.as<float>(),
+                PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}, c->h0.as<float>(), c->dim, c->ld, c->metric, 0u, pstats);
+            CK(cudaGetLastError());
+        };
+        launch();  // warm-up
         CK(cudaStreamSynchronize(c->stream));
         double total_ms = 0;
         for (int it = 0; it < iters; ++it) {
             if (flush_l2) CK(cudaMemsetAsync(c->s_misc.p, it & 0xff, flush_bytes, c->stream));
+            if (planes) CK(cudaMemsetAsync(pstats, 0, 24, c->stream));
             CK(cudaEventRecord(c->ev0, c->stream));
-            launch_work(c, c->s_job.as<Job>(), 1, grid);
+            launch();
             CK(cudaEventRecord(c->ev1, c->stream));
             CK(cudaEventSynchronize(c->ev1));
             float ms = 0;
@@ -2285,6 +2300,12 @@ int32_t arroy_b200_time_scan(arroy_ctx* c, const float* normal, float hdr0, floa
             total_ms += ms;
         }
         *out_ms_avg = (float)(total_ms / iters);
+        if (planes) {
+            unsigned long long hs[3] = {0, 0, 0};
+            CK(cudaMemcpyAsync(hs, pstats, 24, cudaMemcpyDeviceToHost, c->stream));
+            CK(cudaStreamSynchronize(c->stream));
+            c->shadow_rows = hs[0]; c->shadow_rescored = hs[1]; c->shadow_stage2 = hs[2]; c->fused_root_rows = 0; c->fused_root_read = 0;
+        }
         if (out_left_count) {
             std::vector<uint32_t> ul(units);
             CK(cudaMemcpyAsync(ul.data(), c->s_unit.p, units * 4, cudaMemcpyDeviceToHost, c->stream));

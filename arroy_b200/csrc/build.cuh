@@ -967,15 +967,15 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ uint32_t w_sm[16];
     __shared__ uint32_t w_list[SCAN_UNIT * PLANES_CHUNK], w_list2[SCAN_UNIT * PLANES_CHUNK];   // positions stage 1 / stage 2 could not decide
     __shared__ uint32_t w_cnt[PLANES_CHUNK + 2];
-    __shared__ double w_l1[CTRL_THREADS / 32];
-    float* sm_perm = sm_normal + P.ld;                      // the normal in the planes' lane order
+    __shared__ PlanesScratch w_sc;
+    __shared__ PlanesNormal w_pn;                           // the loaded normal's pre-filter factors (scan_claim_planes)
+    uint8_t* sm_limbs = reinterpret_cast<uint8_t*>(sm_normal + P.ld);   // and its limbs
     const uint32_t T = P.n_trees;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t rot = (blockIdx.x - T) * 7u;
     const bool latency_class = ((blockIdx.x - T) & LAT_MASK) == 0u;
     uint32_t loaded_t = 0xffffffffu, loaded_seq = 0xffffffffu;
     float nh0 = 0.f;
-    float2 wf = make_float2(0.f, 0.f);   // the loaded normal's bound factors (scan_claim_planes)
     if (tid == 0) w_exit = 0;
     if (P.root_fused) proot(P, sm_normal);
     for (;;) {
@@ -1055,24 +1055,30 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
                 if (want_normal || seq != w_pseq) {
                     double l1 = 0.0;
+                    uint32_t mb = 0;
 #pragma unroll
                     for (int u = 0; u < 8; ++u) {
                         const uint32_t i = tid + u * CTRL_THREADS;
                         if (i < P.ld) {
                             sm_normal[i] = nreg[u];
-                            if (P.planes.hi != nullptr) { sm_perm[planes_perm_index(i)] = nreg[u]; l1 += (double)fabsf(nreg[u]); }
+                            l1 += (double)fabsf(nreg[u]);
+                            mb = max(mb, __float_as_uint(fabsf(nreg[u])));
                         }
                     }
-                    if (P.planes.hi != nullptr) { l1 = warp_sum_f64(l1); if (lane == 0) w_l1[warp] = l1; }
+                    if (P.planes.hi != nullptr) {
+                        l1 = warp_sum_f64(l1);
+                        mb = __reduce_max_sync(0xffffffffu, mb);
+                        if (lane == 0) { w_sc.l1[warp] = l1; w_sc.mx[warp] = mb; }
+                    }
                     nh0 = __ldcg(nsrc);
                     loaded_t = t; loaded_seq = seq;
                     __syncthreads();
-                    if (P.planes.hi != nullptr) wf = planes_job_factors(w_l1, P.d);
+                    if (P.planes.hi != nullptr && units > P.shadow_min_units) planes_job_factors(sm_normal, P.ld, P.d, sm_limbs, w_sc, &w_pn);
                 }
                 if (P.planes.hi != nullptr && units > P.shadow_min_units)
                     for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
-                        scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_perm, nh0,
-                                          wf.x, wf.y, w_list, w_list2, w_cnt, P.shadow_stats);
+                        scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_limbs,
+                                          &w_pn, nh0, w_list, w_list2, w_cnt, P.shadow_stats);
                 else
                     for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
             } else if (jb.kind == JOB_PARTITION) {

@@ -150,32 +150,32 @@ __device__ __forceinline__ void scan_unit(const Job& jb, uint32_t unit, const fl
 // A row whose scale is not a normal finite f32 keeps zero planes and is never decided through them: M = 0 stores s = 0 (the
 // row's dot is exactly 0), M = inf stores +inf, a NaN or tiny (M < 127 FLT_MIN) row stores NaN (0x7fffffff); the tests below
 // are false for NaN and +inf.
+// The normal is read as integer limbs, so that both stages are exact integer dot products (IDP.4A). Once per job, with sigma the
+// least power of two above max_i |n_i| / 127 and t_i = n_i / sigma (exact, |t_i| < 127):
+//     a_i = rint(t_i),  b_i = rint(254 (t_i - a_i)),  c_i = rint(254 (254 (t_i - a_i) - b_i)),  U_i = ceil(2 |t_i|)
+// (every step exact in f64; |a|, |b|, |c| <= 127, U <= 254), n1_i = sigma (a_i + b_i / 254), n2_i = n1_i + sigma c_i / 254^2,
+// |n_i| <= sigma U_i / 2, and D1 >= sum |n_i - n1_i|, D2 >= sum |n_i - n2_i| are summed in f64 and rounded up, as is N1 >= |n|_1.
 // The reference's margin is fl(dot + c) (c = the bias / extra-dim term, formed exactly as the reference forms it; fl keeps the
 // sign of dot + c), with |dot - sum n_i x_i| <= gamma_R sum |n_i x_i|, gamma_R <= 1.001 d u in any summation order, and
-// sum |n_i x_i| <= 127.001 s |n|_1. A lane sums a row in two f32 chains of at most ld/16 + 7 terms, then 1 + 3 adds: gamma_k <=
-// (d/8 + 16) u for either stage. N1 >= |n|_1 is summed in f64 once per job and rounded up.
-//  stage 1, hi plane only (d bytes per row): t = f32 sum n_i h_i (sum |n_i h_i| <= 127 |n|_1), and
-//    |dot - fl(s t)| <= s |n|_1 (E1 + 127.001 (gamma_R + gamma_k + u)) <= s N1 K1(d) / (1 + 2^-20),  K1(d) = 0.5002 + 8.6e-6 d;
-//    the row is certain when |fl(fl(s t) + c)| > fl(s w1), w1 = N1 K1(d) rounded up (the factor 1 + 2^-20 covers the test's
-//    own roundings).
-//  stage 2, the rows stage 1 left (both planes; the hi row was just streamed by this CTA): m = f32 sum n_i y_i,
-//    A = f32 sum |n_i| |y_i|, s2 = fl(s / 254), and
-//    |dot - fl(s2 m)| <= s2 (254 E2 |n|_1 (1 + gamma_R) + A (gamma_R + gamma_k + 4 u)) <= s2 (N1 W2(d) + rel2(d) A) / (1 + 2^-20),
-//    W2(d) = 0.50216 (1 + 6.1e-8 (d + 16)), rel2(d) = 1.3e-6 + 6.8e-8 d; certain when |fl(fl(s2 m) + c)| > fl(s2 fl(w2 + fl(rel2 A))),
-//    w2 = N1 W2(d) rounded up.
+// |x_i| <= M <= 127.001 s.
+//  stage 1, hi plane only (d bytes per row): T1 = 254 sum h_i a_i + sum h_i b_i, an exact integer (each int32 sum is at most
+//    127 * 127 * 8192 < 2^31 in magnitude for d <= PLANES_MAX_D), so s sigma T1 / 254 = s sum h_i n1_i and
+//    |dot - s sum h_i n1_i| <= s (E1 N1 + 127 D1 + 127.001 gamma_R N1).
+//    The row is certain when |p + c| > s w1 in f64, p = fl(fl(T1 s) k1), k1 = fl(sigma / 254), w1 = (N1 (E1 + 127.001 gamma_R)
+//    + 127 D1) (1 + 2^-20) rounded up: the factor 1 + 2^-20 covers the relative errors of p (3 roundings on |p| <= 254 s N1)
+//    and of the test (2^-53 each).
+//  stage 2, the rows stage 1 left (both planes; the hi row was just streamed by this CTA): y_i = 254 h_i + l_i (|y_i| <= 32385),
+//    T2 = sum y_i (254^2 a_i + 254 b_i + c_i) from the six int32 sums of h, l times a, b, c (|T2| <= 2.2e15 < 2^53: exact in f64),
+//    so s sigma T2 / 254^3 = (s / 254) sum y_i n2_i, and with A = 254 sum |h_i| U_i + sum |l_i| U_i (sum |n_i| |y_i| <= sigma A / 2):
+//    |dot - (s/254) sum y_i n2_i| <= s E2 N1 + (s/254) 32385 D2 + gamma_R ((s/254) sigma A / 2 + s E2 N1)
+//                                  = (s/254) (254 E2 (1 + gamma_R) N1 + 32385 D2 + gamma_R sigma A / 2).
+//    The row is certain when |p2 + c| > s (w2 + rel2 A) in f64, p2 = fl(fl(T2 s) k2), k2 = fl(sigma / 254^3),
+//    w2 = (254 E2 (1 + gamma_R) N1 + 32385 D2) (1 + 2^-20) / 254, rel2 = gamma_R sigma / 508 (1 + 2^-20), both rounded up (the
+//    factor covers p2's 3 roundings on |p2| <= 255 s N1 and the test's own).
 //  stage 3: every other row — near the hyperplane, zero, non-finite — is scored from the f32 row in the reference's summation
 //    order (scan_unit's arithmetic). Flags and unit counts are the exact scan's.
-// The bounds are relative: like any such rule they assume that no product n_i x_i underflows.
-// sm_perm: the normal re-laid for the planes' lane order: the 16 elements of 16-byte word q = 8 c + g of a row sit at float4
-// 32 c + 8 j + g (j = 0..3, four elements each), so that the eight lanes of a row read consecutive float4s.
-__host__ __device__ __forceinline__ float planes_k1(uint32_t d) { return 0.5002f + (float)d * 8.6e-6f; }
-__host__ __device__ __forceinline__ float planes_w2(uint32_t d) { return 0.50216f * (1.0f + 6.1e-8f * (float)(d + 16u)); }
-__host__ __device__ __forceinline__ float planes_rel2(uint32_t d) { return 1.3e-6f + (float)d * 6.8e-8f; }
-__host__ __device__ __forceinline__ uint32_t planes_perm_floats(uint32_t ld) { return (ld + 127u) & ~127u; }   // sm_perm's size
-__host__ __device__ __forceinline__ uint32_t planes_perm_index(uint32_t i) {
-    const uint32_t q = i >> 4, w = i & 15u;
-    return (((q >> 3) * 32u + (w >> 2) * 8u + (q & 7u)) << 2) + (w & 3u);
-}
+// A normal with a non-finite element gets NaN factors: no row is certain. The bounds are relative: like any such rule they assume
+// that no product n_i x_i underflows.
 constexpr uint32_t PLANES_MAX_D = 8192;
 constexpr uint32_t PLANES_CHUNK = 4;          // scan units per claim on this path (256 rows)
 
@@ -229,55 +229,49 @@ __device__ __forceinline__ uint4 ldg_stream_u4(const uint4* p) {
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
-// byte k of w (signed) as a float, without I2F: b ^ 0x80 = b + 128 is put into the mantissa of 2^23 (exactly 2^23 + 128 + b),
-// one add removes the offset. wx = w ^ 0x80808080.
-__device__ __forceinline__ float s8_to_f32(uint32_t wx, uint32_t k) {
-    return __fsub_rn(__uint_as_float(__byte_perm(wx, 0x4B000000u, 0x7540u | k)), 8388736.0f);
+// sum over the 16 bytes of x and y of x_k y_k: signed (planes times a, b, c limbs) and unsigned (|h|, |l| times U)
+__device__ __forceinline__ int dp16(const uint4 x, const uint4 y, int acc) {
+    acc = __dp4a((int)x.x, (int)y.x, acc); acc = __dp4a((int)x.y, (int)y.y, acc);
+    acc = __dp4a((int)x.z, (int)y.z, acc); return __dp4a((int)x.w, (int)y.w, acc);
 }
-// 16 hi-plane elements of one word times their normal elements (y: the four float4s of sm_perm for this word): two chains
-__device__ __forceinline__ void planes_fma16(const uint4 v, const float4 (&y)[4], float& m0, float& m1) {
-    const uint32_t w[4] = {v.x ^ 0x80808080u, v.y ^ 0x80808080u, v.z ^ 0x80808080u, v.w ^ 0x80808080u};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        m0 = fmaf(s8_to_f32(w[j], 0), y[j].x, m0); m1 = fmaf(s8_to_f32(w[j], 1), y[j].y, m1);
-        m0 = fmaf(s8_to_f32(w[j], 2), y[j].z, m0); m1 = fmaf(s8_to_f32(w[j], 3), y[j].w, m1);
-    }
+__device__ __forceinline__ uint32_t dp16u(const uint4 x, const uint4 y, uint32_t acc) {
+    acc = __dp4a(x.x, y.x, acc); acc = __dp4a(x.y, y.y, acc);
+    acc = __dp4a(x.z, y.z, acc); return __dp4a(x.w, y.w, acc);
 }
-// the same word of both planes: y = 254 h + l (exact), m += n y, a += |n| |y|
-__device__ __forceinline__ void planes_fma16x2(const uint4 vh, const uint4 vl, const float4 (&y)[4], float& m0, float& m1, float& a0, float& a1) {
-    const uint32_t wh[4] = {vh.x ^ 0x80808080u, vh.y ^ 0x80808080u, vh.z ^ 0x80808080u, vh.w ^ 0x80808080u};
-    const uint32_t wl[4] = {vl.x ^ 0x80808080u, vl.y ^ 0x80808080u, vl.z ^ 0x80808080u, vl.w ^ 0x80808080u};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float n4[4] = {y[j].x, y[j].y, y[j].z, y[j].w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float v = fmaf(s8_to_f32(wh[j], (uint32_t)k), 254.0f, s8_to_f32(wl[j], (uint32_t)k));
-            if (k & 1) { m1 = fmaf(v, n4[k], m1); a1 = fmaf(fabsf(v), fabsf(n4[k]), a1); }
-            else { m0 = fmaf(v, n4[k], m0); a0 = fmaf(fabsf(v), fabsf(n4[k]), a0); }
-        }
-    }
+// |b| of every signed byte b of w (the planes hold no -128): b ^ 0x80 = b + 128 as an unsigned byte, its distance to 128
+__device__ __forceinline__ uint4 abs_bytes(const uint4 w) {
+    return make_uint4(__vabsdiffu4(w.x ^ 0x80808080u, 0x80808080u), __vabsdiffu4(w.y ^ 0x80808080u, 0x80808080u),
+                      __vabsdiffu4(w.z ^ 0x80808080u, 0x80808080u), __vabsdiffu4(w.w ^ 0x80808080u, 0x80808080u));
 }
 
-__device__ __forceinline__ float prefilter_finish(int metric, float v, float nh0, float item_h0) {
-    if (metric == COSINE) return v;
-    if (metric == DOT_PRODUCT) return __fadd_rn(v, __fmul_rn(nh0, item_h0));
-    return __fadd_rn(nh0, v);
+// A job's normal as the pre-filter reads it: the limbs a, b, c, U (above) as four ld-byte arrays in shared memory, natural
+// element order, and its factors.
+struct PlanesNormal {
+    double w1, k1;               // stage 1: bound factor, sigma / 254
+    double w2, rel2, k2;         // stage 2: bound factors, sigma / 254^3
+};
+constexpr uint32_t PLANES_LIMBS = 4;   // ld bytes each
+
+__device__ __forceinline__ double prefilter_c(int metric, float nh0, float item_h0) {
+    if (metric == COSINE) return 0.0;
+    if (metric == DOT_PRODUCT) return (double)__fmul_rn(nh0, item_h0);
+    return (double)nh0;
 }
 
 // scan units [u0, u1) (at most PLANES_CHUNK) of a job. sm_list, sm_list2: 64 * PLANES_CHUNK positions each (the rows stage 1,
-// stage 2 left); sm_cnt: PLANES_CHUNK + 2 counters. w1, w2: the job's bound factors (above). stats (optional): [0] rows through
-// the pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
+// stage 2 left); sm_cnt: PLANES_CHUNK + 2 counters. limbs, pn: the job's normal as planes_job_factors left it. stats (optional):
+// [0] rows through the pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
 __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, uint32_t u1, const float* __restrict__ items, const PlaneRows pl,
-                                                  const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric, const float* sm_normal, const float* sm_perm,
-                                                  float nh0, float w1, float w2, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt, unsigned long long* stats) {
+                                                  const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric, const float* sm_normal, const uint8_t* limbs,
+                                                  const PlanesNormal* pn, float nh0, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt, unsigned long long* stats) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
     if (tid <= (int)PLANES_CHUNK + 1) sm_cnt[tid] = 0;
     __syncthreads();
     const uint32_t base = u0 * SCAN_UNIT, end = min(jb.len, u1 * SCAN_UNIT);
     const uint32_t nq = ld >> 4;                       // 16-byte words per plane row
     const int nsteps = (int)((nq + 7) >> 3);
-    const float4* PN = reinterpret_cast<const float4*>(sm_perm);
+    const uint4* LA = reinterpret_cast<const uint4*>(limbs);
+    const uint4* LB = LA + nq;
     // ---- stage 1: the hi plane of every row ----
     for (uint32_t pbase = base; pbase < end; pbase += 128) {
         uint32_t pos[4], rid[4];
@@ -288,9 +282,9 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
             rid[r] = pos[r] < end ? (jb.rows ? __ldcg(jb.rows + pos[r]) : pos[r]) : 0u;
             S[r] = reinterpret_cast<const uint4*>(pl.hi + (size_t)rid[r] * ld) + g8;
         }
-        float m0[4], m1[4];
+        int sa[4], sb[4];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) { m0[r] = 0.f; m1[r] = 0.f; }
+        for (int r = 0; r < 4; ++r) { sa[r] = 0; sb[r] = 0; }
         for (int c0 = 0; c0 < nsteps; c0 += 3) {
             uint4 v[3][4];
 #pragma unroll
@@ -303,24 +297,23 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
 #pragma unroll
             for (int sidx = 0; sidx < 3; ++sidx) {
                 const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                float4 y[4];
+                const uint4 la = q < nq ? LA[q] : make_uint4(0u, 0u, 0u, 0u), lb = q < nq ? LB[q] : make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
-                for (int j = 0; j < 4; ++j) y[j] = q < nq ? PN[(c0 + sidx) * 32 + j * 8 + g8] : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                for (int r = 0; r < 4; ++r) planes_fma16(v[sidx][r], y, m0[r], m1[r]);
+                for (int r = 0; r < 4; ++r) { sa[r] = dp16(v[sidx][r], la, sa[r]); sb[r] = dp16(v[sidx][r], lb, sb[r]); }
             }
         }
+        const double w1 = pn->w1, k1 = pn->k1;
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-            float t = m0[r] + m1[r];
 #pragma unroll
-            for (int o = 1; o < 8; o <<= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+            for (int o = 1; o < 8; o <<= 1) { sa[r] += __shfl_xor_sync(0xffffffffu, sa[r], o); sb[r] += __shfl_xor_sync(0xffffffffu, sb[r], o); }
             const bool valid = pos[r] < end;
             const float s = valid ? __ldg(pl.scale + rid[r]) : 0.f;
-            const float mt = prefilter_finish(metric, __fmul_rn(s, t), nh0, (metric == DOT_PRODUCT && valid) ? ih0[rid[r]] : 0.f);
-            const bool certain = fabsf(mt) > __fmul_rn(s, w1);      // false for NaN / Inf scales
+            const double t1 = (double)(254ll * sa[r] + sb[r]);
+            const double mt = __dadd_rn(__dmul_rn(__dmul_rn(t1, (double)s), k1), prefilter_c(metric, nh0, (metric == DOT_PRODUCT && valid) ? ih0[rid[r]] : 0.f));
+            const bool certain = fabs(mt) > __dmul_rn((double)s, w1);      // false for NaN / Inf scales and NaN factors
             const bool leader = g8 == 0 && valid;
-            const int side = mt > 0.f ? 1 : 0;
+            const int side = mt > 0.0 ? 1 : 0;
             if (leader && certain) jb.flags[pos[r]] = (uint8_t)side;
             if (leader && !certain) sm_list[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = pos[r];
             const unsigned lefts = __ballot_sync(0xffffffffu, leader && certain && side == 0);
@@ -331,7 +324,8 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
     __syncthreads();
     // ---- stage 2: both planes of the rows stage 1 left, one 8-lane group per row ----
     const uint32_t n1 = sm_cnt[PLANES_CHUNK];
-    const float rel2 = planes_rel2(d);
+    const uint4* LC = LB + nq;
+    const uint4* LU = LC + nq;
     for (uint32_t it = 0; it * 32u < n1; ++it) {
         const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
         const bool act = idx < n1;
@@ -339,7 +333,8 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         const uint32_t r = jb.rows ? __ldcg(jb.rows + p) : p;
         const uint4* Hr = reinterpret_cast<const uint4*>(pl.hi + (size_t)r * ld) + g8;
         const uint4* Lr = reinterpret_cast<const uint4*>(pl.lo + (size_t)r * ld) + g8;
-        float m0 = 0.f, m1 = 0.f, a0 = 0.f, a1 = 0.f;
+        int ha = 0, hb = 0, hc = 0, la = 0, lb = 0, lc = 0;
+        uint32_t hu = 0, lu = 0;
         for (int c0 = 0; c0 < nsteps; c0 += 3) {
             uint4 vh[3], vl[3];
 #pragma unroll
@@ -351,19 +346,23 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
 #pragma unroll
             for (int sidx = 0; sidx < 3; ++sidx) {
                 const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                float4 y[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) y[j] = q < nq ? PN[(c0 + sidx) * 32 + j * 8 + g8] : make_float4(0.f, 0.f, 0.f, 0.f);
-                planes_fma16x2(vh[sidx], vl[sidx], y, m0, m1, a0, a1);
+                if (q < nq) {   // the rows' words past nq were loaded as zeros
+                    const uint4 na = LA[q], nb = LB[q], nc = LC[q], nu = LU[q];
+                    ha = dp16(vh[sidx], na, ha); hb = dp16(vh[sidx], nb, hb); hc = dp16(vh[sidx], nc, hc);
+                    la = dp16(vl[sidx], na, la); lb = dp16(vl[sidx], nb, lb); lc = dp16(vl[sidx], nc, lc);
+                    hu = dp16u(abs_bytes(vh[sidx]), nu, hu); lu = dp16u(abs_bytes(vl[sidx]), nu, lu);
+                }
             }
         }
-        float m = m0 + m1, a = a0 + a1;
+        // this lane's share of T2 and A: integers below 2^53, so the doubles and their butterfly are exact
+        double m = (double)(16387064ll * ha + 64516ll * (hb + la) + 254ll * (hc + lb) + lc);
+        double a = (double)(254ull * hu + lu);
 #pragma unroll
         for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
-        const float s2 = __fdiv_rn(__ldg(pl.scale + r), 254.0f);
-        const float mt = prefilter_finish(metric, __fmul_rn(s2, m), nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f);
-        const bool certain = fabsf(mt) > __fmul_rn(s2, __fadd_rn(w2, __fmul_rn(rel2, a)));
-        const int side = mt > 0.f ? 1 : 0;
+        const float s = __ldg(pl.scale + r);
+        const double mt = __dadd_rn(__dmul_rn(__dmul_rn(m, (double)s), pn->k2), prefilter_c(metric, nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f));
+        const bool certain = fabs(mt) > __dmul_rn((double)s, __dadd_rn(pn->w2, __dmul_rn(pn->rel2, a)));
+        const int side = mt > 0.0 ? 1 : 0;
         if (act && g8 == 0) {
             if (certain) { jb.flags[p] = (uint8_t)side; if (side == 0) atomicAdd(&sm_cnt[(p - base) / SCAN_UNIT], 1u); }
             else sm_list2[atomicAdd(&sm_cnt[PLANES_CHUNK + 1], 1u)] = p;
@@ -411,18 +410,61 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
     if (tid < (int)(u1 - u0)) jb.unit_left[u0 + tid] = sm_cnt[tid];
 }
 
-// The bound factors of a job's normal from the per-warp partial sums of |n_i| (f64, eight warps): {w1, w2}, rounded up.
-__device__ __forceinline__ float2 planes_job_factors(const double* sm_l1, uint32_t d) {
-    double s = 0.0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) s += sm_l1[w];
-    s *= 1.0 + 0x1p-30;    // the f64 sum's own rounding (< 8192 * 2^-53)
-    return make_float2(__double2float_ru(s * (double)planes_k1(d)), __double2float_ru(s * (double)planes_w2(d)));
-}
 __device__ __forceinline__ double warp_sum_f64(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// Per-warp partials of planes_job_factors (eight warps): the caller's sum of |n_i| and max |n_i| (as bits, NaN above +inf), then
+// the limb errors.
+struct PlanesScratch { double l1[8], d1[8], d2[8]; uint32_t mx[8]; };
+
+// The pre-filter's view of a job's normal (above). The caller has written sm_normal (ld floats) and sc.l1 / sc.mx, then passed a
+// CTA barrier. Writes the limbs and, after one more barrier, pn (thread 0; scan_claim_planes reads it after its first barrier).
+__device__ __forceinline__ void planes_job_factors(const float* sm_normal, uint32_t ld, uint32_t d, uint8_t* limbs, PlanesScratch& sc, PlanesNormal* pn) {
+    uint32_t mb = 0;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) mb = max(mb, sc.mx[w]);
+    const bool finite = mb < 0x7f800000u;
+    int e = 0;                                        // sigma = 2^e > max |n_i| / 127 (f64 rounding is monotone)
+    if (finite && mb != 0u) frexp((double)__uint_as_float(mb) / 127.0, &e);
+    const double inv = ldexp(1.0, -e);
+    double d1 = 0.0, d2 = 0.0;
+    for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) {
+        const double t = finite ? (double)sm_normal[i] * inv : 0.0;     // every step exact (at most 40 significant bits)
+        const double a = rint(t), r1 = 254.0 * (t - a), b = rint(r1), r2 = 254.0 * (r1 - b), c = rint(r2);
+        limbs[i] = (uint8_t)(int)a;
+        limbs[ld + i] = (uint8_t)(int)b;
+        limbs[2 * ld + i] = (uint8_t)(int)c;
+        limbs[3 * ld + i] = (uint8_t)(int)ceil(2.0 * fabs(t));
+        d1 += fabs(r1 - b);                           // |n_i - n1_i| = sigma |r1 - b| / 254
+        d2 += fabs(r2 - c);                           // |n_i - n2_i| = sigma |r2 - c| / 254^2
+    }
+    d1 = warp_sum_f64(d1);
+    d2 = warp_sum_f64(d2);
+    if ((threadIdx.x & 31) == 0) { sc.d1[threadIdx.x >> 5] = d1; sc.d2[threadIdx.x >> 5] = d2; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double n1 = 0.0, s1 = 0.0, s2 = 0.0;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) { n1 += sc.l1[w]; s1 += sc.d1[w]; s2 += sc.d2[w]; }
+        const double g = 1.0 + 0x1p-30, slack = 1.0 + 0x1p-20, u = 0x1p-24;   // g: the f64 sums' own rounding (< 8192 * 2^-53)
+        // sigma / q rounded up as sigma times 1 / q rounded up (sigma is a power of two: that product is exact)
+        const double sigma = ldexp(1.0, e), r254 = 0x1.0204081020409p-8, r64516 = 0x1.040c2050c1c41p-16;
+        n1 = __dmul_ru(n1, g);
+        const double D1 = __dmul_ru(__dmul_ru(s1, g), sigma * r254), D2 = __dmul_ru(__dmul_ru(s2, g), sigma * r64516);
+        const double gR = __dmul_ru(1.001 * u, (double)d);
+        const double E1 = 0.5 + 128.0 * u, E2x254 = 0.5 + 32766.0 * u;
+        PlanesNormal f;
+        f.w1 = __dmul_ru(__dadd_ru(__dmul_ru(n1, __dadd_ru(E1, __dmul_ru(127.001, gR))), __dmul_ru(127.0, D1)), slack);
+        f.w2 = __dmul_ru(__dmul_ru(__dadd_ru(__dmul_ru(__dmul_ru(n1, E2x254), __dadd_ru(1.0, gR)), __dmul_ru(32385.0, D2)), slack), r254);
+        f.rel2 = __dmul_ru(__dmul_ru(gR, sigma * (0.5 * r254)), slack);
+        f.k1 = sigma * (1.0 / 254.0);
+        f.k2 = sigma * (1.0 / 16387064.0);
+        if (!finite) { f.w1 = __longlong_as_double(0x7ff8000000000000ll); f.w2 = f.w1; }
+        *pn = f;
+    }
 }
 
 // Stable partition of one PART_UNIT block of ids. left_before = number of Left flags in all
@@ -502,20 +544,21 @@ work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ i
 }
 
 // work_kernel for contexts that hold the 8-bit planes of the items: scan jobs of more than min_units units are cut into items of
-// PLANES_CHUNK units and go through scan_claim_planes; everything else is work_kernel's. Shared memory: the normal, the normal in
-// the planes' lane order (planes_perm_floats(ld) floats) and the prefix table.
+// PLANES_CHUNK units and go through scan_claim_planes; everything else is work_kernel's. Shared memory: the normal, its limbs
+// (PLANES_LIMBS * ld bytes) and the prefix table.
 __global__ void __launch_bounds__(WORK_THREADS, 2)
 work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const PlaneRows planes, const float* __restrict__ ih0,
                    uint32_t d, uint32_t ld, int metric, uint32_t min_units, unsigned long long* stats) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sm_normal = reinterpret_cast<float*>(smem_raw);
-    float* sm_perm = sm_normal + ld;
-    uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_perm + planes_perm_floats(ld));
+    uint8_t* sm_limbs = reinterpret_cast<uint8_t*>(sm_normal + ld);
+    uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_limbs + PLANES_LIMBS * ld);
     __shared__ uint32_t sm_count;
     __shared__ uint32_t sm_w[16];
     __shared__ uint32_t sm_list[SCAN_UNIT * PLANES_CHUNK], sm_list2[SCAN_UNIT * PLANES_CHUNK];
     __shared__ uint32_t sm_cnt[PLANES_CHUNK + 2];
-    __shared__ double sm_l1[WORK_THREADS / 32];
+    __shared__ PlanesScratch sm_sc;
+    __shared__ PlanesNormal sm_pn;
     auto via_shadow = [&](const Job& jb) { return jb.kind == JOB_SCAN && jb.margins == nullptr && (jb.len + SCAN_UNIT - 1) / SCAN_UNIT > min_units; };
     for (int j = threadIdx.x; j < njobs; j += blockDim.x) {
         const Job jb = jobs[j];
@@ -538,7 +581,6 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
     const uint32_t total = sm_prefix[njobs];
     int loaded_job = -1;
     float nh0 = 0.f;
-    float2 wf = make_float2(0.f, 0.f);
     for (uint32_t u = blockIdx.x; u < total; u += gridDim.x) {
         int lo = 0, hi = njobs;  // last j with prefix[j] <= u
         while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (sm_prefix[mid] <= u) lo = mid; else hi = mid; }
@@ -549,22 +591,24 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
             if (loaded_job != j) {
                 __syncthreads();
                 double l1 = 0.0;
+                uint32_t mb = 0;
                 for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) {
                     const float v = jb.normal[NORMAL_HDR + i];
                     sm_normal[i] = v;
-                    sm_perm[planes_perm_index(i)] = v;
                     l1 += (double)fabsf(v);
+                    mb = max(mb, __float_as_uint(fabsf(v)));
                 }
                 l1 = warp_sum_f64(l1);
-                if ((threadIdx.x & 31) == 0) sm_l1[threadIdx.x >> 5] = l1;
+                mb = __reduce_max_sync(0xffffffffu, mb);
+                if ((threadIdx.x & 31) == 0) { sm_sc.l1[threadIdx.x >> 5] = l1; sm_sc.mx[threadIdx.x >> 5] = mb; }
                 nh0 = jb.normal[0];
                 loaded_job = j;
                 __syncthreads();
-                wf = planes_job_factors(sm_l1, d);
+                if (via_shadow(jb)) planes_job_factors(sm_normal, ld, d, sm_limbs, sm_sc, &sm_pn);
             }
             if (via_shadow(jb)) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
-                scan_claim_planes(jb, item * PLANES_CHUNK, min(units, (item + 1u) * PLANES_CHUNK), items, planes, ih0, d, ld, metric, sm_normal, sm_perm, nh0, wf.x, wf.y,
+                scan_claim_planes(jb, item * PLANES_CHUNK, min(units, (item + 1u) * PLANES_CHUNK), items, planes, ih0, d, ld, metric, sm_normal, sm_limbs, &sm_pn, nh0,
                                   sm_list, sm_list2, sm_cnt, stats);
             } else scan_unit<true>(jb, item, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
         } else {

@@ -307,7 +307,10 @@ int32_t arroy_b200_synth_device(arroy_ctx* ctx, const uint8_t seed[32], uint32_t
 /* Time `iters` launches of the side()/margin scan kernel over `n_rows` staged rows
  * (rows == NULL: rows 0..n_rows-1) with CUDA events on the library's stream; optional
  * L2 flush between launches. Returns the average milliseconds per launch. Results stay on
- * the device (this measures the kernel, not the boundary). */
+ * the device (this measures the kernel, not the boundary). variant 0: the f32 scan
+ * (work_kernel); variant 1: the build's 8-bit pre-filter (work_kernel_shadow, every unit
+ * through the planes; float metrics, 64 <= dim <= 8192), whose stage counts of the last
+ * launch arroy_b200_build_prefilter_stats then reports. */
 int32_t arroy_b200_time_scan(arroy_ctx* ctx, const float* normal, float hdr0, float hdr1,
                              const uint32_t* rows, uint64_t n_rows, int32_t variant, int32_t iters,
                              int32_t flush_l2, float* out_ms_avg, uint64_t* out_left_count);

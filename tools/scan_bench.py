@@ -33,14 +33,23 @@ def main():
     r = np.random.default_rng(0)
     normal = (r.standard_normal(args.d) / np.sqrt(args.d)).astype(np.float32)
     out = []
+    # the same row lists for every variant, so that their Left counts can be compared
+    cases = (("contiguous", None), ("gathered_half", np.sort(r.choice(args.n, size=args.n // 2, replace=False)).astype(np.uint32)),
+             ("gathered_4k", np.sort(r.choice(args.n, size=4096, replace=False)).astype(np.uint32)))
     for variant in [int(v) for v in args.variants.split(",")]:
-        for name, rows in (("contiguous", None), ("gathered_half", np.sort(r.choice(args.n, size=args.n // 2, replace=False)).astype(np.uint32)),
-                           ("gathered_4k", np.sort(r.choice(args.n, size=4096, replace=False)).astype(np.uint32))):
+        for name, rows in cases:
             n_rows = args.n if rows is None else rows.size
             ms, left = ctx.time_scan(normal, (0.0, 0.0), n_rows, rows=rows, iters=args.iters, flush_l2=True, variant=variant)
-            gbs = n_rows * args.d * 4 / (ms * 1e-3) / 1e9
-            rec = {"variant": variant, "rows": name, "n_rows": n_rows, "d": args.d, "ms": round(ms, 4), "GBps": round(gbs, 1),
-                   "frac_of_measured_hbm": round(gbs / peaks["hbm_gbs"], 3), "left": left}
+            rec = {"variant": variant, "rows": name, "n_rows": n_rows, "d": args.d, "ms": round(ms, 4)}
+            if variant == 1:
+                # the pre-filter reads the hi plane of every row, the lo plane of stage 2's rows and the f32 row of stage 3's
+                st = ctx.build_prefilter_stats()
+                nbytes = n_rows * args.d + st["rows_stage2"] * args.d + st["rows_rescored_f32"] * args.d * 4
+                rec.update(stage2_frac=round(st["rows_stage2"] / n_rows, 5), stage3_frac=round(st["rows_rescored_f32"] / n_rows, 6))
+            else:
+                nbytes = n_rows * args.d * 4
+            gbs = nbytes / (ms * 1e-3) / 1e9
+            rec.update(GBps=round(gbs, 1), frac_of_measured_hbm=round(gbs / peaks["hbm_gbs"], 3), left=left)
             print(json.dumps(rec), flush=True)
             out.append(rec)
     return out
