@@ -187,11 +187,9 @@ size_t work_smem(uint32_t ld, int njobs) { return (size_t)ld * 4 + (size_t)(njob
 
 void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
     size_t smem = work_smem(c->ld, njobs);
-    static std::atomic<size_t> configured{0};
-    if (smem > 48 * 1024 && smem > configured.load()) {
-        CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        configured = smem;
-    }
+    // set on every launch: build_wave sets the same attribute to its own (possibly smaller) request, so a value remembered
+    // here could be stale
+    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     work_kernel<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric);
     CK(cudaGetLastError());
     c->n_launches += 1;
@@ -548,6 +546,11 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         W.root.ensure(8);
         CK(cudaMemsetAsync(W.root.p, 0, 8, c->stream));
         P.root_ready = W.root.as<uint32_t>(); P.root_ticket = W.root.as<uint32_t>() + 1;
+    }
+    // the schedule this wave runs, OR-ed over the waves of the build (bits: arroy_b200_build_breakdown in arroy_b200.h)
+    {
+        const uint32_t sched = persist ? 1u : lockstep ? 2u : cluster == 16 ? 16u : cluster == 8 ? 8u : 4u;
+        c->breakdown[6] = (double)((uint32_t)c->breakdown[6] | sched | (use_smem ? 0u : 32u) | (P.spec ? 64u : 0u));
     }
 
     CK(cudaStreamSynchronize(c->stream));

@@ -335,7 +335,11 @@ int32_t arroy_b200_arena_get(arroy_b200_arena* arena, uint32_t node_id, const ui
 
 /* Host-side wall-clock breakdown of the last build (ms): [0] buffer setup + tree init,
  * [1] CUDA graph capture + instantiate, [2] device step loop, [3] finalize + device->host copies,
- * [4] NodeCodec encoding + sink calls, [5] graph launches (count), [6..7] reserved. */
+ * [4] NodeCodec encoding + sink calls, [5] graph launches (count), [6] the schedules the build's
+ * waves ran, one bit each, OR-ed over the waves: 1 persistent (one cooperative launch per wave),
+ * 2 lockstep, 4 async CUDA graph with one control CTA per tree, 8 / 16 async with a thread-block
+ * cluster of 8 / 16 control CTAs per tree, 32 two_means workspace in global memory (rows wider
+ * than 3648 floats), 64 speculative two_means; [7] reserved. */
 int32_t arroy_b200_build_breakdown(arroy_ctx* ctx, double out[8]);
 
 /* Counters since arroy_b200_create: out[0] = kernel launches issued by this library,
