@@ -107,11 +107,12 @@ struct arroy_ctx {
     int metric = 0;
     uint32_t dim = 0, ld = 0;   // dim = the vectors' length on the device (binary-quantized metrics: the padded bit count)
     uint32_t user_dim = 0;      // the index' dimensions (what normalized_distance of the binary-quantized metrics divides by)
+    uint32_t row_bytes = 0;     // bytes per item row: 4 ld, binary-quantized metrics: the bit string (kernels.cuh bq_row_u4)
     uint64_t n = 0;
     DevBuf items, h0, h1, norms, maxbits;
     std::vector<uint32_t> ids;
     // scratch
-    DevBuf s_rows, s_flags, s_margins, s_normal, s_unit, s_job, s_keys, s_keys2, s_dists, s_q, s_qh0, s_off, s_orows, s_odist, s_olen, s_misc;
+    DevBuf s_rows, s_flags, s_margins, s_normal, s_unit, s_job, s_keys, s_keys2, s_dists, s_q, s_qbits, s_qh0, s_off, s_orows, s_odist, s_olen, s_misc;
     PinBuf pin;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaStream_t side_stream = nullptr;   // host -> device flags while the persistent build kernel occupies `stream`
@@ -185,12 +186,16 @@ void require_staged(arroy_ctx* c) { if (!c->staged) throw NotStaged("items have 
 
 size_t work_smem(uint32_t ld, int njobs) { return (size_t)ld * 4 + (size_t)(njobs + 1) * 4 + 16; }
 
+// the scan kernel of the staged items: f32 rows, or bit-string rows for the binary-quantized metrics
+auto work_fn(int metric) { return is_bq(metric) ? &work_kernel<true> : &work_kernel<false>; }
+
 void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
     size_t smem = work_smem(c->ld, njobs);
+    const auto work = work_fn(c->metric);
     // set on every launch: build_wave sets the same attribute to its own (possibly smaller) request, so a value remembered
     // here could be stale
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    work_kernel<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric);
+    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    work<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric);
     CK(cudaGetLastError());
     c->n_launches += 1;
 }
@@ -219,8 +224,9 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
     c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false; c->staging_open = false;
     c->stage_epoch += 1;
     c->metric = metric; c->dim = dim; c->ld = (dim + 31u) & ~31u; c->n = n;
+    c->row_bytes = is_bq(metric) ? 16u * bq_row_u4(dim) : 4u * c->ld;
     c->ids.assign(ids, ids + n);
-    c->items.ensure(std::max<size_t>(16, (size_t)n * c->ld * 4));
+    c->items.ensure(std::max<size_t>(16, (size_t)n * c->row_bytes));
     c->h0.ensure(std::max<size_t>(16, n * 4));
     c->h1.ensure(std::max<size_t>(16, n * 4));
     CK(cudaMemsetAsync(c->h0.p, 0, std::max<size_t>(16, n * 4), c->stream));
@@ -229,7 +235,14 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
 
 // headers as Writer::add_item stores them: D::new_header(vector) (src/writer.rs:388-390)
 void default_headers(arroy_ctx* c) {
-    if ((c->metric == COSINE || c->metric == BQ_COSINE) && c->n > 0) {   // BQ cosine: sqrt(popcount-dot(v, v)) = sqrt(dim), exact in f32
+    if (c->metric == BQ_COSINE && c->n > 0) {   // sqrt(dot(v, v)) of a +-1 vector: sqrt(dim), dim exact in f32
+        const float h = sqrtf((float)c->dim);
+        uint32_t bits;
+        memcpy(&bits, &h, 4);
+        fill_u32_kernel<<<(unsigned)std::min<uint64_t>((c->n + 255) / 256, (uint64_t)c->sm_count * 8), 256, 0, c->stream>>>(c->h0.as<uint32_t>(), c->n, bits);
+        CK(cudaGetLastError());
+        c->n_launches += 1;
+    } else if (c->metric == COSINE && c->n > 0) {
         compute_norms(c, false);
         CK(cudaMemcpyAsync(c->h0.p, c->norms.p, c->n * 4, cudaMemcpyDeviceToDevice, c->stream));
     }
@@ -237,29 +250,29 @@ void default_headers(arroy_ctx* c) {
 
 // Staging pipeline: W host threads, each decoding row chunks into its own pinned bounce buffers and
 // issuing its own cudaMemcpyAsync on its own stream, so decode (host memcpy of unaligned values)
-// and PCIe transfers of different chunks overlap. row_src(i) = address of the dim floats of row i.
-// mode 0: row_src(i) = dim f32 (byte aligned only); mode 1 (binary quantized): row_src(i) = src_dim f32 to be quantized to +-1;
-// mode 2 (binary quantized): row_src(i) = the stored bit string (dim / 8 bytes) to be expanded to +-1
+// and PCIe transfers of different chunks overlap. Rows of row_bytes bytes, zero padded.
+// mode 0: row_src(i) = dim f32 (byte aligned only); mode 1 (binary quantized): row_src(i) = src_dim f32 to be quantized to a
+// bit string (is_sign_positive); mode 2 (binary quantized): row_src(i) = the stored bit string (dim / 8 bytes), copied
 template <class RowSrc>
-void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t ld, RowSrc row_src, float* dst_override = nullptr, size_t chunk_mb_override = 0, bool count_bytes = true,
+void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_bytes, RowSrc row_src, uint8_t* dst_override = nullptr, size_t chunk_mb_override = 0, bool count_bytes = true,
                          int mode = 0, uint32_t src_dim = 0) {
     if (n == 0) return;
     // 8 lanes x 4 MB chunks: decode of one chunk overlaps the PCIe copies of the others
     unsigned W = std::min(8u, std::max(1u, std::thread::hardware_concurrency()));
     const size_t chunk_mb = chunk_mb_override ? chunk_mb_override : 4;
-    const uint64_t chunk_rows = std::max<uint64_t>(1, (chunk_mb << 20) / ((size_t)ld * 4));
+    const uint64_t chunk_rows = std::max<uint64_t>(1, (chunk_mb << 20) / row_bytes);
     const uint64_t n_chunks = (n + chunk_rows - 1) / chunk_rows;
     W = (unsigned)std::min<uint64_t>(W, n_chunks);
     if (c->stage_workers.size() < W) c->stage_workers.resize(W);
     for (unsigned w = 0; w < W; ++w) {
         StageWorker& sw = c->stage_workers[w];
         if (!sw.st) CK(cudaStreamCreateWithFlags(&sw.st, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; ++k) { sw.pin[k].ensure(chunk_rows * ld * 4); if (!sw.ev[k]) CK(cudaEventCreateWithFlags(&sw.ev[k], cudaEventDisableTiming)); }
+        for (int k = 0; k < 2; ++k) { sw.pin[k].ensure(chunk_rows * row_bytes); if (!sw.ev[k]) CK(cudaEventCreateWithFlags(&sw.ev[k], cudaEventDisableTiming)); }
     }
     CK(cudaStreamSynchronize(c->stream));  // the destination buffer must not be in use
     std::mutex emu;
     std::string err;
-    float* dst = dst_override ? dst_override : c->items.as<float>();
+    uint8_t* dst = dst_override ? dst_override : c->items.as<uint8_t>();
     auto worker = [&](unsigned w) {
         try {
             CK(cudaSetDevice(c->device));
@@ -269,21 +282,19 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t ld, Ro
             for (uint64_t ch = w; ch < n_chunks; ch += W, k ^= 1) {
                 const uint64_t r0 = ch * chunk_rows, rows = std::min<uint64_t>(chunk_rows, n - r0);
                 if (used[k]) CK(cudaEventSynchronize(sw.ev[k]));
-                float* b = sw.pin[k].as<float>();
+                uint8_t* b = sw.pin[k].as<uint8_t>();
                 for (uint64_t i = 0; i < rows; ++i) {
-                    float* o = b + i * ld;
-                    if (mode == 0) memcpy(o, row_src(r0 + i), 4ull * dim);
-                    else if (mode == 1) {
+                    uint8_t* o = b + i * row_bytes;
+                    const size_t used = mode == 0 ? 4ull * dim : dim / 8;
+                    if (mode == 0) memcpy(o, row_src(r0 + i), used);
+                    else if (mode == 1) {   // little-endian words: bit t of the string is bit t & 7 of byte t >> 3
                         const uint8_t* sp = row_src(r0 + i);
-                        for (uint32_t t = 0; t < src_dim; ++t) { uint32_t bits; memcpy(&bits, sp + 4ull * t, 4); o[t] = (bits >> 31) ? -1.0f : 1.0f; }
-                        for (uint32_t t = src_dim; t < dim; ++t) o[t] = -1.0f;
-                    } else {
-                        const uint8_t* sp = row_src(r0 + i);
-                        for (uint32_t t = 0; t < dim; ++t) o[t] = ((sp[t >> 3] >> (t & 7)) & 1) ? 1.0f : -1.0f;   // little-endian words: bit t of the string
-                    }
-                    for (uint32_t t = dim; t < ld; ++t) o[t] = 0.f;
+                        memset(o, 0, used);
+                        for (uint32_t t = 0; t < src_dim; ++t) { uint32_t bits; memcpy(&bits, sp + 4ull * t, 4); if (!(bits >> 31)) o[t >> 3] |= (uint8_t)(1u << (t & 7)); }
+                    } else memcpy(o, row_src(r0 + i), used);
+                    memset(o + used, 0, row_bytes - used);
                 }
-                CK(cudaMemcpyAsync(dst + r0 * ld, b, rows * ld * 4, cudaMemcpyHostToDevice, sw.st));
+                CK(cudaMemcpyAsync(dst + r0 * row_bytes, b, rows * row_bytes, cudaMemcpyHostToDevice, sw.st));
                 CK(cudaEventRecord(sw.ev[k], sw.st));
                 used[k] = true;
             }
@@ -293,7 +304,7 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t ld, Ro
     if (W == 1) worker(0);
     else { std::vector<std::thread> th; for (unsigned w = 0; w < W; ++w) th.emplace_back(worker, w); for (auto& x : th) x.join(); }
     if (!err.empty()) throw CudaError(err);
-    if (count_bytes) c->h2d_bytes += n * (uint64_t)ld * 4;
+    if (count_bytes) c->h2d_bytes += n * (uint64_t)row_bytes;
 }
 
 // ---- RoaringBitmap::serialize_into (roaring 0.10.9, portable format, no run containers) ------
@@ -471,7 +482,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     const size_t ctrl_smem = use_smem ? ws_bytes : 0;
     if (ctrl_smem > 48 * 1024) CK(cudaFuncSetAttribute(control_fn(true, 1, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
     const size_t wsmem = work_smem(ld, (int)tw);
-    if (wsmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
+    const auto work = work_fn(c->metric);
+    if (wsmem > 48 * 1024) CK(cudaFuncSetAttribute(work, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
     const size_t limb_smem = (size_t)PLANES_LIMBS * ld;   // work_kernel_shadow's limbs of the normal
     if (wsmem + limb_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + limb_smem)));
     const int work_grid = c->sm_count * 3;
@@ -541,8 +553,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         P.cur_normal = W.cur_normal.as<float>();
         P.abort = W.abort.as<int>();
         // fused root scan: every tree of the wave starts at the root of the whole index (no subtree mode), rows go through the
-        // 8-lanes-per-row path, and a batch of normals fits next to nothing else in the workers' shared memory
-        P.root_fused = (!sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem) ? 1 : 0;
+        // 8-lanes-per-row path, and a batch of normals fits next to nothing else in the workers' shared memory (f32 rows only: the
+        // bit-string rows of the binary-quantized metrics take the popcount scan, kernels.cuh bq_scan_unit)
+        P.root_fused = (!is_bq(c->metric) && !sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem) ? 1 : 0;
         W.root.ensure(8);
         CK(cudaMemsetAsync(W.root.p, 0, 8, c->stream));
         P.root_ready = W.root.as<uint32_t>(); P.root_ticket = W.root.as<uint32_t>() + 1;
@@ -581,7 +594,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
                 for (int i = 0; i < ASYNC_BATCH; ++i) {
                     launch_control(ctrlc, 1, cluster, ctrl_smem, st, P, t);
                     if (P.planes.hi) work_kernel_shadow<<<c->sm_count, WORK_THREADS, wsmem1 + limb_smem, st>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-                    else work_kernel<<<c->sm_count, WORK_THREADS, wsmem1, st>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric);
+                    else work<<<c->sm_count, WORK_THREADS, wsmem1, st>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric);
                 }
                 CK(cudaEventRecord(c->tree_events[1 + t], st));
                 CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
@@ -654,7 +667,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
                 launch_control(ctrl1, tw, 1, ctrl_smem, c->stream, P, 0u);
                 if (profile) CK(cudaEventRecord(pev[2 * i], c->stream));
                 if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + limb_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-                else work_kernel<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric);
+                else work<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric);
                 if (profile) CK(cudaEventRecord(pev[2 * i + 1], c->stream));
             }
             CK(cudaGetLastError());
@@ -1063,11 +1076,12 @@ struct Marks {
 };
 
 // A call's queries on the device: by item their rows (vecs == nullptr), by vector their vectors (rows == nullptr), and their
-// first header.
+// first header. Binary-quantized metrics: always their +-1 vectors (rows == nullptr), and their bit strings.
 struct DevQueries {
     const float* vecs = nullptr;
     const uint32_t* rows = nullptr;
     const float* h0 = nullptr;
+    const uint4* bits = nullptr;
 };
 
 // Uploads queries q0 .. q0 + m of a call: by item their rows into w_qrows, by vector their vectors into s_q (rows padded to ld
@@ -1090,6 +1104,20 @@ DevQueries upload_queries(arroy_ctx* c, uint32_t q0, uint32_t m, const uint32_t*
     else if (query_rows) { gather_f32_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->s_qh0.as<float>(), c->h0.as<float>(), Q.rows, m); CK(cudaGetLastError()); }
     else CK(cudaMemsetAsync(c->s_qh0.p, 0, 4ull * m, c->stream));
     Q.h0 = c->s_qh0.as<float>();
+    if (is_bq(c->metric) && m) {   // the walks take the +-1 vector, the re-rank the bit string (ld = dim for these metrics)
+        const uint32_t w32 = c->row_bytes / 4;
+        c->s_qbits.ensure((size_t)m * c->row_bytes);
+        const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)m * ld + 255) / 256, (uint64_t)c->sm_count * 8);
+        if (Q.rows) {
+            c->s_q.ensure((size_t)m * ld * 4);
+            bq_query_rows_kernel<<<grid, 256, 0, c->stream>>>(c->items.as<uint32_t>(), w32, Q.rows, m, ld, c->s_q.as<float>(), c->s_qbits.as<uint32_t>());
+            Q.vecs = c->s_q.as<float>();
+            Q.rows = nullptr;
+        } else bq_pack_rows_kernel<<<grid, 256, 0, c->stream>>>(Q.vecs, ld, c->s_qbits.as<uint32_t>(), m, ld, w32);
+        CK(cudaGetLastError());
+        c->n_launches += 1;
+        Q.bits = c->s_qbits.as<uint4>();
+    }
     return Q;
 }
 
@@ -1105,12 +1133,17 @@ void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32
         CK(cudaStreamSynchronize(c->stream));
         if (frerank_ok(c, m)) { if (mark) (*mark)(); return; }
     }
-    if (max_len) {   // Manhattan sums one row per lane, the other metrics four rows per warp
-        const uint64_t per = (c->metric == MANHATTAN || c->metric == BQ_MANHATTAN) ? 32 : 4;
+    if (max_len) {
+        // (Manhattan sums one row per lane, the bit-string rows take four lanes per row, the other metrics eight)
+        const uint64_t per = c->metric == MANHATTAN ? 32 : is_bq(c->metric) ? 8 : 4;
         const uint64_t warps = (max_len + per - 1) / per;
         const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, std::max<uint64_t>(1, ((uint64_t)c->sm_count * 8) / std::min<uint32_t>(m, c->sm_count * 8u))));
-        distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric, Q.vecs, Q.rows, Q.h0, m,
-                                                           rows, beg, end, c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
+        if (is_bq(c->metric))
+            bq_distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<uint4>(), c->h0.as<float>(), c->dim, c->metric, Q.bits, Q.h0, rows, beg, end,
+                                                                  c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
+        else
+            distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric, Q.vecs, Q.rows, Q.h0, m,
+                                                               rows, beg, end, c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
         CK(cudaGetLastError());
     }
     if (mark) (*mark)();
@@ -1247,7 +1280,7 @@ int32_t arroy_b200_create(int32_t device, arroy_ctx** out) {
         CK(cudaEventCreate(&c->tev1));
         // fail loudly if the kernels were not built for this device
         cudaFuncAttributes fa;
-        CK(cudaFuncGetAttributes(&fa, work_kernel));
+        CK(cudaFuncGetAttributes(&fa, work_kernel<false>));
     } catch (const std::exception& e) {
         fprintf(stderr, "arroy_b200_create: %s\n", e.what());
         delete c;
@@ -1298,7 +1331,6 @@ int32_t arroy_b200_stage_items(arroy_ctx* c, int32_t metric, uint32_t dim, uint6
         set_device(c);
         if (n && (!ids || !leaf_values)) throw ArgError("null ids / leaf_values");
         alloc_items(c, metric, dim, n, ids);
-        const uint32_t ld = c->ld;
         const int hf = metric_header_floats(metric);
         std::vector<float> h0(n), h1(n, 0.f);
         // decode the unaligned LMDB values: [tag][Header][dim x f32]
@@ -1319,7 +1351,7 @@ int32_t arroy_b200_stage_items(arroy_ctx* c, int32_t metric, uint32_t dim, uint6
         }
         const size_t voff = 1 + 4 * (size_t)hf;
         // binary-quantized leaves store the bit string (node.rs:224-228 with VectorCodec = BinaryQuantized)
-        stage_rows_pipeline(c, n, c->dim, ld, [&](uint64_t i) { return leaf_values[i] + voff; }, nullptr, 0, true, is_bq(metric) ? 2 : 0);
+        stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return leaf_values[i] + voff; }, nullptr, 0, true, is_bq(metric) ? 2 : 0);
         if (n) {
             CK(cudaMemcpyAsync(c->h0.p, h0.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
             CK(cudaMemcpyAsync(c->h1.p, h1.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
@@ -1357,7 +1389,8 @@ int32_t arroy_b200_stage_rows(arroy_ctx* c, uint64_t row0, uint64_t n_rows, cons
             if (hf == 2) memcpy(&c->stage_h1[row0 + i], v + 5, 4);
         }
         const size_t voff = 1 + 4 * (size_t)hf;
-        stage_rows_pipeline(c, n_rows, c->dim, c->ld, [&](uint64_t i) { return leaf_values[i] + voff; }, c->items.as<float>() + (size_t)row0 * c->ld, 0, true, is_bq(c->metric) ? 2 : 0);
+        stage_rows_pipeline(c, n_rows, c->dim, c->row_bytes, [&](uint64_t i) { return leaf_values[i] + voff; }, c->items.as<uint8_t>() + (size_t)row0 * c->row_bytes, 0, true,
+                            is_bq(c->metric) ? 2 : 0);
     });
 }
 
@@ -1386,7 +1419,7 @@ int32_t arroy_b200_stage_items_flat(arroy_ctx* c, int32_t metric, uint32_t dim, 
             const uint8_t* base = reinterpret_cast<const uint8_t*>(vectors);
             const size_t stride = 4ull * dim;
             // binary-quantized metrics: the f32 vectors are quantized on the way (Writer::add_item -> UnalignedVector::from_slice)
-            stage_rows_pipeline(c, n, c->dim, c->ld, [&](uint64_t i) { return base + i * stride; }, nullptr, 0, true, is_bq(metric) ? 1 : 0, dim);
+            stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return base + i * stride; }, nullptr, 0, true, is_bq(metric) ? 1 : 0, dim);
             if (hdr0) CK(cudaMemcpyAsync(c->h0.p, hdr0, n * 4, cudaMemcpyHostToDevice, c->stream));
             else default_headers(c);
             if (hdr1) CK(cudaMemcpyAsync(c->h1.p, hdr1, n * 4, cudaMemcpyHostToDevice, c->stream));
@@ -1403,7 +1436,7 @@ int32_t arroy_b200_stage_items_device(arroy_ctx* c, int32_t metric, uint32_t dim
         if (n && (!ids || !device_vectors)) throw ArgError("null ids / vectors");
         alloc_items(c, metric, dim, n, ids);
         if (n && is_bq(metric)) {
-            bq_sign_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(static_cast<const float*>(device_vectors), c->items.as<float>(), n, dim, c->dim, c->ld);
+            bq_pack_rows_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(static_cast<const float*>(device_vectors), dim, c->items.as<uint32_t>(), n, dim, c->row_bytes / 4);
             CK(cudaGetLastError());
             c->n_launches += 1;
             default_headers(c);
@@ -1609,6 +1642,7 @@ int32_t arroy_b200_prefilter_planes(arroy_ctx* c, int8_t* hi, int8_t* lo, float*
     return guarded(c, [&] {
         if (!hi || !lo || !scale) throw ArgError("null argument");
         require_staged(c);
+        if (is_bq(c->metric)) throw ArgError("prefilter_planes needs a float metric (binary-quantized items are bit strings)");
         set_device(c);
         planes_prepare(c);
         const size_t bytes = (size_t)c->n * c->ld;
@@ -2373,6 +2407,7 @@ int32_t arroy_b200_prefilter_scores(arroy_ctx* c, uint32_t nq, const float* quer
         require_staged(c); set_device(c);
         if (nq == 0 || n_rows == 0) return;
         if (!queries || !rows || !out_scores) throw ArgError("null argument");
+        if (is_bq(c->metric)) throw ArgError("prefilter_scores needs a float metric (binary-quantized items are bit strings)");
         if (c->dim < 32) throw ArgError("prefilter_scores needs dim >= 32");
         if (n_rows > 0x7fffffffull || (uint64_t)nq * n_rows > (1ull << 29)) throw ArgError("prefilter_scores: problem too large");
         for (uint64_t i = 0; i < n_rows; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
@@ -2479,7 +2514,7 @@ int32_t arroy_b200_device_ptrs(arroy_ctx* c, void* out[3], uint32_t* out_ld) {
     return guarded(c, [&] {
         if (!c->staging_open) require_staged(c);
         out[0] = c->items.p; out[1] = c->h0.p; out[2] = c->h1.p;
-        if (out_ld) *out_ld = c->ld;
+        if (out_ld) *out_ld = c->row_bytes / 4;
     });
 }
 

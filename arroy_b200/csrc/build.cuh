@@ -573,6 +573,14 @@ __device__ __forceinline__ void create_split_cta(const BuildParams& P, Rng& rng 
     {   // gather: warp w copies rows w and w + 8; all loads of a thread are issued before any store
         if (tid < 12) { S.h0[tid] = P.ih0 ? P.ih0[my_row] : 0.f; S.h1[tid] = P.ih1 ? P.ih1[my_row] : 0.f; }
         const int l4 = ld >> 2;
+        if constexpr (BQ) {   // bit-string rows (kernels.cuh bq_row_u4) expanded to the +-1 f32 leaves two_means works on
+            const uint32_t w32 = 4u * bq_row_u4(P.d);
+            for (int j = warp; j < 12; j += 8) {
+                const uint32_t* src = reinterpret_cast<const uint32_t*>(P.items) + (size_t)S.rows[j] * w32;
+                float* dst = ws + (size_t)j * ld;
+                for (int i = lane; i < ld; i += 32) dst[i] = ((__ldg(src + (i >> 5)) >> (i & 31)) & 1u) ? 1.0f : -1.0f;
+            }
+        } else
         for (int j = warp; j < 12; j += 8) {
             const float4* src = reinterpret_cast<const float4*>(P.items + (size_t)S.rows[j] * ld);
             float4* dst = reinterpret_cast<float4*>(ws + (size_t)j * ld);
@@ -961,6 +969,9 @@ __device__ __noinline__ void proot(const BuildParams& P, float* smN) {
 
 // A worker CTA: claims units of whatever the control CTAs have published and runs the same scan / partition code as work_kernel.
 // Returns when every tree is done (or on error). sm_normal: ld floats of dynamic shared memory.
+// BQ: the items are bit-string rows, the loaded normal's first words of sm_normal hold its bit string and the scans are
+// bq_scan_unit's (no fused root pass, no pre-filter planes).
+template <bool BQ>
 __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ uint32_t w_t, w_u0, w_n, w_seq, w_pseq, w_found, w_exit, w_count;
     __shared__ PSlot w_job;        // fields of the claimed job (first 64 bytes)
@@ -977,7 +988,7 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     uint32_t loaded_t = 0xffffffffu, loaded_seq = 0xffffffffu;
     float nh0 = 0.f;
     if (tid == 0) w_exit = 0;
-    if (P.root_fused) proot(P, sm_normal);
+    if constexpr (!BQ) { if (P.root_fused) proot(P, sm_normal); }
     for (;;) {
         // ---- poll: one load per slot, 32 slots per pass; pick a slot with unclaimed units ----
         if (warp == 0) {
@@ -1053,34 +1064,52 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
             const uint32_t chunk = max(1u, w_job.chunk);
             if (jb.kind == JOB_SCAN) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
-                if (want_normal || seq != w_pseq) {
-                    double l1 = 0.0;
-                    uint32_t mb = 0;
+                if constexpr (BQ) {
+                    if (want_normal || seq != w_pseq) {
+                        // element tid + 256 u of the normal is nreg[u]: one ballot per warp and u is u32 word 8 u + warp of the bit
+                        // string (ld <= 8 * CTRL_THREADS; the words past ld come out 0, the padding of the rows)
 #pragma unroll
-                    for (int u = 0; u < 8; ++u) {
-                        const uint32_t i = tid + u * CTRL_THREADS;
-                        if (i < P.ld) {
-                            sm_normal[i] = nreg[u];
-                            l1 += (double)fabsf(nreg[u]);
-                            mb = max(mb, __float_as_uint(fabsf(nreg[u])));
+                        for (int u = 0; u < 8; ++u) {
+                            const uint32_t i = tid + u * CTRL_THREADS;
+                            const unsigned b = __ballot_sync(0xffffffffu, i < P.ld && !(__float_as_uint(nreg[u]) >> 31));
+                            if (lane == 0 && (uint32_t)(u * 8 + warp) < 4u * bq_row_u4(P.d)) reinterpret_cast<uint32_t*>(sm_normal)[u * 8 + warp] = b;
                         }
+                        nh0 = __ldcg(nsrc);
+                        loaded_t = t; loaded_seq = seq;
+                        __syncthreads();
                     }
-                    if (P.planes.hi != nullptr) {
-                        l1 = warp_sum_f64(l1);
-                        mb = __reduce_max_sync(0xffffffffu, mb);
-                        if (lane == 0) { w_sc.l1[warp] = l1; w_sc.mx[warp] = mb; }
+                    for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u)
+                        bq_scan_unit(jb, u, reinterpret_cast<const uint4*>(P.items), P.d, P.metric, reinterpret_cast<const uint4*>(sm_normal), nh0, &w_count);
+                } else {
+                    if (want_normal || seq != w_pseq) {
+                        double l1 = 0.0;
+                        uint32_t mb = 0;
+#pragma unroll
+                        for (int u = 0; u < 8; ++u) {
+                            const uint32_t i = tid + u * CTRL_THREADS;
+                            if (i < P.ld) {
+                                sm_normal[i] = nreg[u];
+                                l1 += (double)fabsf(nreg[u]);
+                                mb = max(mb, __float_as_uint(fabsf(nreg[u])));
+                            }
+                        }
+                        if (P.planes.hi != nullptr) {
+                            l1 = warp_sum_f64(l1);
+                            mb = __reduce_max_sync(0xffffffffu, mb);
+                            if (lane == 0) { w_sc.l1[warp] = l1; w_sc.mx[warp] = mb; }
+                        }
+                        nh0 = __ldcg(nsrc);
+                        loaded_t = t; loaded_seq = seq;
+                        __syncthreads();
+                        if (P.planes.hi != nullptr && units > P.shadow_min_units) planes_job_factors(sm_normal, P.ld, P.d, sm_limbs, w_sc, &w_pn);
                     }
-                    nh0 = __ldcg(nsrc);
-                    loaded_t = t; loaded_seq = seq;
-                    __syncthreads();
-                    if (P.planes.hi != nullptr && units > P.shadow_min_units) planes_job_factors(sm_normal, P.ld, P.d, sm_limbs, w_sc, &w_pn);
+                    if (P.planes.hi != nullptr && units > P.shadow_min_units)
+                        for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
+                            scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_limbs,
+                                              &w_pn, nh0, w_list, w_list2, w_cnt, P.shadow_stats);
+                    else
+                        for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
                 }
-                if (P.planes.hi != nullptr && units > P.shadow_min_units)
-                    for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
-                        scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_limbs,
-                                          &w_pn, nh0, w_list, w_list2, w_cnt, P.shadow_stats);
-                else
-                    for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
             } else if (jb.kind == JOB_PARTITION) {
                 const uint32_t units = (jb.len + PART_UNIT - 1) / PART_UNIT;
                 for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u)
@@ -1118,10 +1147,13 @@ __device__ __forceinline__ void cluster_scan_share(const BuildParams& P, const J
 template <bool SMEM_WS, int CS, int METRIC>
 __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kernel(BuildParams P, uint32_t tree_base) {
     static_assert(CS <= 1 || SMEM_WS, "the cluster path keeps the normal in the shared-memory workspace");
+    // the cluster path scans f32 rows (cluster_scan_share); the bit-string rows of the binary-quantized metrics go to the workers
+    static_assert(CS <= 1 || !is_bq(METRIC), "no cluster variants for the binary-quantized metrics");
+    static_assert(CTRL_THREADS == 4 * SCAN_UNIT, "pworker<true>: bq_scan_unit takes four lanes per position of a scan unit");
     constexpr bool PERSIST = CS == 0;
     constexpr int CSD = CS < 1 ? 1 : CS;
     extern __shared__ __align__(16) unsigned char ctrl_smem[];
-    if (PERSIST && blockIdx.x >= P.n_trees) { pworker(P, reinterpret_cast<float*>(ctrl_smem)); return; }
+    if (PERSIST && blockIdx.x >= P.n_trees) { pworker<is_bq(METRIC)>(P, reinterpret_cast<float*>(ctrl_smem)); return; }
     __shared__ uint32_t s_scan_count;
     __shared__ TwoMeansShared TM;
     __shared__ uint32_t sm_tmp[CTRL_THREADS + 1];

@@ -134,7 +134,7 @@ int32_t arroy_b200_group_stage_items(arroy_group* g, int32_t metric, uint32_t di
         for (size_t r = 0; r < R; ++r) ck(r, arroy_b200_stage_begin(g->ctx[r], metric, dim, n, ids));
         std::vector<uint8_t*> items(R), h0(R), h1(R);
         for (size_t r = 0; r < R; ++r) { items[r] = static_cast<uint8_t*>(g->ctx[r]->items.p); h0[r] = static_cast<uint8_t*>(g->ctx[r]->h0.p); h1[r] = static_cast<uint8_t*>(g->ctx[r]->h1.p); }
-        const size_t row_bytes = (size_t)g->ctx[0]->ld * 4;
+        const size_t row_bytes = g->ctx[0]->row_bytes;
         // chunks of ~256 MB: big enough for NCCL to run at line rate, small enough that the last broadcast (the only one that is
         // not hidden behind an H2D copy) is short
         const uint64_t chunk_rows = std::max<uint64_t>(1, (256ull << 20) / row_bytes);

@@ -490,8 +490,60 @@ __device__ __forceinline__ void partition_block(const uint32_t* __restrict__ src
     __syncthreads();
 }
 
+// ---- binary-quantized items: bit strings ----------------------------------------------------------------------------------
+// A binary-quantized item row is the reference's bit string (binary_quantized.rs:80-92): bit i of u64 word w set when element
+// 64 w + i is positive, i.e. bit j of u32 word k = element 32 k + j. `d` (the bit count) is a multiple of 64; rows are padded with
+// zero words to 16 bytes. Every element is +-1, so each sum the reference forms over two such vectors is an exact integer in any
+// summation order: dot = d - 2 popcount(a ^ b), sum (a - b)^2 = 4 popcount, sum |a - b| = 2 popcount.
+__host__ __device__ constexpr uint32_t bq_row_u4(uint32_t d) { return (d + 127u) / 128u; }   // 16-byte words per row
+
+// A +-1 normal (f32, d elements) as a bit string in shared memory: 4 bq_row_u4(d) u32 words, bit = is_sign_positive, padding 0.
+// Every thread of the CTA calls it; the caller puts a barrier between this and the first read.
+__device__ __forceinline__ void bq_pack_normal(const float* __restrict__ v, uint32_t d, uint32_t* sm_bits) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t nw = 4u * bq_row_u4(d);
+    for (uint32_t w = threadIdx.x >> 5; w < nw; w += blockDim.x >> 5) {
+        const uint32_t i = w * 32u + (uint32_t)lane;
+        const unsigned b = __ballot_sync(0xffffffffu, i < d && !(__float_as_uint(v[i]) >> 31));
+        if (lane == 0) sm_bits[w] = b;
+    }
+}
+
+// scan_unit for bit-string rows: four lanes per row (a CTA of 4 SCAN_UNIT threads covers the unit's positions). The margin is
+// margin_finish of the exact dot, as scan_unit forms it from its f32 sum of the same +-1 products; flags, margins and the unit's
+// Left count are scan_unit's.
+static_assert(WORK_THREADS == 4 * SCAN_UNIT, "bq_scan_unit: four lanes per position of a scan unit");
+__device__ __forceinline__ void bq_scan_unit(const Job& jb, uint32_t unit, const uint4* __restrict__ items, uint32_t d, int metric,
+                                             const uint4* sm_bits, float nh0, uint32_t* sm_count) {
+    const uint32_t rq = bq_row_u4(d);
+    const int lane = threadIdx.x & 31, sub = threadIdx.x & 3;
+    if (threadIdx.x == 0) *sm_count = 0;
+    __syncthreads();
+    const uint32_t p = unit * SCAN_UNIT + (threadIdx.x >> 2);
+    const bool v = p < jb.len;
+    const uint32_t r = v ? (jb.rows ? __ldcg(jb.rows + p) : p) : 0u;
+    const uint4* x = items + (size_t)r * rq;
+    int pc = 0;
+    for (uint32_t c = (uint32_t)sub; c < rq; c += 4) {
+        const uint4 a = ldg_stream_u4(x + c), b = sm_bits[c];
+        pc += __popc(a.x ^ b.x) + __popc(a.y ^ b.y) + __popc(a.z ^ b.z) + __popc(a.w ^ b.w);
+    }
+    pc += __shfl_xor_sync(0xffffffffu, pc, 1);
+    pc += __shfl_xor_sync(0xffffffffu, pc, 2);
+    const float m = margin_finish(metric, (float)((int)d - 2 * pc), nh0, 0.f);
+    const int s = side_of(m);
+    const bool leader = sub == 0 && v;
+    if (leader) { if (jb.flags) jb.flags[p] = (uint8_t)s; if (jb.margins) jb.margins[p] = m; }
+    const unsigned l = __ballot_sync(0xffffffffu, leader && s == 0);
+    if (lane == 0 && l) atomicAdd(sm_count, (uint32_t)__popc(l));
+    __syncthreads();
+    if (threadIdx.x == 0 && jb.unit_left) jb.unit_left[unit] = *sm_count;
+}
+
 // Persistent-style grid: every CTA strides over the units of all posted jobs.
-// Dynamic shared memory: ld floats (normal) + (njobs + 1) uint32 (unit prefix).
+// Dynamic shared memory: ld floats (normal) + (njobs + 1) uint32 (unit prefix). BQ: `items` holds bit-string rows and the
+// normal's first ld floats of shared memory hold its bit string (bq_scan_unit).
+template <bool BQ>
 __global__ void __launch_bounds__(WORK_THREADS, 3)
 work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const float* __restrict__ ih0,
             uint32_t d, uint32_t ld, int metric) {
@@ -531,12 +583,14 @@ work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ i
         if (jb.kind == JOB_SCAN) {
             if (loaded_job != j) {
                 __syncthreads();
-                for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) sm_normal[i] = jb.normal[NORMAL_HDR + i];
+                if constexpr (BQ) bq_pack_normal(jb.normal + NORMAL_HDR, d, reinterpret_cast<uint32_t*>(sm_normal));
+                else for (uint32_t i = threadIdx.x; i < ld; i += blockDim.x) sm_normal[i] = jb.normal[NORMAL_HDR + i];
                 nh0 = jb.normal[0];
                 loaded_job = j;
                 __syncthreads();
             }
-            scan_unit(jb, unit, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
+            if constexpr (BQ) bq_scan_unit(jb, unit, reinterpret_cast<const uint4*>(items), d, metric, reinterpret_cast<const uint4*>(sm_normal), nh0, &sm_count);
+            else scan_unit(jb, unit, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
         } else {
             partition_block(jb.rows, jb.flags, jb.dst, unit * PART_UNIT, jb.len, jb.unit_left[unit * (PART_UNIT / SCAN_UNIT)], jb.total_left, sm_w);
         }
@@ -878,17 +932,68 @@ __global__ void bq_normalize_kernel(float* __restrict__ dist, uint64_t n, int me
     if (metric != BQ_COSINE) dist[i] = __fdiv_rn(d, dims);
 }
 
-// dense f32 rows (n x d_in) -> the padded +-1 layout (n x ld, the first dpad = 64 * ceil(d_in / 64) columns +-1, the rest 0):
-// BinaryQuantized::from_slice + ::iter (binary_quantized.rs:80-92, :276-289) — bit = is_sign_positive
-__global__ void bq_sign_rows_kernel(const float* __restrict__ src, float* __restrict__ dst, uint64_t n, uint32_t d_in, uint32_t dpad, uint32_t ld) {
-    const uint64_t total = n * ld;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t r = i / ld;
-        const uint32_t c = (uint32_t)(i - r * ld);
-        float v = 0.f;
-        if (c < d_in) v = (__float_as_uint(src[r * d_in + c]) >> 31) ? -1.0f : 1.0f;
-        else if (c < dpad) v = -1.0f;
-        dst[i] = v;
+// dense f32 rows (n x d_in, row pitch `pitch` floats) -> bit-string rows of w32 u32 words: BinaryQuantized::from_slice
+// (binary_quantized.rs:80-92) — bit = is_sign_positive, so +0.0 -> 1, -0.0 -> 0 and a NaN's sign bit decides; elements from d_in
+// on are 0 (the padding of the bit string and of the row). One warp per word.
+__global__ void bq_pack_rows_kernel(const float* __restrict__ src, uint64_t pitch, uint32_t* __restrict__ dst, uint64_t n, uint32_t d_in, uint32_t w32) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t total = n * w32, nw = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t w = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < total; w += nw) {
+        const uint64_t r = w / w32;
+        const uint32_t c = (uint32_t)(w - r * w32) * 32u + (uint32_t)lane;
+        const unsigned b = __ballot_sync(0xffffffffu, c < d_in && !(__float_as_uint(src[r * pitch + c]) >> 31));
+        if (lane == 0) dst[w] = b;
+    }
+}
+
+// queries by item of a binary-quantized index: their bit strings (rows of w32 words) copied to bits, and expanded to the +-1
+// f32 vectors (ld floats each) that the forest walks take
+__global__ void bq_query_rows_kernel(const uint32_t* __restrict__ items, uint32_t w32, const uint32_t* __restrict__ rows, uint32_t m, uint32_t ld,
+                                     float* __restrict__ vecs, uint32_t* __restrict__ bits) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (uint64_t)m * ld; i += stride) {
+        const uint64_t q = i / ld;
+        const uint32_t c = (uint32_t)(i - q * ld);
+        vecs[i] = ((items[(size_t)rows[q] * w32 + (c >> 5)] >> (c & 31u)) & 1u) ? 1.0f : -1.0f;
+    }
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (uint64_t)m * w32; i += stride) {
+        const uint64_t q = i / w32;
+        bits[i] = items[(size_t)rows[q] * w32 + (i - q * w32)];
+    }
+}
+
+// distance_kernel for bit-string rows: query q's bit string is qbits[q] (bq_row_u4(d) 16-byte words), four lanes per candidate.
+// D::built_distance of binary_quantized_{euclidean,cosine,manhattan}.rs from the exact popcount sums, as distance_kernel forms it
+// from its f32 sums of the same +-1 terms; keys as distance_kernel's.
+__global__ void __launch_bounds__(256)
+bq_distance_kernel(const uint4* __restrict__ items, const float* __restrict__ ih0, uint32_t d, int metric, const uint4* __restrict__ qbits,
+                   const float* __restrict__ qh0, const uint32_t* __restrict__ rows, const uint64_t* __restrict__ seg_beg,
+                   const uint64_t* __restrict__ seg_end, float* __restrict__ dists, unsigned long long* __restrict__ keys) {
+    const uint32_t q = blockIdx.y, rq = bq_row_u4(d);
+    const uint64_t beg = seg_beg[q], end = seg_end[q];
+    const uint4* qv = qbits + (size_t)q * rq;
+    const float qhdr = qh0 ? qh0[q] : 0.f;
+    const int sub = threadIdx.x & 3;
+    const uint64_t slot = (uint64_t)blockIdx.x * (blockDim.x >> 2) + (threadIdx.x >> 2), nslots = (uint64_t)gridDim.x * (blockDim.x >> 2);
+    for (uint64_t p0 = beg; p0 < end; p0 += nslots) {   // the same trip count on every lane: the shuffles below need all 32
+        const uint64_t p = p0 + slot;
+        const bool v = p < end;
+        const uint32_t r = v ? rows[p] : 0u;
+        const uint4* x = items + (size_t)r * rq;
+        int pc = 0;
+        for (uint32_t c = (uint32_t)sub; c < rq; c += 4) {
+            const uint4 a = ldg_stream_u4(x + c), b = __ldg(qv + c);
+            pc += __popc(a.x ^ b.x) + __popc(a.y ^ b.y) + __popc(a.z ^ b.z) + __popc(a.w ^ b.w);
+        }
+        pc += __shfl_xor_sync(0xffffffffu, pc, 1);
+        pc += __shfl_xor_sync(0xffffffffu, pc, 2);
+        if (v && sub == 0) {
+            const float dist = metric == BQ_EUCLIDEAN ? (float)(4 * pc)
+                             : metric == BQ_MANHATTAN ? (float)(2 * pc)
+                             : built_finish(BQ_COSINE, (float)((int)d - 2 * pc), qhdr, ih0[r]);
+            dists[p] = dist;
+            keys[p] = ((unsigned long long)ordered_key(dist) << 32) | (unsigned long long)(uint32_t)(p - beg);
+        }
     }
 }
 

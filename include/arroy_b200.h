@@ -74,7 +74,8 @@ const char* arroy_b200_version(void);
  * [tag 0x00][Header POD][dim x f32 native endian], byte aligned only
  * (src/node.rs:224-228, src/unaligned_vector/f32.rs). The library decodes the unaligned
  * bytes into pinned host memory and uploads them once into float[n][ld] (ld = dim
- * rounded up to 32 floats, zero padded) plus header arrays. */
+ * rounded up to 32 floats, zero padded) plus header arrays; binary-quantized values are
+ * bit strings and stay bit strings on the device (arroy_b200_device_ptrs). */
 int32_t arroy_b200_stage_items(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
                                const uint32_t* ids_ascending, const uint8_t* const* leaf_values);
 
@@ -114,7 +115,10 @@ int32_t arroy_b200_dot_preprocess(arroy_ctx* ctx, float* out_extra_dim /* n or N
 
 /* For each row: margin = D::margin(normal, item) bit-exact with the reference's x86_64
  * AVX+FMA / SSE / scalar summation order; side = margin.is_sign_positive() ? 1 (Right)
- * : 0 (Left) (src/distance/mod.rs:103-110). out_margin may be NULL. */
+ * : 0 (Left) (src/distance/mod.rs:103-110). out_margin may be NULL. Binary-quantized metrics:
+ * the normal is a bit string in the reference, so only the sign of each element counts
+ * (is_sign_positive: +0.0 -> +1, -0.0 -> -1); the margin is hdr0 + dot of the +-1 vectors
+ * (Cosine: the dot). The same holds for arroy_b200_side_multi. */
 int32_t arroy_b200_side_batch(arroy_ctx* ctx, const float* normal, float hdr0, float hdr1,
                               const uint32_t* rows, uint64_t n_rows,
                               uint8_t* out_side, float* out_margin);
@@ -395,7 +399,8 @@ uint32_t arroy_b200_bq_quantize(const float* in, uint32_t dims, float* out);
 int32_t arroy_b200_epochs(arroy_ctx* ctx, uint64_t out[2]);
 
 /* Raw device pointers of the staged items (for the NCCL broadcast of the multi-GPU path):
- * out[0] = float[n][ld] matrix, out[1] = hdr0[n], out[2] = hdr1[n] (may be 0); *out_ld = ld. */
+ * out[0] = float[n][ld] matrix, out[1] = hdr0[n], out[2] = hdr1[n] (may be 0); *out_ld = ld. Binary-quantized metrics: the
+ * rows are bit strings of 16 * ceil(dims / 128) bytes and *out_ld is that byte count / 4. */
 int32_t arroy_b200_device_ptrs(arroy_ctx* ctx, void* out[3], uint32_t* out_ld);
 
 /* ---- several GPUs of one node behind one handle (SURVEY.md §8b / §8e) -------------------------------------------------
