@@ -31,6 +31,10 @@ SIGNATURES = [
     ("arroy_b200_destroy", None, [C.c_void_p]),
     ("arroy_b200_last_error", C.c_char_p, [C.c_void_p]),
     ("arroy_b200_stage_items", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.POINTER(C.c_void_p)]),
+    ("arroy_b200_stage_items_delta", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.POINTER(C.c_void_p), C.c_uint64, _u32p]),
+    ("arroy_b200_stage_stats", C.c_int32, [C.c_void_p, _u64p]),
+    ("arroy_b200_read_items", C.c_int32, [C.c_void_p, _u32p, C.c_uint64, C.c_void_p]),
+    ("arroy_b200_stage_delta_plan", C.c_uint64, [_u32p, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_uint64, C.POINTER(C.c_int64)]),
     ("arroy_b200_stage_items_flat", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.c_void_p, _f32p, _f32p]),
     ("arroy_b200_stage_items_device", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.c_void_p]),
     ("arroy_b200_item_headers", C.c_int32, [C.c_void_p, _f32p, _f32p]),
@@ -140,6 +144,15 @@ def bq_quantize(vector):
     out = np.empty((v.size + 63) // 64 * 64, dtype=np.float32)
     load().arroy_b200_bq_quantize(_fp(v), v.size, _fp(out))
     return out
+
+
+def stage_delta_plan(old_ids, new_ids, changed_ids):
+    """The plan of Context.stage_items_delta (host only): for every row of new_ids the row of old_ids it keeps, -1 = uploaded.
+    Returns (src int64 array, number of uploaded rows). The three id lists ascend strictly."""
+    old, new, ch = (np.ascontiguousarray(a, dtype=np.uint32) for a in (old_ids, new_ids, changed_ids))
+    src = np.empty(new.size, dtype=np.int64)
+    n = load().arroy_b200_stage_delta_plan(_up(old), old.size, _up(new), new.size, _up(ch), ch.size, src.ctypes.data_as(C.POINTER(C.c_int64)))
+    return src, int(n)
 
 
 class Context:
@@ -314,6 +327,28 @@ class Context:
         ptrs = np.ascontiguousarray(ptr_array, dtype=np.uint64)
         self._ck(self.lib.arroy_b200_stage_items(self.h, metric, dim, ids.size, _up(ids), ptrs.ctypes.data_as(C.POINTER(C.c_void_p))))
         self._staged(ids.size, dim, metric)
+
+    def stage_items_delta(self, metric, dim, ids, ptr_array, changed_ids):
+        """stage_items_ptrs that keeps the resident rows of every id not in changed_ids (ascending); see stage_stats()."""
+        metric = METRICS[metric] if isinstance(metric, str) else metric
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        ptrs = np.ascontiguousarray(ptr_array, dtype=np.uint64)
+        ch = np.ascontiguousarray(changed_ids, dtype=np.uint32)
+        self._ck(self.lib.arroy_b200_stage_items_delta(self.h, metric, dim, ids.size, _up(ids), ptrs.ctypes.data_as(C.POINTER(C.c_void_p)), ch.size, _up(ch)))
+        self._staged(ids.size, dim, metric)
+
+    def stage_stats(self):
+        out = (C.c_uint64 * 4)()
+        self._ck(self.lib.arroy_b200_stage_stats(self.h, out))
+        return {"uploaded_rows": int(out[0]), "moved_rows": int(out[1]), "delta": int(out[2]), "h2d_bytes": int(out[3])}
+
+    def read_items(self, rows=None):
+        """The raw resident rows (all of them by default) as a uint8 array n_rows x row_bytes, padding included."""
+        rows = np.arange(self.n, dtype=np.uint32) if rows is None else np.ascontiguousarray(rows, dtype=np.uint32)
+        _, ld = self.device_ptrs()
+        out = np.empty((rows.size, 4 * ld), dtype=np.uint8)
+        self._ck(self.lib.arroy_b200_read_items(self.h, _up(rows), rows.size, out.ctypes.data))
+        return out
 
     def stage_begin(self, metric, dim, ids):
         metric = METRICS[metric] if isinstance(metric, str) else metric

@@ -18,6 +18,7 @@ HOST_SIGNATURES = [
     ("arroy_env_free", None, [C.c_void_p]),
     ("arroy_env_len", C.c_uint64, [C.c_void_p]),
     ("arroy_env_iter", C.c_int32, [C.c_void_p, KV_SINK, C.c_void_p]),
+    ("arroy_env_resident", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_env_put_raw", C.c_int32, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64]),
     ("arroy_host_reencode", C.c_int32, [C.c_int32, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, _u64p]),
     ("arroy_rng_from_seed", C.c_void_p, [_u8p]),
@@ -177,6 +178,13 @@ class Env:
     def put_raw(self, key, value):
         """Insert one (key, value) pair as is (importing the content of a real arroy LMDB file)."""
         _ck(_lib().arroy_env_put_raw(self.h, key, len(key), value, len(value)))
+
+    def resident(self):
+        """The table's record of the items it left on the device: None, or {"index", "epoch", "dirty"} (dirty = how many item
+        ids were written or deleted since those rows were staged)."""
+        out = (C.c_uint64 * 4)()
+        _ck(_lib().arroy_env_resident(self.h, out))
+        return {"index": int(out[1]), "epoch": int(out[2]), "dirty": int(out[3])} if out[0] else None
 
     def tree_nodes(self, index=0):
         """{node id: NodeCodec bytes} of one index."""

@@ -23,6 +23,7 @@
 #include "xrerank.cuh"
 #include "tcgemm.cuh"
 #include "frerank.cuh"
+#include "restage.cuh"
 
 using namespace ab;
 
@@ -125,6 +126,7 @@ struct arroy_ctx {
     std::vector<StageWorker> stage_workers;
     bool staging_open = false;             // between arroy_b200_stage_begin and arroy_b200_stage_end
     std::vector<float> stage_h0, stage_h1;  // headers decoded from the leaf values staged so far
+    uint64_t stage_stats[4] = {0, 0, 0, 0};  // the last arroy_b200_stage_items / _delta call (arroy_b200_stage_stats)
     // device-resident forest for the batched query path (arroy_b200_load_forest)
     DevBuf f_kind, f_left, f_right, f_nidx, f_nh0, f_doff, f_dlen, f_normals, f_desc, f_roots, f_rec, f_nofn;
     DevForest forest{};
@@ -212,6 +214,10 @@ void compute_norms(arroy_ctx* c, bool with_max) {
     c->n_launches += 1;
 }
 
+// Stage epochs are unique in the process, not per context: an owner that remembers (context, epoch) is not fooled by a new
+// context that was created at the address of a destroyed one.
+uint64_t next_stage_epoch() { static std::atomic<uint64_t> last{0}; return ++last; }
+
 void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint32_t* ids) {
     if (metric < 0 || metric > BQ_MANHATTAN) throw ArgError("unknown metric");
     if (dim == 0) throw ArgError("dim must be > 0");
@@ -222,7 +228,7 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
     // a restage invalidates everything derived from the previous items: the bf16 shadow, the 8-bit planes and the device forest
     // (its descendant rows were validated against the previous item count)
     c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false; c->staging_open = false;
-    c->stage_epoch += 1;
+    c->stage_epoch = next_stage_epoch();
     c->metric = metric; c->dim = dim; c->ld = (dim + 31u) & ~31u; c->n = n;
     c->row_bytes = is_bq(metric) ? 16u * bq_row_u4(dim) : 4u * c->ld;
     c->ids.assign(ids, ids + n);
@@ -1326,40 +1332,177 @@ void arroy_b200_destroy(arroy_ctx* c) {
 
 const char* arroy_b200_last_error(arroy_ctx* c) { return c ? c->err.c_str() : "null context"; }
 
+}  // extern "C"
+
+namespace {
+
+// h0 / h1 of the raw stored Leaf values: [tag 0x00][Header POD][vector], byte aligned only
+void decode_leaf_headers(const uint8_t* const* leaf_values, uint64_t n, int hf, std::vector<float>& h0, std::vector<float>& h1) {
+    h0.assign(n, 0.f); h1.assign(n, 0.f);
+    std::atomic<int> bad{0};
+    const unsigned nt = n < 65536 ? 1u : std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
+    auto hdrs = [&](uint64_t i0, uint64_t i1) {
+        for (uint64_t i = i0; i < i1; ++i) {
+            const uint8_t* v = leaf_values[i];
+            if (!v || v[0] != 0) { bad = 1; return; }
+            memcpy(&h0[i], v + 1, 4);
+            if (hf == 2) memcpy(&h1[i], v + 5, 4);
+        }
+    };
+    if (nt <= 1) hdrs(0, n);
+    else { std::vector<std::thread> th; for (unsigned t = 0; t < nt; ++t) th.emplace_back(hdrs, n * t / nt, n * (t + 1) / nt); for (auto& x : th) x.join(); }
+    if (bad.load()) throw ArgError("leaf value does not start with the Leaf tag 0x00");
+}
+
+void upload_headers(arroy_ctx* c, const std::vector<float>& h0, const std::vector<float>& h1) {
+    const uint64_t n = c->n;
+    if (n) {
+        CK(cudaMemcpyAsync(c->h0.p, h0.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(c->h1.p, h1.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    c->h2d_bytes += 8 * n;
+}
+
+void stage_items_full(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values) {
+    const uint64_t h2d0 = c->h2d_bytes;
+    alloc_items(c, metric, dim, n, ids);
+    const int hf = metric_header_floats(metric);
+    std::vector<float> h0, h1;
+    decode_leaf_headers(leaf_values, n, hf, h0, h1);
+    const size_t voff = 1 + 4 * (size_t)hf;
+    // binary-quantized leaves store the bit string (node.rs:224-228 with VectorCodec = BinaryQuantized)
+    stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return leaf_values[i] + voff; }, nullptr, 0, true, is_bq(metric) ? 2 : 0);
+    upload_headers(c, h0, h1);
+    c->staged = true;
+    c->stage_stats[0] = n; c->stage_stats[1] = 0; c->stage_stats[2] = 0; c->stage_stats[3] = c->h2d_bytes - h2d0;
+}
+
+constexpr size_t RESTAGE_SCRATCH_BYTES = 192ull << 20;   // with DevBuf's slack: at most 240 MB + 256 bytes, whatever the index size
+constexpr size_t RESTAGE_PIECE_BYTES = 64ull << 10;
+
+void launch_restage(arroy_ctx* c, const RestagePiece* pieces, uint64_t n_pieces, uint4* scratch, int phase) {
+    if (n_pieces == 0) return;
+    const unsigned grid = (unsigned)std::min<uint64_t>(n_pieces, (uint64_t)c->sm_count * 8);
+    restage_copy_rows_kernel<<<grid, RESTAGE_THREADS, 0, c->stream>>>(c->items.as<uint4>(), scratch, pieces, n_pieces, c->row_bytes / 16, phase);
+    CK(cudaGetLastError());
+    c->n_launches += 1;
+}
+
+// The delta path of arroy_b200_stage_items_delta; false = one of the conditions for it does not hold (nothing was changed).
+bool stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values, uint64_t n_changed,
+                       const uint32_t* changed_ids) {
+    if (!c->staged || c->staging_open || n == 0 || c->n == 0) return false;
+    if (metric != c->metric || dim != c->user_dim) return false;   // row_bytes follows from the two
+    if ((size_t)n * c->row_bytes > c->items.cap) return false;     // the resident buffer cannot hold the new matrix
+    std::vector<int64_t> src(n);
+    const uint64_t n_upload = stage_delta_plan(c->ids.data(), c->n, ids, n, changed_ids, n_changed, src.data());
+    if (n_upload * 4 > n) return false;   // more than a quarter of the matrix crosses PCIe anyway: the plain pipeline is as good
+    const uint64_t window_rows = std::max<uint64_t>(1, RESTAGE_SCRATCH_BYTES / c->row_bytes), piece_rows = std::max<uint64_t>(1, RESTAGE_PIECE_BYTES / c->row_bytes);
+    const RestagePieces mv = restage_move_pieces(src.data(), n, window_rows, piece_rows), up = restage_upload_pieces(src.data(), n, window_rows, piece_rows);
+    const int hf = metric_header_floats(metric);
+    std::vector<float> h0, h1;
+    decode_leaf_headers(leaf_values, n, hf, h0, h1);
+    // scratch for one window, released again below: a card filled by its index has no room to lend for longer
+    DevBuf scratch, d_pieces;
+    struct Release { DevBuf &a, &b; ~Release() { a.release(); b.release(); } } release{scratch, d_pieces};
+    const uint64_t n_pieces = mv.pieces.size() + up.pieces.size();
+    if (n_pieces) {
+        try {
+            scratch.ensure(std::min<size_t>(RESTAGE_SCRATCH_BYTES, (size_t)std::min<uint64_t>(window_rows, std::max(mv.rows, up.rows)) * c->row_bytes));
+            d_pieces.ensure(n_pieces * sizeof(RestagePiece));
+        } catch (const CudaError&) { cudaGetLastError(); return false; }   // no room for the scratch: the full staging needs none
+    }
+    // from here on the context changes: what alloc_items invalidates is invalid here too (the bf16 shadow, the 8-bit planes and
+    // the device forest follow rows, not ids)
+    const uint64_t h2d0 = c->h2d_bytes;
+    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false;
+    c->stage_epoch = next_stage_epoch();
+    c->n = n;
+    c->ids.assign(ids, ids + n);
+    CK(cudaStreamSynchronize(c->stream));   // h0 / h1 may be reallocated: nothing may still read them
+    c->h0.ensure(std::max<size_t>(16, n * 4));
+    c->h1.ensure(std::max<size_t>(16, n * 4));
+    if (n_pieces) {
+        RestagePiece* dp = d_pieces.as<RestagePiece>();
+        if (!mv.pieces.empty()) CK(cudaMemcpyAsync(dp, mv.pieces.data(), mv.pieces.size() * sizeof(RestagePiece), cudaMemcpyHostToDevice, c->stream));
+        if (!up.pieces.empty()) CK(cudaMemcpyAsync(dp + mv.pieces.size(), up.pieces.data(), up.pieces.size() * sizeof(RestagePiece), cudaMemcpyHostToDevice, c->stream));
+        c->h2d_bytes += n_pieces * sizeof(RestagePiece);
+        for (const RestageWindow& w : mv.windows) {
+            launch_restage(c, dp + w.piece0, w.n_pieces, scratch.as<uint4>(), 0);
+            launch_restage(c, dp + w.piece0, w.n_pieces, scratch.as<uint4>(), 1);
+        }
+        // the uploaded rows, after every move (they overwrite rows the moves read): host -> scratch through the bounce buffers of
+        // the staging pipeline, scratch -> their rows
+        std::vector<uint64_t> up_rows;
+        up_rows.reserve(n_upload);
+        for (uint64_t r = 0; r < n; ++r) if (src[r] < 0) up_rows.push_back(r);
+        const size_t voff = 1 + 4 * (size_t)hf;
+        uint64_t k0 = 0;
+        for (const RestageWindow& w : up.windows) {
+            uint64_t rows = 0;
+            for (uint64_t p = 0; p < w.n_pieces; ++p) rows += up.pieces[w.piece0 + p].len;
+            stage_rows_pipeline(c, rows, c->dim, c->row_bytes, [&](uint64_t i) { return leaf_values[up_rows[k0 + i]] + voff; }, scratch.as<uint8_t>(), 0, true,
+                                is_bq(metric) ? 2 : 0);
+            launch_restage(c, dp + mv.pieces.size() + w.piece0, w.n_pieces, scratch.as<uint4>(), 1);
+            k0 += rows;
+        }
+    }
+    upload_headers(c, h0, h1);   // ends in a stream synchronise: the scratch buffer is idle when it is released
+    c->staged = true;
+    c->stage_stats[0] = n_upload; c->stage_stats[1] = mv.rows; c->stage_stats[2] = 1; c->stage_stats[3] = c->h2d_bytes - h2d0;
+    return true;
+}
+
+}  // namespace
+
+extern "C" {
+
 int32_t arroy_b200_stage_items(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values) {
     return guarded(c, [&] {
         set_device(c);
         if (n && (!ids || !leaf_values)) throw ArgError("null ids / leaf_values");
-        alloc_items(c, metric, dim, n, ids);
-        const int hf = metric_header_floats(metric);
-        std::vector<float> h0(n), h1(n, 0.f);
-        // decode the unaligned LMDB values: [tag][Header][dim x f32]
-        {
-            std::atomic<int> bad{0};
-            const unsigned nt = n < 65536 ? 1u : std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
-            auto hdrs = [&](uint64_t i0, uint64_t i1) {
-                for (uint64_t i = i0; i < i1; ++i) {
-                    const uint8_t* v = leaf_values[i];
-                    if (!v || v[0] != 0) { bad = 1; return; }
-                    memcpy(&h0[i], v + 1, 4);
-                    if (hf == 2) memcpy(&h1[i], v + 5, 4);
-                }
-            };
-            if (nt <= 1) hdrs(0, n);
-            else { std::vector<std::thread> th; for (unsigned t = 0; t < nt; ++t) th.emplace_back(hdrs, n * t / nt, n * (t + 1) / nt); for (auto& x : th) x.join(); }
-            if (bad.load()) throw ArgError("leaf value does not start with the Leaf tag 0x00");
-        }
-        const size_t voff = 1 + 4 * (size_t)hf;
-        // binary-quantized leaves store the bit string (node.rs:224-228 with VectorCodec = BinaryQuantized)
-        stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return leaf_values[i] + voff; }, nullptr, 0, true, is_bq(metric) ? 2 : 0);
-        if (n) {
-            CK(cudaMemcpyAsync(c->h0.p, h0.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
-            CK(cudaMemcpyAsync(c->h1.p, h1.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+        stage_items_full(c, metric, dim, n, ids, leaf_values);
+    });
+}
+
+int32_t arroy_b200_stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values, uint64_t n_changed,
+                                     const uint32_t* changed_ids) {
+    return guarded(c, [&] {
+        set_device(c);
+        if (n && (!ids || !leaf_values)) throw ArgError("null ids / leaf_values");
+        if (n_changed && !changed_ids) throw ArgError("null changed_ids");
+        if (n > 0xffffffffull) throw ArgError("too many items");
+        for (uint64_t i = 1; i < n; ++i) if (ids[i] <= ids[i - 1]) throw ArgError("ids must be strictly ascending");
+        for (uint64_t i = 1; i < n_changed; ++i) if (changed_ids[i] <= changed_ids[i - 1]) throw ArgError("changed_ids must be strictly ascending");
+        if (!stage_items_delta(c, metric, dim, n, ids, leaf_values, n_changed, changed_ids)) stage_items_full(c, metric, dim, n, ids, leaf_values);
+    });
+}
+
+int32_t arroy_b200_stage_stats(arroy_ctx* c, uint64_t out[4]) {
+    return guarded(c, [&] { if (!out) throw ArgError("null argument"); for (int i = 0; i < 4; ++i) out[i] = c->stage_stats[i]; });
+}
+
+int32_t arroy_b200_read_items(arroy_ctx* c, const uint32_t* rows, uint64_t n_rows, uint8_t* out) {
+    return guarded(c, [&] {
+        require_staged(c); set_device(c);
+        if (n_rows == 0) return;
+        if (!rows || !out) throw ArgError("null argument");
+        for (uint64_t i = 0; i < n_rows; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
+        for (uint64_t i = 0; i < n_rows;) {   // one copy per run of consecutive rows
+            uint64_t e = i + 1;
+            while (e < n_rows && rows[e] == rows[e - 1] + 1) ++e;
+            CK(cudaMemcpyAsync(out + i * c->row_bytes, c->items.as<uint8_t>() + (size_t)rows[i] * c->row_bytes, (e - i) * (size_t)c->row_bytes, cudaMemcpyDeviceToHost, c->stream));
+            i = e;
         }
         CK(cudaStreamSynchronize(c->stream));
-        c->h2d_bytes += 8 * n;
-        c->staged = true;
+        c->d2h_bytes += n_rows * (uint64_t)c->row_bytes;
     });
+}
+
+uint64_t arroy_b200_stage_delta_plan(const uint32_t* old_ids, uint64_t n_old, const uint32_t* new_ids, uint64_t n_new, const uint32_t* changed_ids, uint64_t n_changed,
+                                     int64_t* out_src) {
+    return stage_delta_plan(old_ids, n_old, new_ids, n_new, changed_ids, n_changed, out_src);
 }
 
 // ---- staging in pieces (multi-GPU: the H2D copy of chunk k + 1 overlaps the broadcast of chunk k) ---------------------------

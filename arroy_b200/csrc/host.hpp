@@ -135,6 +135,22 @@ struct arroy_env {
                                               // value it was opened at (the table has no RoTxn snapshots: a reader that outlives a
                                               // write to its index fails with NeedBuild instead of mixing two states)
     void touch(uint16_t index) { generation++; index_gen[index]++; }
+    // Which items are resident on the device, as far as this table knows: the item rows of `index` as they were when `ctx`
+    // staged them under stage epoch `epoch` (arroy_b200_epochs), and the ids written or deleted since (`dirty`). A build hands
+    // `dirty` to arroy_b200_stage_items_delta and a Reader adopts the rows when `dirty` is empty, as long as the context still
+    // reports `epoch`: any staging by somebody else changes it. Whatever else could change an Item value or what the index is
+    // drops the record; a dropped record only costs one full staging.
+    struct Resident {
+        bool valid = false;
+        arroy_ctx* ctx = nullptr;
+        uint64_t epoch = 0;
+        uint16_t index = 0;
+        int metric = 0;
+        uint32_t dims = 0;
+        std::set<uint32_t> dirty;
+    } resident;
+    void mark_dirty(uint16_t index, uint32_t item) { if (resident.valid && resident.index == index) resident.dirty.insert(item); }
+    void drop_resident(uint16_t index) { if (resident.valid && resident.index == index) resident = Resident(); }
     uint64_t gen_of(uint16_t index) const { auto it = index_gen.find(index); return it == index_gen.end() ? 0 : it->second; }
 };
 struct arroy_rng {
@@ -210,8 +226,12 @@ inline void put_item(arroy_writer* w, uint32_t item, const float* v) {  // Write
     new_header(w->metric, v, w->dims, h0, h1);
     w->env->kv[make_key(w->index, MODE_ITEM, item)] = encode_leaf(w->metric, v, w->dims, h0, h1);
     w->env->kv[make_key(w->index, MODE_UPDATED, item)] = std::string();
+    w->env->mark_dirty(w->index, item);
     w->env->touch(w->index);
 }
+
+// ARROY_B200_FULL_RESTAGE=1: no residency record is kept, so every build and every reader stages all items (DESIGN.md section 10)
+inline bool full_restage() { const char* v = getenv("ARROY_B200_FULL_RESTAGE"); return v && v[0] == '1'; }
 
 struct ItemView { std::vector<uint32_t> ids; std::vector<const uint8_t*> ptrs; std::vector<size_t> sizes; };
 inline ItemView collect_items(arroy_env* env, uint16_t index) {
@@ -223,6 +243,24 @@ inline ItemView collect_items(arroy_env* env, uint16_t index) {
         v.sizes.push_back(it->second.size());
     }
     return v;
+}
+// Stage the items of a build or a reader: only what the residency record says has changed when it is about this index on this
+// context and the context still holds what it recorded, everything otherwise. Items are not part of a build's transaction
+// (add_item / del_item wrote them before), so the record is renewed here and stays right when the build fails or is cancelled
+// afterwards. DotProduct: arroy_b200_dot_preprocess recomputes every header on the device from the resident vectors and the
+// commit writes the same values into the table, and the delta staging uploads all headers anyway: the record stays valid.
+inline void stage_resident(arroy_env* env, arroy_ctx* ctx, uint16_t index, int metric, uint32_t dims, const ItemView& items) {
+    arroy_env::Resident& res = env->resident;
+    uint64_t ep[2] = {0, 0};
+    dev_ck(ctx, arroy_b200_epochs(ctx, ep));
+    const bool delta = !full_restage() && res.valid && res.ctx == ctx && res.index == index && res.metric == metric && res.dims == dims && ep[0] != 0 && ep[0] == res.epoch;
+    const std::vector<uint32_t> changed(res.dirty.begin(), res.dirty.end());
+    res = arroy_env::Resident();   // a staging that fails leaves nothing to rely on
+    if (delta) dev_ck(ctx, arroy_b200_stage_items_delta(ctx, metric, dims, items.ids.size(), items.ids.data(), items.ptrs.data(), changed.size(), changed.data()));
+    else dev_ck(ctx, arroy_b200_stage_items(ctx, metric, dims, items.ids.size(), items.ids.data(), items.ptrs.data()));
+    if (full_restage()) return;
+    dev_ck(ctx, arroy_b200_epochs(ctx, ep));
+    res.valid = true; res.ctx = ctx; res.epoch = ep[0]; res.index = index; res.metric = metric; res.dims = dims;
 }
 inline void erase_mode(arroy_env* env, uint16_t index, uint8_t mode) {
     auto b = env->kv.lower_bound(make_key(index, mode, 0));
@@ -782,9 +820,11 @@ inline void writer_build(arroy_writer* w, arroy_ctx* ctx, arroy_rng* rng, int64_
     const bool needs_device = n > K_early || (w->metric == ARROY_B200_DOT_PRODUCT && n > 0);
     if (needs_device) {
         if (!ctx) throw HostError(ARROY_B200_ERR_CUDA, "no CUDA device context: arroy_b200 has no CPU fallback");
-        dev_ck(ctx, arroy_b200_stage_items(ctx, w->metric, d, n, items.ids.data(), items.ptrs.data()));
+        stage_resident(env, ctx, index, w->metric, d, items);
         w->timings[0] = ms_since(t0);
-        w->timings[5] = (double)n * (((d + 31) & ~31u) * 4.0 + 8.0);
+        uint64_t st[4] = {0, 0, 0, 0};
+        dev_ck(ctx, arroy_b200_stage_stats(ctx, st));
+        w->timings[5] = (double)st[3];
     }
     if (w->metric == ARROY_B200_DOT_PRODUCT && n > 0) {
         t0 = clk::now();
@@ -1081,9 +1121,17 @@ inline void ensure_staged(arroy_reader* r) {
     if (r->stage_epoch != 0 && ep[0] == r->stage_epoch) return;   // the resident items are still the ones this reader staged
     std::lock_guard<std::mutex> lk(r->env->mu);
     check_fresh_locked(r);
+    {   // the rows a build of this index left on the device, with nothing written since: they are this reader's items
+        const arroy_env::Resident& res = r->env->resident;
+        if (!full_restage() && res.valid && res.ctx == r->ctx && res.index == r->index && res.metric == r->metric && res.dims == r->dims && res.dirty.empty() &&
+            ep[0] != 0 && ep[0] == res.epoch) {
+            r->stage_epoch = ep[0];
+            return;
+        }
+    }
     ItemView iv = collect_items(r->env, r->index);
     if (iv.ids != r->items) throw HostError(ARROY_ERR_NEED_BUILD, "The trees have not been built after an update on index " + std::to_string(r->index));
-    dev_ck(r->ctx, arroy_b200_stage_items(r->ctx, r->metric, r->dims, iv.ids.size(), iv.ids.data(), iv.ptrs.data()));
+    stage_resident(r->env, r->ctx, r->index, r->metric, r->dims, iv);
     dev_ck(r->ctx, arroy_b200_epochs(r->ctx, ep));
     r->stage_epoch = ep[0];
     r->forest_epoch = 0;   // staging drops whatever forest was resident
@@ -1306,6 +1354,13 @@ int32_t arroy_env_iter(arroy_env* e, arroy_kv_sink sink, void* arg) {
     });
 }
 
+int32_t arroy_env_resident(arroy_env* e, uint64_t out[4]) {
+    return hguard([&] {
+        std::lock_guard<std::mutex> lk(e->mu);
+        out[0] = e->resident.valid ? 1 : 0; out[1] = e->resident.index; out[2] = e->resident.epoch; out[3] = e->resident.dirty.size();
+    });
+}
+
 // Raw access to the table (tests: importing the key/value pairs of a real LMDB file; exporting ours).
 int32_t arroy_env_put_raw(arroy_env* e, const uint8_t* key, uint64_t key_len, const uint8_t* val, uint64_t val_len) {
     return hguard([&] {
@@ -1314,6 +1369,7 @@ int32_t arroy_env_put_raw(arroy_env* e, const uint8_t* key, uint64_t key_len, co
         Key8 k;
         memcpy(k.data(), key, 8);
         e->kv[k] = std::string(reinterpret_cast<const char*>(val), val_len);
+        e->drop_resident((uint16_t)(((uint16_t)key[0] << 8) | key[1]));
         e->touch((uint16_t)(((uint16_t)key[0] << 8) | key[1]));
     });
 }
@@ -1368,6 +1424,10 @@ void arroy_rng_fill_f32(arroy_rng* r, float* out, uint64_t n) { for (uint64_t i 
 arroy_writer* arroy_writer_new(arroy_env* env, uint16_t index, uint32_t dimensions, int32_t metric) {
     auto* w = new arroy_writer();
     w->env = env; w->index = index; w->dims = dimensions; w->metric = metric;
+    {   // a Writer with another distance or dimension on the index whose items are resident: they are not that index' any more
+        std::lock_guard<std::mutex> lk(env->mu);
+        if (env->resident.metric != metric || env->resident.dims != dimensions) env->drop_resident(index);
+    }
     return w;
 }
 void arroy_writer_free(arroy_writer* w) { delete w; }
@@ -1395,7 +1455,7 @@ int32_t arroy_writer_del_item(arroy_writer* w, uint32_t item, int32_t* out_exist
     return hguard([&] {
         std::lock_guard<std::mutex> lk(w->env->mu);
         bool ex = w->env->kv.erase(make_key(w->index, MODE_ITEM, item)) > 0;
-        if (ex) { w->env->kv[make_key(w->index, MODE_UPDATED, item)] = std::string(); w->env->touch(w->index); }
+        if (ex) { w->env->kv[make_key(w->index, MODE_UPDATED, item)] = std::string(); w->env->mark_dirty(w->index, item); w->env->touch(w->index); }
         if (out_existed) *out_existed = ex ? 1 : 0;
     });
 }
@@ -1403,6 +1463,7 @@ int32_t arroy_writer_clear(arroy_writer* w) {  // writer.rs:444-457
     return hguard([&] {
         std::lock_guard<std::mutex> lk(w->env->mu);
         for (uint8_t m = 0; m < 4; ++m) erase_mode(w->env, w->index, m);
+        w->env->drop_resident(w->index);
         w->env->touch(w->index);
     });
 }

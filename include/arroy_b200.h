@@ -79,6 +79,38 @@ const char* arroy_b200_version(void);
 int32_t arroy_b200_stage_items(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
                                const uint32_t* ids_ascending, const uint8_t* const* leaf_values);
 
+/* The same staging for a caller that knows which items it has written since the resident ones were staged: same arguments and
+ * the same postcondition as arroy_b200_stage_items (the context holds exactly the n items given, row = rank of the id, headers
+ * from the leaf values, a new stage epoch; the bf16 shadow, the 8-bit planes and the loaded forest are invalid), but the rows
+ * that are resident already stay on the device and only move to their new place (csrc/restage.cuh).
+ * The caller's promise: for every id that is resident (given to the last staging call) and in ids_ascending and NOT in
+ * changed_ids, the resident row equals the vector in leaf_values. changed_ids ascends strictly; ids in it that are not in
+ * ids_ascending (deleted items) are ignored; ids of ids_ascending that are not resident are uploaded whether listed or not.
+ * Headers are small and DotProduct::preprocess rewrites all of them, so h0 / h1 of all n leaf values are read and uploaded.
+ * The library stages in full, exactly as arroy_b200_stage_items, when one of these holds (arroy_b200_stage_stats tells):
+ *   - nothing is staged, or a staging is open (arroy_b200_stage_begin without _end), or n or the resident count is 0;
+ *   - metric or dim differ from the resident ones (the row size follows from the two);
+ *   - n rows do not fit the capacity of the resident buffer (it is allocated with 25 % of slack, so repeated small appends
+ *     stay in place);
+ *   - more than a quarter of the n rows would be uploaded;
+ *   - the scratch buffer of the move (at most 240 MB, released before the call returns) cannot be allocated. */
+int32_t arroy_b200_stage_items_delta(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
+                                     const uint32_t* ids_ascending, const uint8_t* const* leaf_values,
+                                     uint64_t n_changed, const uint32_t* changed_ids);
+/* Of the last arroy_b200_stage_items / arroy_b200_stage_items_delta call: out[0] = rows uploaded from the host, out[1] = rows
+ * moved on the device, out[2] = 1 if the delta path ran, 0 for a full staging, out[3] = bytes it copied host -> device: the
+ * uploaded rows, 8 n of headers and, on the delta path, 16 bytes per piece of its copy plan (a run of consecutive rows that
+ * moves or is uploaded, cut at 64 KB). */
+int32_t arroy_b200_stage_stats(arroy_ctx* ctx, uint64_t out[4]);
+/* The raw resident rows `rows` (row size as arroy_b200_device_ptrs reports it, padding included) copied to `out`; for tests,
+ * next to arroy_b200_item_headers and arroy_b200_prefilter_planes. */
+int32_t arroy_b200_read_items(arroy_ctx* ctx, const uint32_t* rows, uint64_t n_rows, uint8_t* out);
+/* The plan of the delta staging (host only, no device): out_src[r] = the row of old_ids that row r of new_ids keeps, -1 when
+ * its vector is uploaded (the id is not in old_ids, or is in changed_ids). All three lists ascend strictly. Returns the number
+ * of -1 entries. */
+uint64_t arroy_b200_stage_delta_plan(const uint32_t* old_ids, uint64_t n_old, const uint32_t* new_ids, uint64_t n_new,
+                                     const uint32_t* changed_ids, uint64_t n_changed, int64_t* out_src);
+
 /* The same staging in pieces: _begin sizes the device buffers for n items, _rows decodes + uploads the leaf values of rows
  * [row0, row0 + n_rows) (leaf_values[i] belongs to row row0 + i) and returns when they are in device memory, _end uploads the
  * headers collected from the leaf values and marks the items staged (headers_on_device != 0: the caller has filled the header
@@ -393,7 +425,8 @@ uint32_t arroy_b200_bq_quantize(const float* in, uint32_t dims, float* out);
 /* Ownership tokens of the device-resident state, for callers that share one context between several
  * readers / writers (the host keeps one context per heed::Env): out[0] = epoch of the staged items,
  * out[1] = epoch of the loaded forest; each is bumped by every arroy_b200_stage_items* /
- * arroy_b200_load_forest call and reads 0 while nothing valid is resident. A caller remembers the
+ * arroy_b200_load_forest call and reads 0 while nothing valid is resident (stage epochs are not reused by another context of
+ * the process). A caller remembers the
  * epochs it produced and re-stages / re-loads when they differ, instead of trusting state another
  * owner has replaced. */
 int32_t arroy_b200_epochs(arroy_ctx* ctx, uint64_t out[2]);

@@ -58,6 +58,11 @@ uint64_t arroy_env_len(arroy_env* env);
 typedef int32_t (*arroy_kv_sink)(void* arg, const uint8_t* key, uint64_t key_len, const uint8_t* val, uint64_t val_len);
 int32_t arroy_env_iter(arroy_env* env, arroy_kv_sink sink, void* arg);
 
+/* What the table knows about the items on the device (it keeps the rows of one index resident between builds and readers and
+ * hands arroy_b200_stage_items_delta the ids written since): out[0] = 1 if it has a record, out[1] = the index, out[2] = the
+ * stage epoch it was made under (arroy_b200_epochs), out[3] = item ids written or deleted since. For tests. */
+int32_t arroy_env_resident(arroy_env* env, uint64_t out[4]);
+
 /* raw put of one (key, value) pair — importing the content of a real arroy LMDB file (keys are the 8 bytes of src/key.rs:56-68) */
 int32_t arroy_env_put_raw(arroy_env* env, const uint8_t* key, uint64_t key_len, const uint8_t* val, uint64_t val_len);
 /* decode a stored value with the library's decoders and encode it again with its encoders (what = 0: tree node, 1: Metadata);
