@@ -156,26 +156,30 @@ __device__ __forceinline__ void scan_unit(const Job& jb, uint32_t unit, const fl
 // (every step exact in f64; |a|, |b|, |c| <= 127, U <= 254), n1_i = sigma (a_i + b_i / 254), n2_i = n1_i + sigma c_i / 254^2,
 // |n_i| <= sigma U_i / 2, and D1 >= sum |n_i - n1_i|, D2 >= sum |n_i - n2_i| are summed in f64 and rounded up, as is N1 >= |n|_1.
 // The reference's margin is fl(dot + c) (c = the bias / extra-dim term, formed exactly as the reference forms it; fl keeps the
-// sign of dot + c), with |dot - sum n_i x_i| <= gamma_R sum |n_i x_i|, gamma_R <= 1.001 d u in any summation order, and
-// |x_i| <= M <= 127.001 s.
+// sign of dot + c), with |dot - sum n_i x_i| <= gamma_R sum |n_i x_i| + wa, gamma_R <= 1.001 d u in any summation order, and
+// |x_i| <= M <= 127.001 s. wa is the part of the reference's error that is not relative: a product n_i x_i (a multiply or the
+// multiply of an FMA) whose result is subnormal loses up to 2^-150 absolutely, and rows far below 1 make every product do so
+// (rows below 2^-73 also leave the reference's split normal unnormalized, so n is as tiny as x). An add whose result is
+// subnormal is exact, and each of the d losses is carried through at most d later roundings (a factor of at most 1 + gamma_R,
+// with d gamma_R <= 5 for d <= PLANES_MAX_D), so wa = (d + 32) 2^-150 covers them all, exact in f64. Both stage tests below
+// add wa to their bound; at ordinary magnitudes it is far below one ulp of the bound and changes no decision.
 //  stage 1, hi plane only (d bytes per row): T1 = 254 sum h_i a_i + sum h_i b_i, an exact integer (each int32 sum is at most
 //    127 * 127 * 8192 < 2^31 in magnitude for d <= PLANES_MAX_D), so s sigma T1 / 254 = s sum h_i n1_i and
 //    |dot - s sum h_i n1_i| <= s (E1 N1 + 127 D1 + 127.001 gamma_R N1).
-//    The row is certain when |p + c| > s w1 in f64, p = fl(fl(T1 s) k1), k1 = fl(sigma / 254), w1 = (N1 (E1 + 127.001 gamma_R)
-//    + 127 D1) (1 + 2^-20) rounded up: the factor 1 + 2^-20 covers the relative errors of p (3 roundings on |p| <= 254 s N1)
-//    and of the test (2^-53 each).
+//    The row is certain when |p + c| > s w1 + wa in f64, p = fl(fl(T1 s) k1), k1 = fl(sigma / 254), w1 = (N1 (E1 + 127.001
+//    gamma_R) + 127 D1) (1 + 2^-20) rounded up: the factor 1 + 2^-20 covers the relative errors of p (3 roundings on
+//    |p| <= 254 s N1) and of the test (2^-53 each; s w1 and wa are both positive, so the sum's rounding is relative too).
 //  stage 2, the rows stage 1 left (both planes; the hi row was just streamed by this CTA): y_i = 254 h_i + l_i (|y_i| <= 32385),
 //    T2 = sum y_i (254^2 a_i + 254 b_i + c_i) from the six int32 sums of h, l times a, b, c (|T2| <= 2.2e15 < 2^53: exact in f64),
 //    so s sigma T2 / 254^3 = (s / 254) sum y_i n2_i, and with A = 254 sum |h_i| U_i + sum |l_i| U_i (sum |n_i| |y_i| <= sigma A / 2):
-//    |dot - (s/254) sum y_i n2_i| <= s E2 N1 + (s/254) 32385 D2 + gamma_R ((s/254) sigma A / 2 + s E2 N1)
-//                                  = (s/254) (254 E2 (1 + gamma_R) N1 + 32385 D2 + gamma_R sigma A / 2).
-//    The row is certain when |p2 + c| > s (w2 + rel2 A) in f64, p2 = fl(fl(T2 s) k2), k2 = fl(sigma / 254^3),
+//    |dot - (s/254) sum y_i n2_i| <= s E2 N1 + (s/254) 32385 D2 + gamma_R ((s/254) sigma A / 2 + s E2 N1) + wa
+//                                  = (s/254) (254 E2 (1 + gamma_R) N1 + 32385 D2 + gamma_R sigma A / 2) + wa.
+//    The row is certain when |p2 + c| > s (w2 + rel2 A) + wa in f64, p2 = fl(fl(T2 s) k2), k2 = fl(sigma / 254^3),
 //    w2 = (254 E2 (1 + gamma_R) N1 + 32385 D2) (1 + 2^-20) / 254, rel2 = gamma_R sigma / 508 (1 + 2^-20), both rounded up (the
 //    factor covers p2's 3 roundings on |p2| <= 255 s N1 and the test's own).
 //  stage 3: every other row — near the hyperplane, zero, non-finite — is scored from the f32 row in the reference's summation
 //    order (scan_unit's arithmetic). Flags and unit counts are the exact scan's.
-// A normal with a non-finite element gets NaN factors: no row is certain. The bounds are relative: like any such rule they assume
-// that no product n_i x_i underflows.
+// A normal with a non-finite element gets NaN factors: no row is certain.
 constexpr uint32_t PLANES_MAX_D = 8192;
 constexpr uint32_t PLANES_CHUNK = 4;          // scan units per claim on this path (256 rows)
 
@@ -249,6 +253,7 @@ __device__ __forceinline__ uint4 abs_bytes(const uint4 w) {
 struct PlanesNormal {
     double w1, k1;               // stage 1: bound factor, sigma / 254
     double w2, rel2, k2;         // stage 2: bound factors, sigma / 254^3
+    double wa;                   // both stages: the absolute term (d + 32) 2^-150 of products that underflow
 };
 constexpr uint32_t PLANES_LIMBS = 4;   // ld bytes each
 
@@ -302,7 +307,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
                 for (int r = 0; r < 4; ++r) { sa[r] = dp16(v[sidx][r], la, sa[r]); sb[r] = dp16(v[sidx][r], lb, sb[r]); }
             }
         }
-        const double w1 = pn->w1, k1 = pn->k1;
+        const double w1 = pn->w1, k1 = pn->k1, wa = pn->wa;
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
 #pragma unroll
@@ -311,7 +316,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
             const float s = valid ? __ldg(pl.scale + rid[r]) : 0.f;
             const double t1 = (double)(254ll * sa[r] + sb[r]);
             const double mt = __dadd_rn(__dmul_rn(__dmul_rn(t1, (double)s), k1), prefilter_c(metric, nh0, (metric == DOT_PRODUCT && valid) ? ih0[rid[r]] : 0.f));
-            const bool certain = fabs(mt) > __dmul_rn((double)s, w1);      // false for NaN / Inf scales and NaN factors
+            const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, w1), wa);      // false for NaN / Inf scales and NaN factors
             const bool leader = g8 == 0 && valid;
             const int side = mt > 0.0 ? 1 : 0;
             if (leader && certain) jb.flags[pos[r]] = (uint8_t)side;
@@ -361,7 +366,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
         const float s = __ldg(pl.scale + r);
         const double mt = __dadd_rn(__dmul_rn(__dmul_rn(m, (double)s), pn->k2), prefilter_c(metric, nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f));
-        const bool certain = fabs(mt) > __dmul_rn((double)s, __dadd_rn(pn->w2, __dmul_rn(pn->rel2, a)));
+        const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, __dadd_rn(pn->w2, __dmul_rn(pn->rel2, a))), pn->wa);
         const int side = mt > 0.0 ? 1 : 0;
         if (act && g8 == 0) {
             if (certain) { jb.flags[p] = (uint8_t)side; if (side == 0) atomicAdd(&sm_cnt[(p - base) / SCAN_UNIT], 1u); }
@@ -462,6 +467,7 @@ __device__ __forceinline__ void planes_job_factors(const float* sm_normal, uint3
         f.rel2 = __dmul_ru(__dmul_ru(gR, sigma * (0.5 * r254)), slack);
         f.k1 = sigma * (1.0 / 254.0);
         f.k2 = sigma * (1.0 / 16387064.0);
+        f.wa = (double)(d + 32u) * 0x1p-150;
         if (!finite) { f.w1 = __longlong_as_double(0x7ff8000000000000ll); f.w2 = f.w1; }
         *pn = f;
     }

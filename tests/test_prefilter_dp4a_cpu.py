@@ -9,7 +9,8 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
-from test_prefilter_planes_cpu import CASES, encode, make_case, reference_sides
+import oracle
+from test_prefilter_planes_cpu import CASES, TINY, encode, make_case, reference_sides
 
 F32 = np.float32
 
@@ -69,7 +70,7 @@ def limbs(nrm):
     return a.astype(np.int64), b.astype(np.int64), c.astype(np.int64), u.astype(np.int64), (finite, e, n1s, s1, s2)
 
 
-def factors(d, raw, factor=1.0, drop_limb_error=False):
+def factors(d, raw, factor=1.0, drop_limb_error=False, drop_abs_term=False):
     finite, e, n1s, s1, s2 = raw
     g, slack, u = 1.0 + 2.0 ** -30, 1.0 + 2.0 ** -20, 2.0 ** -24
     sigma = math.ldexp(1.0, e)
@@ -77,7 +78,7 @@ def factors(d, raw, factor=1.0, drop_limb_error=False):
     k1, k2 = sigma * (1.0 / 254.0), sigma * (1.0 / 16387064.0)
     if not finite:
         nan = float("nan")
-        return dict(w1=nan, k1=k1, w2=nan, rel2=0.0, k2=k2)
+        return dict(w1=nan, k1=k1, w2=nan, rel2=0.0, k2=k2, wa=0.0)
     n1 = mul_ru(n1s, g)
     D1 = mul_ru(mul_ru(s1, g), sigma * r254)
     D2 = mul_ru(mul_ru(s2, g), sigma * r64516)
@@ -88,7 +89,8 @@ def factors(d, raw, factor=1.0, drop_limb_error=False):
     w1 = mul_ru(add_ru(mul_ru(n1, add_ru(E1, mul_ru(127.001, gR))), mul_ru(127.0, D1)), slack)
     w2 = mul_ru(mul_ru(add_ru(mul_ru(mul_ru(n1, E2x254), add_ru(1.0, gR)), mul_ru(32385.0, D2)), slack), r254)
     rel2 = mul_ru(mul_ru(gR, sigma * (0.5 * r254)), slack)
-    return dict(w1=w1 * factor, k1=k1, w2=w2 * factor, rel2=rel2 * factor, k2=k2)
+    wa = 0.0 if drop_abs_term else math.ldexp(float(d + 32), -150)   # products that underflow: 2^-150 each, exact in f64
+    return dict(w1=w1 * factor, k1=k1, w2=w2 * factor, rel2=rel2 * factor, k2=k2, wa=wa * factor)
 
 
 def c_term(metric, nh0, ih0):
@@ -99,21 +101,21 @@ def c_term(metric, nh0, ih0):
     return np.full(ih0.size, float(F32(nh0)))
 
 
-def decide_planes(metric, nrm, nh0, hi, lo, s, ih0, d, factor=1.0, drop_limb_error=False):
+def decide_planes(metric, nrm, nh0, hi, lo, s, ih0, d, factor=1.0, drop_limb_error=False, drop_abs_term=False):
     """(stage-1 certain, stage-1 side, stage-2 certain, stage-2 side) for every row from its planes and scale."""
     a, b, c, u, raw = limbs(nrm)
-    f = factors(d, raw, factor, drop_limb_error)
+    f = factors(d, raw, factor, drop_limb_error, drop_abs_term)
     h, l = hi.astype(np.int64), lo.astype(np.int64)
     cc = c_term(metric, nh0, ih0)
     sd = s.astype(np.float64)
     with np.errstate(all="ignore"):
         t1 = (254 * (h @ a) + h @ b).astype(np.float64)
         mt1 = (t1 * sd) * f["k1"] + cc
-        c1 = np.abs(mt1) > sd * f["w1"]
+        c1 = np.abs(mt1) > sd * f["w1"] + f["wa"]
         t2 = (16387064 * (h @ a) + 64516 * (h @ b + l @ a) + 254 * (h @ c + l @ b) + l @ c).astype(np.float64)
         aa = (254 * (np.abs(h) @ u) + np.abs(l) @ u).astype(np.float64)
         mt2 = (t2 * sd) * f["k2"] + cc
-        c2 = np.abs(mt2) > sd * (f["w2"] + f["rel2"] * aa)
+        c2 = np.abs(mt2) > sd * (f["w2"] + f["rel2"] * aa) + f["wa"]
     return c1, mt1 > 0, c2, mt2 > 0
 
 
@@ -200,3 +202,119 @@ def test_limbs_fit_their_bytes_and_the_errors_are_bounded_above():
         D2 = mul_ru(mul_ru(raw[4], float(g)), float(sigma) * div_ru(1.0, 64516.0))
         assert Fraction(D1) >= sum(abs(n[i] - n1[i]) for i in range(512)) > 0
         assert Fraction(D2) >= sum(abs(n[i] - n2[i]) for i in range(512)) > 0
+
+
+# ---- rows whose products n_i x_i underflow ---------------------------------------------------------------------------------
+# Below about 2^-73 the reference's split normal keeps the magnitude of the rows (|p - q|^2 underflows, so normalize leaves it
+# as it is) and every product rounds to +-0: its margins are all +0, every row goes Right. The planes see the exact products in
+# f64, so only the absolute term wa keeps them from calling those rows certain.
+SEED = bytes([42] * 32)
+METRICS = ["euclidean", "cosine", "dot-product", "manhattan"]
+SWEEP_ROWS = {64: 3000, 768: 1000, 8192: 150}
+
+
+def headers(metric, rows):
+    """the items' header columns as the reference forms them: (h0, h1, the h0 the pre-filter reads)"""
+    n = rows.shape[0]
+    if metric == "cosine":
+        return np.array([oracle.new_header(oracle.COSINE, r)[0] for r in rows], dtype=np.float32), None, np.zeros(n, np.float32)
+    if metric == "dot-product":
+        h0, h1 = oracle.dot_preprocess(rows)
+        return h0, h1, h0
+    z = np.zeros(n, dtype=np.float32)
+    return z, None, z
+
+
+def split_case(metric, rows, normal=None):
+    """(oracle sides, pre-filter call) on rows for the normal create_split draws over all of them (or the normal given)"""
+    m = oracle.METRICS[metric]
+    h0, h1, ih0 = headers(metric, rows)
+    idx = np.arange(rows.shape[0], dtype=np.uint32)
+    hdr = (0.0, 0.0)
+    if normal is None:
+        normal, hdr = oracle.create_split(m, oracle.StdRng(SEED), rows, h0, h1, idx)
+    side, mg = oracle.side_batch(m, normal, hdr, rows, h0, h1, idx)
+
+    def call(**kw):
+        return decide(metric, normal, hdr[0], rows, ih0, **kw)
+    return side.astype(bool), mg, call
+
+
+def wrong_calls(ref, calls):
+    c1, r1, c2, r2 = calls
+    return int((c1 & (r1 != ref)).sum()), int((c2 & (r2 != ref)).sum())
+
+
+@pytest.mark.parametrize("d", sorted(SWEEP_ROWS))
+@pytest.mark.parametrize("metric", METRICS)
+def test_exponent_sweep_makes_no_wrong_call(metric, d):
+    base = oracle.synth_rows(SEED, d, 0, SWEEP_ROWS[d], 0.5)
+    underflowed = 0
+    for e in range(-60, -127, -1):
+        rows = (base * F32(2.0 ** e)).astype(np.float32)
+        ref, mg, call = split_case(metric, rows)
+        assert wrong_calls(ref, call()) == (0, 0), e
+        underflowed += bool(e <= -75 and not mg.view(np.uint32).any())
+    assert underflowed >= 40          # the sweep does reach the rows whose margins all round to +0
+
+
+@pytest.mark.parametrize("metric", METRICS)
+def test_the_absolute_term_is_needed(metric):
+    """Without wa both stages call rows Left whose reference margin is +0 (Right), at every exponent from -75 on."""
+    base = oracle.synth_rows(SEED, 768, 0, 1000, 0.5)
+    for e in (-75, -80, -100, -118):
+        ref, mg, call = split_case(metric, (base * F32(2.0 ** e)).astype(np.float32))
+        assert not mg.view(np.uint32).any() and ref.all(), e
+        w1, w2 = wrong_calls(ref, call(drop_abs_term=True))
+        assert w1 > 0 and w2 > 0, (e, w1, w2)
+
+
+@pytest.mark.parametrize("metric", METRICS)
+def test_the_absolute_term_changes_no_call_at_ordinary_magnitudes(metric):
+    base = oracle.synth_rows(SEED, 768, 0, 1000, 0.5)
+    for e in (0, -20, -40, -60):
+        _, _, call = split_case(metric, (base * F32(2.0 ** e)).astype(np.float32))
+        c1, r1, c2, r2 = call()
+        d1, s1, d2, s2 = call(drop_abs_term=True)
+        assert np.array_equal(c1, d1) and np.array_equal(c2, d2) and np.array_equal(r1, s1) and np.array_equal(r2, s2), e
+        assert (c1 | c2).sum() > 0.8 * c1.size
+
+
+@pytest.mark.parametrize("metric", METRICS)
+def test_mixed_row_exponents(metric):
+    rng = np.random.default_rng(len(metric))
+    base = oracle.synth_rows(SEED, 768, 0, 2000, 0.5)
+    for lo, hi in ((-126, -60), (-110, -74), (-20, 0)):
+        ex = rng.integers(lo, hi + 1, size=(base.shape[0], 1)).astype(np.float64)
+        rows = (base * np.exp2(ex)).astype(np.float32)
+        ref, _, call = split_case(metric, rows)
+        assert wrong_calls(ref, call()) == (0, 0), (lo, hi)
+
+
+@pytest.mark.parametrize("metric", METRICS)
+def test_rows_at_the_scale_threshold(metric):
+    """Rows whose largest element sits a few ulps above and below 127 FLT_MIN: above it the encoder stores a normal scale and
+    the rows go through the planes, below it they are left to stage 3. Once with the normal create_split draws over them
+    (products underflow) and once with a normal of ordinary magnitude."""
+    d, n = 768, 1200
+    rng = np.random.default_rng(3)
+    base = oracle.synth_rows(SEED, d, 0, n, 0.5).astype(np.float64)
+    base /= np.abs(base).max(axis=1, keepdims=True)
+    steps = rng.integers(-6, 7, size=n)
+    m = np.full(n, F32(127) * TINY, dtype=np.float32)      # exact: the threshold itself
+    for i, k in enumerate(steps):                            # k ulps from it
+        for _ in range(abs(int(k))):
+            m[i] = np.nextafter(m[i], F32(np.inf) if k > 0 else F32(0))
+    rows = (base * m[:, None].astype(np.float64)).astype(np.float32)
+    rows[np.arange(n), np.abs(base).argmax(axis=1)] = m * np.sign(base[np.arange(n), np.abs(base).argmax(axis=1)]).astype(np.float32)
+    _, _, s = encode(rows, d)
+    planes = (s >= TINY) & (s <= np.finfo(np.float32).max)
+    assert 0 < planes.sum() < n                    # both sides of the threshold occur
+    ordinary = (rng.standard_normal(d) / np.sqrt(d)).astype(np.float32)
+    for normal in (None, ordinary):
+        ref, _, call = split_case(metric, rows, normal)
+        c1, r1, c2, r2 = call()
+        assert wrong_calls(ref, (c1, r1, c2, r2)) == (0, 0)
+        assert not (c1 | c2)[~planes].any()       # the rows below the threshold are never certain
+        if normal is not None:
+            assert (c1 | c2)[planes].sum() > 0.5 * planes.sum()
