@@ -35,6 +35,8 @@ SIGNATURES = [
     ("arroy_b200_stage_stats", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_read_items", C.c_int32, [C.c_void_p, _u32p, C.c_uint64, C.c_void_p]),
     ("arroy_b200_stage_delta_plan", C.c_uint64, [_u32p, C.c_uint64, _u32p, C.c_uint64, _u32p, C.c_uint64, C.POINTER(C.c_int64)]),
+    ("arroy_b200_item_placement_plan", C.c_uint32, [C.c_int32, C.c_uint32, C.c_uint64, C.c_uint64]),
+    ("arroy_b200_item_placement", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_stage_items_flat", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.c_void_p, _f32p, _f32p]),
     ("arroy_b200_stage_items_device", C.c_int32, [C.c_void_p, C.c_int32, C.c_uint32, C.c_uint64, _u32p, C.c_void_p]),
     ("arroy_b200_item_headers", C.c_int32, [C.c_void_p, _f32p, _f32p]),
@@ -153,6 +155,13 @@ def stage_delta_plan(old_ids, new_ids, changed_ids):
     src = np.empty(new.size, dtype=np.int64)
     n = load().arroy_b200_stage_delta_plan(_up(old), old.size, _up(new), new.size, _up(ch), ch.size, src.ctypes.data_as(C.POINTER(C.c_int64)))
     return src, int(n)
+
+
+def item_placement_plan(metric, dim, n, free_bytes):
+    """Where stage_items_ptrs / stage_items_flat put an index's f32 rows given free_bytes of device memory (host only):
+    "device", or "host" (mapped pinned host memory; the device keeps the 8-bit planes)."""
+    metric = METRICS[metric] if isinstance(metric, str) else metric
+    return "host" if load().arroy_b200_item_placement_plan(metric, dim, n, free_bytes) == 1 else "device"
 
 
 class Context:
@@ -342,11 +351,21 @@ class Context:
         self._ck(self.lib.arroy_b200_stage_stats(self.h, out))
         return {"uploaded_rows": int(out[0]), "moved_rows": int(out[1]), "delta": int(out[2]), "h2d_bytes": int(out[3])}
 
+    def item_placement(self):
+        """Where the staged f32 rows live: {"placement": "device" | "host", "device_bytes": device bytes held for item data (the
+        rows, or the 8-bit planes and scales of host-placed rows), "host_bytes": pinned host bytes of the rows}."""
+        out = (C.c_uint64 * 3)()
+        self._ck(self.lib.arroy_b200_item_placement(self.h, out))
+        return {"placement": "host" if out[0] == 1 else "device", "device_bytes": int(out[1]), "host_bytes": int(out[2])}
+
     def read_items(self, rows=None):
         """The raw resident rows (all of them by default) as a uint8 array n_rows x row_bytes, padding included."""
         rows = np.arange(self.n, dtype=np.uint32) if rows is None else np.ascontiguousarray(rows, dtype=np.uint32)
-        _, ld = self.device_ptrs()
-        out = np.empty((rows.size, 4 * ld), dtype=np.uint8)
+        if self.metric is not None and self.metric >= BQ_EUCLIDEAN:
+            row_bytes = 16 * ((self.dim + 127) // 128)   # the bit string (arroy_b200_device_ptrs)
+        else:
+            row_bytes = 4 * ((self.dim + 31) // 32 * 32)
+        out = np.empty((rows.size, row_bytes), dtype=np.uint8)
         self._ck(self.lib.arroy_b200_read_items(self.h, _up(rows), rows.size, out.ctypes.data))
         return out
 

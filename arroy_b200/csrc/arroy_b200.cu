@@ -54,8 +54,36 @@ struct DevBuf {
         CK(cudaMalloc(&p, want));
         cap = want;
     }
+    // exactly `bytes` (no slack, nothing larger kept): for the planes of host-placed items, which are most of what such an index
+    // holds on the device
+    void ensure_exact(size_t bytes) {
+        if (bytes == cap) return;
+        release();
+        CK(cudaMalloc(&p, bytes));
+        cap = bytes;
+    }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() { return static_cast<T*>(p); }
+};
+// The f32 item matrix of a host-placed index: mapped pinned host memory, read by the kernels through its device address (UVA).
+// Allocated to size; a buffer more than twice the size asked for is given back rather than kept pinned.
+struct MappedBuf {
+    void* p = nullptr;
+    void* dev = nullptr;
+    size_t cap = 0;
+    void ensure(size_t bytes) {
+        if (bytes <= cap && cap / 2 <= bytes) return;
+        release();
+        const cudaError_t e = cudaHostAlloc(&p, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+        if (e != cudaSuccess) {
+            p = nullptr;
+            cudaGetLastError();
+            throw CudaError("cudaHostAlloc of " + std::to_string(bytes) + " bytes of pinned host memory for the item rows failed: " + cudaGetErrorString(e));
+        }
+        cap = bytes;
+        CK(cudaHostGetDevicePointer(&dev, p, 0));
+    }
+    void release() { if (p) cudaFreeHost(p); p = nullptr; dev = nullptr; cap = 0; }
 };
 struct PinBuf {
     void* p = nullptr;
@@ -88,6 +116,7 @@ struct BuiltTreeView {  // views into the pinned HostWave buffers of the context
 struct StageWorker {  // one H2D lane of the staging pipeline: own stream, two pinned bounce buffers
     cudaStream_t st = nullptr;
     PinBuf pin[2];
+    DevBuf dev[2];   // host placement: the device bounce buffers the chunk encoder reads
     cudaEvent_t ev[2] = {nullptr, nullptr};
 };
 struct HostWave {  // pinned host copies of one wave's results; kept across builds
@@ -111,6 +140,11 @@ struct arroy_ctx {
     uint32_t row_bytes = 0;     // bytes per item row: 4 ld, binary-quantized metrics: the bit string (kernels.cuh bq_row_u4)
     uint64_t n = 0;
     DevBuf items, h0, h1, norms, maxbits;
+    // host placement (arroy_b200_item_placement_plan): the f32 rows live in mapped pinned host memory, `items` is released and
+    // the 8-bit planes are written at staging time
+    bool host_items = false;
+    MappedBuf host_rows;
+    int32_t placed_metric = -1; uint32_t placed_dim = 0; uint64_t placed_n = 0;   // the last device-placed staging that asked
     std::vector<uint32_t> ids;
     // scratch
     DevBuf s_rows, s_flags, s_margins, s_normal, s_unit, s_job, s_keys, s_keys2, s_dists, s_q, s_qbits, s_qh0, s_off, s_orows, s_odist, s_olen, s_misc;
@@ -163,6 +197,7 @@ struct arroy_ctx {
     // tensor-core pre-filter of rerank_shared
     cublasHandle_t blas = nullptr;
     DevBuf x_gather, x_cnorm, x_ca, x_cb, x_gmax, x_qa, x_qb, x_twoe, x_qnorm, x_S, x_sel, x_beg, x_end, x_flag;
+    DevBuf x_gh0, x_iota;   // host placement: the gathered candidates' headers and their positions for the exact dense path
     uint64_t xf_calls = 0, xf_fallbacks = 0, xf_selected = 0, xf_queries = 0;
     cudaEvent_t xev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     double xbreak[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -186,6 +221,30 @@ void set_device(arroy_ctx* c) { CK(cudaSetDevice(c->device)); }
 
 void require_staged(arroy_ctx* c) { if (!c->staged) throw NotStaged("items have not been staged on this context"); }
 
+// The f32 item matrix as kernels address it: device memory, or for host-placed items the device address of the mapped host rows.
+// Kernels that read through it take ordinary loads; TMA and cp.async are only given device copies (xf_candidates).
+const float* items_f32(arroy_ctx* c) { return c->host_items ? static_cast<const float*>(c->host_rows.dev) : c->items.as<float>(); }
+
+// Indexes whose f32 rows may live in host memory: float metrics whose rows the 8-bit planes encode (kernels.cuh PLANES_MAX_D).
+bool host_placement_eligible(int metric, uint32_t dim) { return metric >= EUCLIDEAN && metric <= MANHATTAN && dim >= 64 && dim <= PLANES_MAX_D; }
+
+// Device bytes of a device-placed index and one tree of its build: f32 rows, both planes, scales, headers, and the wave buffers
+// do_build_begin sizes one tree with (split_after = dim).
+uint64_t device_placement_bytes(uint32_t dim, uint64_t n) {
+    const uint64_t ld = (dim + 31u) & ~31u;
+    const uint64_t leaves_est = n / std::max<uint32_t>(dim, 1) + 1;
+    const uint64_t per_tree = n * (4 + 4 + 1 + 4) + (n / SCAN_UNIT + 1) * 4 + sizeof(Frame) * (uint64_t)MAX_DEPTH + 16ull * 8 * leaves_est +
+                              4ull * (ld + NORMAL_HDR) * 4 * leaves_est + 4096;
+    return n * ld * 4 + 2 * n * ld + 4 * n + 8 * n + per_tree;
+}
+
+uint32_t placement_plan(int32_t metric, uint32_t dim, uint64_t n, uint64_t free_bytes) {
+    if (!host_placement_eligible(metric, dim)) return 0;
+    return (double)device_placement_bytes(dim, n) <= (double)free_bytes * 0.7 ? 0u : 1u;
+}
+
+bool host_items_forced() { const char* e = getenv("ARROY_B200_HOST_ITEMS"); return e != nullptr && atoi(e) == 1; }
+
 size_t work_smem(uint32_t ld, int njobs) { return (size_t)ld * 4 + (size_t)(njobs + 1) * 4 + 16; }
 
 // the scan kernel of the staged items: f32 rows, or bit-string rows for the binary-quantized metrics
@@ -197,7 +256,7 @@ void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
     // set on every launch: build_wave sets the same attribute to its own (possibly smaller) request, so a value remembered
     // here could be stale
     if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    work<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric);
+    work<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, items_f32(c), c->h0.as<float>(), c->dim, c->ld, c->metric);
     CK(cudaGetLastError());
     c->n_launches += 1;
 }
@@ -209,7 +268,7 @@ void compute_norms(arroy_ctx* c, bool with_max) {
     uint64_t warps = (c->n + 3) / 4;
     int grid = (int)std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16);
     if (grid < 1) grid = 1;
-    norms_kernel<<<grid, 256, 0, c->stream>>>(c->items.as<float>(), c->n, c->dim, c->ld, c->norms.as<float>(), with_max ? c->maxbits.as<uint32_t>() : nullptr);
+    norms_kernel<<<grid, 256, 0, c->stream>>>(items_f32(c), c->n, c->dim, c->ld, c->norms.as<float>(), with_max ? c->maxbits.as<uint32_t>() : nullptr);
     CK(cudaGetLastError());
     c->n_launches += 1;
 }
@@ -218,9 +277,29 @@ void compute_norms(arroy_ctx* c, bool with_max) {
 // context that was created at the address of a destroyed one.
 uint64_t next_stage_epoch() { static std::atomic<uint64_t> last{0}; return ++last; }
 
-void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint32_t* ids) {
+// Where the f32 rows of a staging go (may_host: the staging calls that can write host-placed rows, arroy_b200_stage_items and
+// _flat). The plan sees the free device memory plus what this context already holds for items, their derived copies and the wave
+// buffers, since the staging replaces or reuses all of it. A staging with the shapes of the last device-placed one that asked
+// takes its answer again: cudaMemGetInfo is a driver round trip of up to tens of milliseconds.
+bool choose_host_placement(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, bool may_host) {
+    if (!may_host || n == 0 || !host_placement_eligible(metric, dim)) return false;
+    if (host_items_forced()) return true;
+    if (c->placed_metric == metric && c->placed_dim == dim && c->placed_n == n) return false;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const Wave& W = c->wave;
+    const uint64_t held = c->items.cap + c->pl_hi.cap + c->pl_lo.cap + c->pl_scale.cap + c->fr_shadow.cap + c->fr_norm.cap + W.perm0.cap + W.perm1.cap +
+                          W.flags.cap + W.final_ids.cap + W.pool.cap + W.recs.cap;
+    if (placement_plan(metric, dim, n, (uint64_t)free_b + held) == 1) return true;
+    c->placed_metric = metric; c->placed_dim = dim; c->placed_n = n;
+    return false;
+}
+
+void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint32_t* ids, bool may_host = false) {
     if (metric < 0 || metric > BQ_MANHATTAN) throw ArgError("unknown metric");
     if (dim == 0) throw ArgError("dim must be > 0");
+    c->staged = false;
+    const bool host = choose_host_placement(c, metric, dim, n, may_host);
     c->user_dim = dim;
     if (is_bq(metric)) dim = (dim + 63u) / 64u * 64u;   // the bit string's length (binary_quantized.rs:80-92)
     if (n > 0xffffffffull) throw ArgError("too many items");
@@ -232,7 +311,18 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
     c->metric = metric; c->dim = dim; c->ld = (dim + 31u) & ~31u; c->n = n;
     c->row_bytes = is_bq(metric) ? 16u * bq_row_u4(dim) : 4u * c->ld;
     c->ids.assign(ids, ids + n);
-    c->items.ensure(std::max<size_t>(16, (size_t)n * c->row_bytes));
+    c->host_items = host;
+    if (host) {   // the device keeps the planes and scales (written by the staging), no f32 rows and no bf16 shadow
+        CK(cudaStreamSynchronize(c->stream));
+        c->items.release(); c->fr_shadow.release(); c->fr_norm.release();
+        c->host_rows.ensure((size_t)n * c->row_bytes);
+        c->pl_hi.ensure_exact((size_t)n * c->ld);
+        c->pl_lo.ensure_exact((size_t)n * c->ld);
+        c->pl_scale.ensure_exact((size_t)n * 4);
+    } else {
+        c->host_rows.release();
+        c->items.ensure(std::max<size_t>(16, (size_t)n * c->row_bytes));
+    }
     c->h0.ensure(std::max<size_t>(16, n * 4));
     c->h1.ensure(std::max<size_t>(16, n * 4));
     CK(cudaMemsetAsync(c->h0.p, 0, std::max<size_t>(16, n * 4), c->stream));
@@ -258,10 +348,13 @@ void default_headers(arroy_ctx* c) {
 // issuing its own cudaMemcpyAsync on its own stream, so decode (host memcpy of unaligned values)
 // and PCIe transfers of different chunks overlap. Rows of row_bytes bytes, zero padded.
 // mode 0: row_src(i) = dim f32 (byte aligned only); mode 1 (binary quantized): row_src(i) = src_dim f32 to be quantized to a
-// bit string (is_sign_positive); mode 2 (binary quantized): row_src(i) = the stored bit string (dim / 8 bytes), copied
+// bit string (is_sign_positive); mode 2 (binary quantized): row_src(i) = the stored bit string (dim / 8 bytes), copied.
+// Host placement (c->host_items, mode 0): the rows are decoded straight into the mapped host matrix, each chunk is copied into a
+// device bounce buffer of its lane and planes_encode_chunk_kernel writes its planes and scales there (and its norms into
+// `norms`, when given), on the lane's stream: the rows cross PCIe once and the planes are complete when the pipeline returns.
 template <class RowSrc>
 void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_bytes, RowSrc row_src, uint8_t* dst_override = nullptr, size_t chunk_mb_override = 0, bool count_bytes = true,
-                         int mode = 0, uint32_t src_dim = 0) {
+                         int mode = 0, uint32_t src_dim = 0, float* norms = nullptr) {
     if (n == 0) return;
     // 8 lanes x 4 MB chunks: decode of one chunk overlaps the PCIe copies of the others
     unsigned W = std::min(8u, std::max(1u, std::thread::hardware_concurrency()));
@@ -269,16 +362,22 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_by
     const uint64_t chunk_rows = std::max<uint64_t>(1, (chunk_mb << 20) / row_bytes);
     const uint64_t n_chunks = (n + chunk_rows - 1) / chunk_rows;
     W = (unsigned)std::min<uint64_t>(W, n_chunks);
+    const bool host = c->host_items && !dst_override;
     if (c->stage_workers.size() < W) c->stage_workers.resize(W);
     for (unsigned w = 0; w < W; ++w) {
         StageWorker& sw = c->stage_workers[w];
         if (!sw.st) CK(cudaStreamCreateWithFlags(&sw.st, cudaStreamNonBlocking));
-        for (int k = 0; k < 2; ++k) { sw.pin[k].ensure(chunk_rows * row_bytes); if (!sw.ev[k]) CK(cudaEventCreateWithFlags(&sw.ev[k], cudaEventDisableTiming)); }
+        for (int k = 0; k < 2; ++k) {
+            if (host) sw.dev[k].ensure(chunk_rows * row_bytes);
+            else sw.pin[k].ensure(chunk_rows * row_bytes);
+            if (!sw.ev[k]) CK(cudaEventCreateWithFlags(&sw.ev[k], cudaEventDisableTiming));
+        }
     }
     CK(cudaStreamSynchronize(c->stream));  // the destination buffer must not be in use
     std::mutex emu;
     std::string err;
-    uint8_t* dst = dst_override ? dst_override : c->items.as<uint8_t>();
+    uint8_t* dst = dst_override ? dst_override : host ? static_cast<uint8_t*>(c->host_rows.p) : c->items.as<uint8_t>();
+    const unsigned enc_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((chunk_rows + 31) / 32, (uint64_t)c->sm_count * 4));
     auto worker = [&](unsigned w) {
         try {
             CK(cudaSetDevice(c->device));
@@ -287,8 +386,8 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_by
             int k = 0;
             for (uint64_t ch = w; ch < n_chunks; ch += W, k ^= 1) {
                 const uint64_t r0 = ch * chunk_rows, rows = std::min<uint64_t>(chunk_rows, n - r0);
-                if (used[k]) CK(cudaEventSynchronize(sw.ev[k]));
-                uint8_t* b = sw.pin[k].as<uint8_t>();
+                if (used[k] && !host) CK(cudaEventSynchronize(sw.ev[k]));
+                uint8_t* b = host ? dst + r0 * row_bytes : sw.pin[k].as<uint8_t>();
                 for (uint64_t i = 0; i < rows; ++i) {
                     uint8_t* o = b + i * row_bytes;
                     const size_t used = mode == 0 ? 4ull * dim : dim / 8;
@@ -300,7 +399,12 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_by
                     } else memcpy(o, row_src(r0 + i), used);
                     memset(o + used, 0, row_bytes - used);
                 }
-                CK(cudaMemcpyAsync(dst + r0 * row_bytes, b, rows * row_bytes, cudaMemcpyHostToDevice, sw.st));
+                if (host) {   // (the bounce buffer's previous chunk was encoded by an earlier launch on this stream)
+                    CK(cudaMemcpyAsync(sw.dev[k].p, b, rows * row_bytes, cudaMemcpyHostToDevice, sw.st));
+                    planes_encode_chunk_kernel<<<enc_grid, 256, 0, sw.st>>>(sw.dev[k].as<float>(), rows, dim, c->ld, c->pl_hi.as<int8_t>() + r0 * c->ld,
+                                                                           c->pl_lo.as<int8_t>() + r0 * c->ld, c->pl_scale.as<float>() + r0, norms ? norms + r0 : nullptr);
+                    CK(cudaGetLastError());
+                } else CK(cudaMemcpyAsync(dst + r0 * row_bytes, b, rows * row_bytes, cudaMemcpyHostToDevice, sw.st));
                 CK(cudaEventRecord(sw.ev[k], sw.st));
                 used[k] = true;
             }
@@ -311,6 +415,7 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_by
     else { std::vector<std::thread> th; for (unsigned w = 0; w < W; ++w) th.emplace_back(worker, w); for (auto& x : th) x.join(); }
     if (!err.empty()) throw CudaError(err);
     if (count_bytes) c->h2d_bytes += n * (uint64_t)row_bytes;
+    if (host) { c->n_launches += n_chunks; c->planes_valid = true; }
 }
 
 // ---- RoaringBitmap::serialize_into (roaring 0.10.9, portable format, no run containers) ------
@@ -441,7 +546,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     if (spec) ws_bytes = (size_t)WS_VECS_SPEC * ld * 4;
 
     BuildParams P{};
-    P.items = c->items.as<float>(); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
+    P.items = items_f32(c); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
     P.n = (uint32_t)n; P.d = c->dim; P.ld = ld; P.metric = c->metric; P.K = K; P.n_trees = tw;
     P.st = W.st.as<TreeState>(); P.frames = W.frames.as<Frame>(); P.recs = W.recs.as<Record>(); P.rec_cap = rec_cap;
     P.perm[0] = W.perm0.as<uint32_t>(); P.perm[1] = W.perm1.as<uint32_t>();
@@ -510,7 +615,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     // Few trees on this GPU = the chain of attempts of each tree is the critical path: the async schedule runs the control kernel
     // as a thread-block cluster that scans small nodes itself (build.cuh control_kernel<.., CS = 8 | 16>).
     // measured: d = 64, 1-10 trees: 24 -> 20 us per attempt; d = 768: 38 -> 37 us for one tree but slower from ~6 trees on
-    const int cluster = (!lockstep && use_smem && c->dim <= 256 && !is_bq(c->metric)) ? (tw <= 8 ? 16 : (tw <= 16 ? 8 : 1)) : 1;
+    // (not for host-placed items: the cluster kernels scan their small nodes from the f32 rows)
+    const int cluster = (!lockstep && use_smem && c->dim <= 256 && !is_bq(c->metric) && !c->host_items) ? (tw <= 8 ? 16 : (tw <= 16 ? 8 : 1)) : 1;
     const void* ctrlc = control_fn(use_smem != 0, cluster, c->metric);
     if (cluster > 1) {
         CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
@@ -538,8 +644,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             if ((nb >= 2 || k == 1) && cap >= (int)tw + std::max(16, c->sm_count / 2)) { persist = true; pgrid = cap; psmem = cand[k]; if (k == 1) P.spec = 0; }
         }
     }
-    // scans through the 8-bit planes of the items (kernels.cuh scan_claim_planes): nodes of more than shadow_min_units units
-    if (!is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && n * (uint64_t)ld >= (1ull << 22)) {
+    // scans through the 8-bit planes of the items (kernels.cuh scan_claim_planes): nodes of more than shadow_min_units units.
+    // Host-placed items: every scan, so that only the rows the planes cannot decide are read over PCIe.
+    if (!is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && (n * (uint64_t)ld >= (1ull << 22) || c->host_items)) {
         planes_prepare(c);
         P.planes = PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()};
         W.shadow_stats.ensure(24);
@@ -547,7 +654,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         P.shadow_stats = W.shadow_stats.as<unsigned long long>();
         // many trees per GPU: bandwidth decides, every node goes through the shadow; few: the chain of attempts decides and
         // small nodes keep the one-unit claims of the exact scan (more CTAs per node)
-        P.shadow_min_units = (!persist || tw >= 32) ? 12u : (tw >= 12 ? 64u : 128u);
+        P.shadow_min_units = c->host_items ? 0u : (!persist || tw >= 32) ? 12u : (tw >= 12 ? 64u : 128u);
     }
     if (persist) {
         W.slots.ensure(sizeof(PSlot) * tw);
@@ -561,7 +668,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         // fused root scan: every tree of the wave starts at the root of the whole index (no subtree mode), rows go through the
         // 8-lanes-per-row path, and a batch of normals fits next to nothing else in the workers' shared memory (f32 rows only: the
         // bit-string rows of the binary-quantized metrics take the popcount scan, kernels.cuh bq_scan_unit)
-        P.root_fused = (!is_bq(c->metric) && !sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem) ? 1 : 0;
+        // (not for host-placed items: the pass streams every f32 row and prefetches them into L2 with bulk copies)
+        P.root_fused = (!is_bq(c->metric) && !sub.rows && tw >= 2 && P.d >= 32 && (size_t)ROOT_TB * ld * 4 <= psmem && !c->host_items) ? 1 : 0;
         W.root.ensure(8);
         CK(cudaMemsetAsync(W.root.p, 0, 8, c->stream));
         P.root_ready = W.root.as<uint32_t>(); P.root_ticket = W.root.as<uint32_t>() + 1;
@@ -957,13 +1065,13 @@ void do_side_batch(arroy_ctx* c, const float* normal, float h0, float h1, const 
 
 // ---- tensor-core pre-filter helpers (rerank_shared) ---------------------------------------------
 // candidate matrix for the score GEMM: the item matrix in place when `rows` is a contiguous range,
-// else a gathered copy
+// else a gathered copy. Host-placed items are always gathered: the GEMM reads its operands with TMA, which takes device memory.
 const float* xf_candidates(arroy_ctx* c, const uint32_t* rows, uint32_t nc) {
-    bool contiguous = true;
+    bool contiguous = !c->host_items;
     for (uint64_t i = 1; i < nc && contiguous; ++i) contiguous = rows[i] == rows[0] + i;
     if (contiguous) return c->items.as<float>() + (size_t)rows[0] * c->ld;
     c->x_gather.ensure(4ull * nc * c->ld);
-    xf_gather_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->x_gather.as<float4>(), c->items.as<float4>(), c->s_rows.as<uint32_t>(), nc, c->ld / 4);
+    xf_gather_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->x_gather.as<float4>(), reinterpret_cast<const float4*>(items_f32(c)), c->s_rows.as<uint32_t>(), nc, c->ld / 4);
     CK(cudaGetLastError());
     c->n_launches += 1;
     return c->x_gather.as<float>();
@@ -994,7 +1102,8 @@ int xf_engine() { const char* e = getenv("ARROY_B200_XGEMM"); return (e && strcm
 bool frerank_enabled(arroy_ctx* c, uint32_t k) {
     const char* e = getenv("ARROY_B200_FRERANK");
     const bool off = e != nullptr && atoi(e) == 0;
-    return !off && c->metric != MANHATTAN && !is_bq(c->metric) && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
+    // (host-placed items have no bf16 shadow: their re-rank takes the plain distance + top-k kernels)
+    return !off && c->metric != MANHATTAN && !is_bq(c->metric) && !c->host_items && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
 }
 
 // bf16 copy of the staged items (round to nearest even; padding stays zero) for the fused re-rank
@@ -1016,7 +1125,7 @@ void planes_prepare(arroy_ctx* c) {
     c->pl_lo.ensure(bytes);
     c->pl_scale.ensure(std::max<size_t>(16, (size_t)c->n * 4));
     const uint64_t blocks = std::max<uint64_t>(1, std::min<uint64_t>((c->n + 7) / 8, (uint64_t)c->sm_count * 16));
-    planes_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(c->items.as<float>(), c->n, c->ld, c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>());
+    planes_encode_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(items_f32(c), c->n, c->ld, c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>());
     CK(cudaGetLastError());
     c->n_launches += 1;
     c->planes_valid = true;
@@ -1148,7 +1257,7 @@ void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32
             bq_distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<uint4>(), c->h0.as<float>(), c->dim, c->metric, Q.bits, Q.h0, rows, beg, end,
                                                                   c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
         else
-            distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, c->ld, c->metric, Q.vecs, Q.rows, Q.h0, m,
+            distance_kernel<<<dim3(gx, m), 256, 0, c->stream>>>(items_f32(c), c->h0.as<float>(), c->dim, c->ld, c->metric, Q.vecs, Q.rows, Q.h0, m,
                                                                rows, beg, end, c->s_dists.as<float>(), c->s_keys.as<unsigned long long>());
         CK(cudaGetLastError());
     }
@@ -1304,12 +1413,14 @@ void arroy_b200_destroy(arroy_ctx* c) {
     DevBuf* bufs[] = {&c->items, &c->h0, &c->h1, &c->norms, &c->maxbits, &c->s_rows, &c->s_flags, &c->s_margins, &c->s_normal, &c->s_unit, &c->s_job,
                       &c->s_keys, &c->s_keys2, &c->s_dists, &c->s_q, &c->s_qh0, &c->s_off, &c->s_orows, &c->s_odist, &c->s_olen, &c->s_misc};
     for (auto* b : bufs) b->release();
-    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag}; for (auto* b : xb) b->release(); }
+    c->host_rows.release();
+    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag,
+                      &c->x_gh0, &c->x_iota}; for (auto* b : xb) b->release(); }
     if (c->blas) cublasDestroy(c->blas);
     for (auto& e : c->xev) if (e) cudaEventDestroy(e);
     if (c->cached_exec) cudaGraphExecDestroy(c->cached_exec);
     if (c->cached_graph) cudaGraphDestroy(c->cached_graph);
-    for (auto& sw : c->stage_workers) { sw.pin[0].release(); sw.pin[1].release(); if (sw.ev[0]) cudaEventDestroy(sw.ev[0]); if (sw.ev[1]) cudaEventDestroy(sw.ev[1]); if (sw.st) cudaStreamDestroy(sw.st); }
+    for (auto& sw : c->stage_workers) { sw.pin[0].release(); sw.pin[1].release(); sw.dev[0].release(); sw.dev[1].release(); if (sw.ev[0]) cudaEventDestroy(sw.ev[0]); if (sw.ev[1]) cudaEventDestroy(sw.ev[1]); if (sw.st) cudaStreamDestroy(sw.st); }
     { DevBuf* fb[] = {&c->f_kind, &c->f_left, &c->f_right, &c->f_nidx, &c->f_nh0, &c->f_doff, &c->f_dlen, &c->f_normals, &c->f_desc, &c->f_roots, &c->f_rec, &c->f_nofn,
                       &c->w_heaps, &c->w_cand, &c->w_cand2, &c->w_count, &c->w_bitmap, &c->w_status, &c->w_beg, &c->w_end, &c->w_qrows, &c->w_tmp, &c->w_pre};
       for (auto* b : fb) b->release(); }
@@ -1366,7 +1477,7 @@ void upload_headers(arroy_ctx* c, const std::vector<float>& h0, const std::vecto
 
 void stage_items_full(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values) {
     const uint64_t h2d0 = c->h2d_bytes;
-    alloc_items(c, metric, dim, n, ids);
+    alloc_items(c, metric, dim, n, ids, true);
     const int hf = metric_header_floats(metric);
     std::vector<float> h0, h1;
     decode_leaf_headers(leaf_values, n, hf, h0, h1);
@@ -1392,7 +1503,7 @@ void launch_restage(arroy_ctx* c, const RestagePiece* pieces, uint64_t n_pieces,
 // The delta path of arroy_b200_stage_items_delta; false = one of the conditions for it does not hold (nothing was changed).
 bool stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, const uint32_t* ids, const uint8_t* const* leaf_values, uint64_t n_changed,
                        const uint32_t* changed_ids) {
-    if (!c->staged || c->staging_open || n == 0 || c->n == 0) return false;
+    if (!c->staged || c->staging_open || n == 0 || c->n == 0 || c->host_items) return false;
     if (metric != c->metric || dim != c->user_dim) return false;   // row_bytes follows from the two
     if ((size_t)n * c->row_bytes > c->items.cap) return false;     // the resident buffer cannot hold the new matrix
     std::vector<int64_t> src(n);
@@ -1489,6 +1600,11 @@ int32_t arroy_b200_read_items(arroy_ctx* c, const uint32_t* rows, uint64_t n_row
         if (n_rows == 0) return;
         if (!rows || !out) throw ArgError("null argument");
         for (uint64_t i = 0; i < n_rows; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
+        if (c->host_items) {   // host-placed rows: read where they are
+            const uint8_t* src = static_cast<const uint8_t*>(c->host_rows.p);
+            for (uint64_t i = 0; i < n_rows; ++i) memcpy(out + i * c->row_bytes, src + (size_t)rows[i] * c->row_bytes, c->row_bytes);
+            return;
+        }
         for (uint64_t i = 0; i < n_rows;) {   // one copy per run of consecutive rows
             uint64_t e = i + 1;
             while (e < n_rows && rows[e] == rows[e - 1] + 1) ++e;
@@ -1503,6 +1619,20 @@ int32_t arroy_b200_read_items(arroy_ctx* c, const uint32_t* rows, uint64_t n_row
 uint64_t arroy_b200_stage_delta_plan(const uint32_t* old_ids, uint64_t n_old, const uint32_t* new_ids, uint64_t n_new, const uint32_t* changed_ids, uint64_t n_changed,
                                      int64_t* out_src) {
     return stage_delta_plan(old_ids, n_old, new_ids, n_new, changed_ids, n_changed, out_src);
+}
+
+uint32_t arroy_b200_item_placement_plan(int32_t metric, uint32_t dim, uint64_t n, uint64_t free_bytes) {
+    return placement_plan(metric, dim, n, free_bytes);
+}
+
+int32_t arroy_b200_item_placement(arroy_ctx* c, uint64_t out[3]) {
+    return guarded(c, [&] {
+        if (!out) throw ArgError("null argument");
+        require_staged(c);
+        out[0] = c->host_items ? 1 : 0;
+        out[1] = c->host_items ? c->pl_hi.cap + c->pl_lo.cap + c->pl_scale.cap : c->items.cap;
+        out[2] = c->host_items ? c->host_rows.cap : 0;
+    });
 }
 
 // ---- staging in pieces (multi-GPU: the H2D copy of chunk k + 1 overlaps the broadcast of chunk k) ---------------------------
@@ -1557,14 +1687,17 @@ int32_t arroy_b200_stage_items_flat(arroy_ctx* c, int32_t metric, uint32_t dim, 
     return guarded(c, [&] {
         set_device(c);
         if (n && (!ids || !vectors)) throw ArgError("null ids / vectors");
-        alloc_items(c, metric, dim, n, ids);
+        alloc_items(c, metric, dim, n, ids, true);
         if (n) {
             const uint8_t* base = reinterpret_cast<const uint8_t*>(vectors);
             const size_t stride = 4ull * dim;
+            // host placement: the Cosine default headers (the norms) come out of the chunk encoder, which reads every row anyway
+            const bool enc_norms = c->host_items && !hdr0 && metric == COSINE;
             // binary-quantized metrics: the f32 vectors are quantized on the way (Writer::add_item -> UnalignedVector::from_slice)
-            stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return base + i * stride; }, nullptr, 0, true, is_bq(metric) ? 1 : 0, dim);
+            stage_rows_pipeline(c, n, c->dim, c->row_bytes, [&](uint64_t i) { return base + i * stride; }, nullptr, 0, true, is_bq(metric) ? 1 : 0, dim,
+                                enc_norms ? c->h0.as<float>() : nullptr);
             if (hdr0) CK(cudaMemcpyAsync(c->h0.p, hdr0, n * 4, cudaMemcpyHostToDevice, c->stream));
-            else default_headers(c);
+            else if (!enc_norms) default_headers(c);
             if (hdr1) CK(cudaMemcpyAsync(c->h1.p, hdr1, n * 4, cudaMemcpyHostToDevice, c->stream));
         }
         CK(cudaStreamSynchronize(c->stream));
@@ -1635,8 +1768,13 @@ int32_t arroy_b200_side_multi(arroy_ctx* c, uint32_t n_jobs, const float* normal
         for (uint64_t i = 0; i < total; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
         if (total == 0) return;
         const uint32_t ld = c->ld, slot = ld + NORMAL_HDR;
-        // jobs per launch bounded by the shared-memory unit-prefix table of work_kernel
-        const uint32_t max_jobs = 40000;
+        // Host-placed items: every job goes through the 8-bit planes (work_kernel_shadow, no minimum size), so that only the rows
+        // the planes cannot decide are read over PCIe; the flags are the f32 scan's.
+        const bool planes = c->host_items;
+        if (planes) planes_prepare(c);
+        const size_t limb_smem = planes ? (size_t)PLANES_LIMBS * ld : 0;
+        // jobs per launch bounded by the shared-memory unit-prefix table of work_kernel (and next to the limbs of work_kernel_shadow)
+        const uint32_t max_jobs = planes ? (uint32_t)std::min<size_t>(40000, (160 * 1024 - 4ull * ld - limb_smem) / 4 - 1) : 40000;
         c->s_rows.ensure(4ull * total);
         c->s_flags.ensure(total);
         CK(cudaMemcpyAsync(c->s_rows.p, rows, 4ull * total, cudaMemcpyHostToDevice, c->stream));
@@ -1663,7 +1801,14 @@ int32_t arroy_b200_side_multi(arroy_ctx* c, uint32_t n_jobs, const float* normal
             CK(cudaMemcpyAsync(c->s_normal.p, slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
             CK(cudaMemcpyAsync(c->s_job.p, jobs.data(), sizeof(Job) * m, cudaMemcpyHostToDevice, c->stream));
             int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(units, (uint64_t)c->sm_count * 3));
-            launch_work(c, c->s_job.as<Job>(), (int)m, grid);
+            if (planes) {
+                const size_t smem = work_smem(ld, (int)m) + limb_smem;
+                if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                work_kernel_shadow<<<(unsigned)std::min<int>(grid, c->sm_count * 2), WORK_THREADS, smem, c->stream>>>(c->s_job.as<Job>(), (int)m, items_f32(c),
+                    PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}, c->h0.as<float>(), c->dim, ld, c->metric, 0u, nullptr);
+                CK(cudaGetLastError());
+                c->n_launches += 1;
+            } else launch_work(c, c->s_job.as<Job>(), (int)m, grid);
             CK(cudaStreamSynchronize(c->stream));   // slots / jobs host vectors are reused by the next chunk
         }
         CK(cudaMemcpyAsync(out_side, c->s_flags.p, total, cudaMemcpyDeviceToHost, c->stream));
@@ -1686,7 +1831,7 @@ int32_t arroy_b200_create_split(arroy_ctx* c, const uint32_t rng_key[8], uint64_
         CK(cudaMemcpyAsync(c->s_rows.p, rows, n_rows * 4, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(c->s_misc.p, rng_key, 32, cudaMemcpyHostToDevice, c->stream));
         BuildParams P{};
-        P.items = c->items.as<float>(); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
+        P.items = items_f32(c); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
         P.n = (uint32_t)c->n; P.d = c->dim; P.ld = ld; P.metric = c->metric;
         size_t ws_bytes = (size_t)WS_VECS * ld * 4;
         P.use_smem_ws = ws_bytes <= 200 * 1024;
@@ -1901,13 +2046,25 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
             if (!done) {
                 c->s_dists.ensure(4ull * m * nc);
                 mark.n = 0; mark();
+                // the kernel stages its operands with cp.async, which takes device memory: host-placed items are read from the
+                // gathered candidates (candidate i at row i, its header gathered alongside)
+                const float* x_items = c->items.as<float>();
+                const float* x_h0 = c->h0.as<float>();
+                const uint32_t* x_rows = c->s_rows.as<uint32_t>();
+                if (c->host_items) {
+                    if (!cand) cand = xf_candidates(c, rows, nc);
+                    c->x_gh0.ensure(4ull * nc); c->x_iota.ensure(4ull * nc);
+                    gather_f32_kernel<<<(nc + 255) / 256, 256, 0, c->stream>>>(c->x_gh0.as<float>(), c->h0.as<float>(), c->s_rows.as<uint32_t>(), nc);
+                    iota_u32_kernel<<<(unsigned)std::min<uint64_t>((nc + 255) / 256, (uint64_t)c->sm_count * 8), 256, 0, c->stream>>>(c->x_iota.as<uint32_t>(), nc);
+                    CK(cudaGetLastError());
+                    c->n_launches += 2;
+                    x_items = cand; x_h0 = c->x_gh0.as<float>(); x_rows = c->x_iota.as<uint32_t>();
+                }
                 dim3 grid((nc + XCB - 1) / XCB, (m + XQB - 1) / XQB);
                 if (c->metric == EUCLIDEAN)
-                    xrerank_kernel<true><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, Q.vecs, Q.h0, m,
-                                                                          c->s_rows.as<uint32_t>(), nc, c->s_dists.as<float>());
+                    xrerank_kernel<true><<<grid, XTHREADS, 0, c->stream>>>(x_items, x_h0, c->dim, ld, c->metric, Q.vecs, Q.h0, m, x_rows, nc, c->s_dists.as<float>());
                 else
-                    xrerank_kernel<false><<<grid, XTHREADS, 0, c->stream>>>(c->items.as<float>(), c->h0.as<float>(), c->dim, ld, c->metric, Q.vecs, Q.h0, m,
-                                                                           c->s_rows.as<uint32_t>(), nc, c->s_dists.as<float>());
+                    xrerank_kernel<false><<<grid, XTHREADS, 0, c->stream>>>(x_items, x_h0, c->dim, ld, c->metric, Q.vecs, Q.h0, m, x_rows, nc, c->s_dists.as<float>());
                 CK(cudaGetLastError());
                 topk_dense_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), nc, k, c->metric,
                                                                      c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
@@ -2105,7 +2262,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                     if (c->f_n_normals > 0 && m <= 4 && nbytes <= DOTS_MAX_BYTES && c->dim >= 32) {
                         c->w_pre.ensure(4ull * F.n_nodes * m);
                         const uint32_t gx = (uint32_t)std::min<uint64_t>(((uint64_t)c->f_n_normals + 7) / 8, (uint64_t)c->sm_count * 8);
-                        forest_dots_kernel<<<dim3(gx, m), 256, (size_t)ld * 4, c->stream>>>(F, c->f_n_normals, c->items.as<float>(), c->dim, ld, Q.rows, Q.vecs, c->w_pre.as<float>());
+                        forest_dots_kernel<<<dim3(gx, m), 256, (size_t)ld * 4, c->stream>>>(F, c->f_n_normals, items_f32(c), c->dim, ld, Q.rows, Q.vecs, c->w_pre.as<float>());
                         CK(cudaGetLastError());
                         c->n_launches += 1;
                         d_pre = c->w_pre.as<float>();
@@ -2121,7 +2278,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 }
                 const auto walk1 = multi ? &walk1_kernel<true, true> : filtered ? &walk1_kernel<true> : &walk1_kernel<false>;
                 const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
-                walk1<<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0, d_pre, c->f_n_normals, w1debug,
+                walk1<<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, items_f32(c), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0, d_pre, c->f_n_normals, w1debug,
                                                                  search_k, c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
                 CK(cudaGetLastError());
                 mark();
@@ -2170,7 +2327,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 WalkFilter Fl = Fl0;
                 if (multi) Fl.qfilter += q0;
                 const auto walk = multi ? &walk_kernel<true, true> : filtered ? &walk_kernel<true> : &walk_kernel<false>;
-                walk<<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, c->items.as<float>(), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0,
+                walk<<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, items_f32(c), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0,
                                                                                                         search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
                                                                                                         c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
                 CK(cudaGetLastError());
@@ -2471,7 +2628,7 @@ int32_t arroy_b200_time_scan(arroy_ctx* c, const float* normal, float hdr0, floa
         if (planes && psmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
         auto launch = [&] {
             if (!planes) { launch_work(c, c->s_job.as<Job>(), 1, grid); return; }
-            work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, psmem, c->stream>>>(c->s_job.as<Job>(), 1, c->items.as<float>(),
+            work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, psmem, c->stream>>>(c->s_job.as<Job>(), 1, items_f32(c),
                 PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}, c->h0.as<float>(), c->dim, c->ld, c->metric, 0u, pstats);
             CK(cudaGetLastError());
         };
@@ -2656,6 +2813,7 @@ int32_t arroy_b200_epochs(arroy_ctx* c, uint64_t out[2]) {
 int32_t arroy_b200_device_ptrs(arroy_ctx* c, void* out[3], uint32_t* out_ld) {
     return guarded(c, [&] {
         if (!c->staging_open) require_staged(c);
+        if (c->host_items) throw ArgError("device_ptrs: the item rows of this context are placed in host memory (arroy_b200_item_placement), not on the device");
         out[0] = c->items.p; out[1] = c->h0.p; out[2] = c->h1.p;
         if (out_ld) *out_ld = c->row_bytes / 4;
     });

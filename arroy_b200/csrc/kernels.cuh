@@ -228,6 +228,69 @@ __global__ void __launch_bounds__(256) planes_encode_kernel(const float* __restr
     }
 }
 
+// The encoder of host-placed items (arroy_b200.cu stage_rows_pipeline): the f32 rows live in mapped host memory, and each chunk
+// of them crosses PCIe once, into a device bounce buffer, where this kernel reads it. It writes the chunk's planes and scales
+// with planes_encode_kernel's arithmetic (the same bytes) and, when `norms` is given, sqrt(dot(v, v)) of every row in
+// norms_kernel's order (d >= 32: the caller only places rows of 64 <= d <= PLANES_MAX_D on the host). One 8-lane group per row,
+// four rows per warp; every lane runs every iteration, so the group shuffles see a full warp.
+__global__ void __launch_bounds__(256) planes_encode_chunk_kernel(const float* __restrict__ rows_f32, uint64_t n, uint32_t d, uint32_t ld,
+                                                                  int8_t* __restrict__ hi, int8_t* __restrict__ lo, float* __restrict__ scale,
+                                                                  float* __restrict__ norms) {
+    const unsigned full = 0xffffffffu;
+    const int lane = threadIdx.x & 31, g8 = lane & 7, grp = lane >> 3;
+    const uint32_t n4 = ld >> 2;   // a multiple of 8
+    const uint64_t nwarps = (uint64_t)gridDim.x * (blockDim.x >> 5);
+    for (uint64_t r0 = ((uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 4; r0 < n; r0 += nwarps * 4) {
+        const uint64_t r = r0 + grp;
+        const bool v = r < n;
+        const float4* row = reinterpret_cast<const float4*>(rows_f32 + (v ? r : 0) * ld);
+        uint32_t mb = 0;
+        for (uint32_t k = g8; k < n4; k += 8) {
+            const float4 x = row[k];
+            mb = max(max(mb, __float_as_uint(fabsf(x.x))), max(__float_as_uint(fabsf(x.y)), max(__float_as_uint(fabsf(x.z)), __float_as_uint(fabsf(x.w)))));
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) mb = max(mb, __shfl_xor_sync(full, mb, o));
+        const float M = __uint_as_float(mb);
+        float s = __fdiv_rn(M, 127.0f);
+        const bool ok = s >= 1.17549435e-38f && s <= 3.40282347e+38f;
+        if (!ok && mb != 0u && mb != 0x7f800000u) s = __int_as_float(0x7fffffff);
+        if (v) {
+            uint32_t* H = reinterpret_cast<uint32_t*>(hi + r * ld);
+            uint32_t* L = reinterpret_cast<uint32_t*>(lo + r * ld);
+            for (uint32_t k = g8; k < n4; k += 8) {
+                const float4 x4 = row[k];
+                const float x[4] = {x4.x, x4.y, x4.z, x4.w};
+                uint32_t hw = 0, lw = 0;
+                if (ok) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const float q = __fdiv_rn(x[j], s), h = rintf(q);
+                        const float l = rintf(__fmul_rn(__fsub_rn(q, h), 254.0f));
+                        hw |= ((uint32_t)(int)h & 0xffu) << (8 * j);
+                        lw |= ((uint32_t)(int)l & 0xffu) << (8 * j);
+                    }
+                }
+                H[k] = hw; L[k] = lw;
+            }
+            if (g8 == 0) scale[r] = s;
+        }
+        if (norms != nullptr) {   // (uniform over the grid)
+            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+            const int nch = d >> 5;
+#pragma unroll 4
+            for (int c = 0; c < nch; ++c) {
+                const float4 x = row[c * 8 + g8];
+                acc.x = fmaf(x.x, x.x, acc.x); acc.y = fmaf(x.y, x.y, acc.y); acc.z = fmaf(x.z, x.z, acc.z); acc.w = fmaf(x.w, x.w, acc.w);
+            }
+            float dt = group8_hsum(acc);
+            const float* rf = reinterpret_cast<const float*>(row);
+            for (uint32_t i = nch * 32; i < d; ++i) dt = __fadd_rn(dt, __fmul_rn(rf[i], rf[i]));
+            if (v && g8 == 0) norms[r] = __fsqrt_rn(dt);
+        }
+    }
+}
+
 __device__ __forceinline__ uint4 ldg_stream_u4(const uint4* p) {
     uint4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
@@ -412,7 +475,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         if (act && g8 == 0) { jb.flags[p] = (uint8_t)sa; if (sa == 0) atomicAdd(&sm_cnt[(p - base) / SCAN_UNIT], 1u); }
     }
     __syncthreads();
-    if (tid < (int)(u1 - u0)) jb.unit_left[u0 + tid] = sm_cnt[tid];
+    if (jb.unit_left != nullptr && tid < (int)(u1 - u0)) jb.unit_left[u0 + tid] = sm_cnt[tid];   // (side_multi's jobs count nothing)
 }
 
 __device__ __forceinline__ double warp_sum_f64(double v) {

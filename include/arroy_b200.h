@@ -75,9 +75,28 @@ const char* arroy_b200_version(void);
  * (src/node.rs:224-228, src/unaligned_vector/f32.rs). The library decodes the unaligned
  * bytes into pinned host memory and uploads them once into float[n][ld] (ld = dim
  * rounded up to 32 floats, zero padded) plus header arrays; binary-quantized values are
- * bit strings and stay bit strings on the device (arroy_b200_device_ptrs). */
+ * bit strings and stay bit strings on the device (arroy_b200_device_ptrs).
+ * Placement: this call and arroy_b200_stage_items_flat let arroy_b200_item_placement_plan decide, with cudaMemGetInfo's free
+ * bytes plus the bytes the context already holds for items, their planes, the bf16 shadow and the wave buffers (a staging with
+ * the metric, dim and n of the last device-placed one that asked takes its answer again). Host placement keeps float[n][ld] in
+ * library-owned mapped pinned host memory: the rows are decoded straight into it and cross PCIe once, in chunks, to a device
+ * bounce buffer where the build's 8-bit planes and scales (and, for _flat's Cosine default headers, the norms) are written; the
+ * device then holds 2 ld + 4 bytes per item plus headers, and no f32 rows. Builds scan through the planes and read the f32 rows
+ * they cannot decide from host memory; queries and re-ranks read host rows too. Results are identical either way. A failed
+ * pinned allocation is ARROY_B200_ERR_CUDA and leaves nothing staged. ARROY_B200_HOST_ITEMS=1 forces host placement for
+ * eligible indexes (tests and measurements). */
 int32_t arroy_b200_stage_items(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
                                const uint32_t* ids_ascending, const uint8_t* const* leaf_values);
+
+/* Where arroy_b200_stage_items / _flat put the f32 rows (host only, no device): 0 = device memory, 1 = mapped pinned host
+ * memory. Device when the f32 rows, both 8-bit planes, the scales, the headers and the wave buffers of one tree (split_after =
+ * dim) fit in 0.7 x free_bytes, the factor the build's wave sizing uses. Otherwise host, but only for a float metric (0-3) with
+ * 64 <= dim <= 8192 (the planes' range); every other index is placed on the device, and fails there as before if it does not
+ * fit. Monotone in free_bytes. */
+uint32_t arroy_b200_item_placement_plan(int32_t metric, uint32_t dim, uint64_t n, uint64_t free_bytes);
+/* The placement of the staged items: out[0] = 0 device / 1 host, out[1] = device bytes held for item data (the f32 rows, or for
+ * host placement the planes and scales), out[2] = pinned host bytes of the f32 rows (0 on the device). */
+int32_t arroy_b200_item_placement(arroy_ctx* ctx, uint64_t out[3]);
 
 /* The same staging for a caller that knows which items it has written since the resident ones were staged: same arguments and
  * the same postcondition as arroy_b200_stage_items (the context holds exactly the n items given, row = rank of the id, headers
@@ -89,6 +108,7 @@ int32_t arroy_b200_stage_items(arroy_ctx* ctx, int32_t metric, uint32_t dim, uin
  * Headers are small and DotProduct::preprocess rewrites all of them, so h0 / h1 of all n leaf values are read and uploaded.
  * The library stages in full, exactly as arroy_b200_stage_items, when one of these holds (arroy_b200_stage_stats tells):
  *   - nothing is staged, or a staging is open (arroy_b200_stage_begin without _end), or n or the resident count is 0;
+ *   - the resident items are placed in host memory (arroy_b200_item_placement);
  *   - metric or dim differ from the resident ones (the row size follows from the two);
  *   - n rows do not fit the capacity of the resident buffer (it is allocated with 25 % of slack, so repeated small appends
  *     stay in place);
@@ -130,7 +150,8 @@ int32_t arroy_b200_stage_items_flat(arroy_ctx* ctx, int32_t metric, uint32_t dim
 /* Same, but the matrix already lives in device memory of ctx's device (n x dim f32,
  * row-major, dense). Used by the multi-GPU path after the NCCL broadcast and by
  * benchmarks whose inputs are resident in HBM. The data is copied into the library's
- * padded layout (device to device). */
+ * padded layout (device to device). Always places the items on the device, as do
+ * arroy_b200_stage_begin / _rows / _end and the group API. */
 int32_t arroy_b200_stage_items_device(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
                                       const uint32_t* ids_ascending, const void* device_vectors);
 
@@ -157,7 +178,8 @@ int32_t arroy_b200_side_batch(arroy_ctx* ctx, const float* normal, float hdr0, f
 
 /* Many side() loops in one launch (level-batched routing of new items down existing trees,
  * src/writer.rs:1398-1459): job j tests rows[row_offsets[j] .. row_offsets[j+1]) against
- * normals[j] (dim floats) with header hdr0[j] (bias / extra_dim). out_side has the layout of rows. */
+ * normals[j] (dim floats) with header hdr0[j] (bias / extra_dim). out_side has the layout of rows. Items placed in host memory
+ * are tested through the build's 8-bit planes first (the same sides; only undecided rows read the f32 row). */
 int32_t arroy_b200_side_multi(arroy_ctx* ctx, uint32_t n_jobs, const float* normals, const float* hdr0, const float* hdr1,
                               const uint32_t* rows, const uint64_t* row_offsets, uint8_t* out_side);
 
@@ -433,7 +455,8 @@ int32_t arroy_b200_epochs(arroy_ctx* ctx, uint64_t out[2]);
 
 /* Raw device pointers of the staged items (for the NCCL broadcast of the multi-GPU path):
  * out[0] = float[n][ld] matrix, out[1] = hdr0[n], out[2] = hdr1[n] (may be 0); *out_ld = ld. Binary-quantized metrics: the
- * rows are bit strings of 16 * ceil(dims / 128) bytes and *out_ld is that byte count / 4. */
+ * rows are bit strings of 16 * ceil(dims / 128) bytes and *out_ld is that byte count / 4. Items placed in host memory
+ * (arroy_b200_item_placement) have no device matrix: ARROY_B200_ERR_INVALID. */
 int32_t arroy_b200_device_ptrs(arroy_ctx* ctx, void* out[3], uint32_t* out_ld);
 
 /* ---- several GPUs of one node behind one handle (SURVEY.md §8b / §8e) -------------------------------------------------
