@@ -971,6 +971,7 @@ __device__ __noinline__ void proot(const BuildParams& P, float* smN) {
 // Returns when every tree is done (or on error). sm_normal: ld floats of dynamic shared memory.
 // BQ: the items are bit-string rows, the loaded normal's first words of sm_normal hold its bit string and the scans are
 // bq_scan_unit's (no fused root pass, no pre-filter planes).
+static_assert(sizeof(PlanesClaimRows) <= (WS_VECS - 2) * 4 * 64, "pworker: the claim rows fit behind the normal and its limbs at ld = 64");
 template <bool BQ>
 __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ uint32_t w_t, w_u0, w_n, w_seq, w_pseq, w_found, w_exit, w_count;
@@ -981,6 +982,10 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ PlanesScratch w_sc;
     __shared__ PlanesNormal w_pn;                           // the loaded normal's pre-filter factors (scan_claim_planes)
     uint8_t* sm_limbs = reinterpret_cast<uint8_t*>(sm_normal + P.ld);   // and its limbs
+    // the claim's row ids, scales and headers (scan_claim_planes), after the limbs: the workspace this kernel is launched with
+    // (at least WS_VECS * ld floats) holds 2 ld floats + 3 KB whenever the planes are used (ld >= 64); kept out of static
+    // shared memory, which every control CTA pays for next to its two_means workspace
+    PlanesClaimRows& w_cr = *reinterpret_cast<PlanesClaimRows*>(sm_normal + 2u * P.ld);
     const uint32_t T = P.n_trees;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t rot = (blockIdx.x - T) * 7u;
@@ -1106,7 +1111,7 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
                     if (P.planes.hi != nullptr && units > P.shadow_min_units)
                         for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
                             scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_limbs,
-                                              &w_pn, nh0, w_list, w_list2, w_cnt, P.shadow_stats);
+                                              &w_pn, nh0, w_list, w_list2, w_cnt, w_cr, P.shadow_stats);
                     else
                         for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
                 }

@@ -326,28 +326,56 @@ __device__ __forceinline__ double prefilter_c(int metric, float nh0, float item_
     return (double)nh0;
 }
 
+// Starts `bytes` (a multiple of 16) at p, 16-byte aligned, on their way from HBM into L2; takes no register for the data.
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
+    // (no "memory" clobber: it writes nothing the program reads, so no load or store has to stay on either side of it)
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(__cvta_generic_to_global(p)), "r"(bytes));
+}
+
+// What scan_claim_planes needs of each row of its claim, fetched once in its prologue (position base + i at index i; zeros past
+// the claim's end).
+constexpr uint32_t PLANES_CLAIM_ROWS = SCAN_UNIT * PLANES_CHUNK;
+struct PlanesClaimRows {
+    uint32_t rid[PLANES_CLAIM_ROWS];   // row ids
+    float scale[PLANES_CLAIM_ROWS];    // the rows' plane scales
+    float ih0[PLANES_CLAIM_ROWS];      // DotProduct: the rows' h0 (the other metrics: unused)
+};
+
 // scan units [u0, u1) (at most PLANES_CHUNK) of a job. sm_list, sm_list2: 64 * PLANES_CHUNK positions each (the rows stage 1,
 // stage 2 left); sm_cnt: PLANES_CHUNK + 2 counters. limbs, pn: the job's normal as planes_job_factors left it. stats (optional):
 // [0] rows through the pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
+// Every read of a plane row is a device read (the planes never live in host memory), so their L2 prefetches are safe.
 __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, uint32_t u1, const float* __restrict__ items, const PlaneRows pl,
                                                   const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric, const float* sm_normal, const uint8_t* limbs,
-                                                  const PlanesNormal* pn, float nh0, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt, unsigned long long* stats) {
+                                                  const PlanesNormal* pn, float nh0, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt,
+                                                  PlanesClaimRows& cr, unsigned long long* stats) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
-    if (tid <= (int)PLANES_CHUNK + 1) sm_cnt[tid] = 0;
-    __syncthreads();
     const uint32_t base = u0 * SCAN_UNIT, end = min(jb.len, u1 * SCAN_UNIT);
+    // ---- prologue: one round for the claim's row ids, one for their scales (and headers); the hi rows of the first 128
+    // positions start towards L2 as soon as their ids are known ----
+    if (tid <= (int)PLANES_CHUNK + 1) sm_cnt[tid] = 0;
+    for (uint32_t i = tid; i < PLANES_CLAIM_ROWS; i += blockDim.x) {
+        const bool v = base + i < end;
+        const uint32_t r = v ? (jb.rows ? __ldcg(jb.rows + base + i) : base + i) : 0u;
+        if (v && i < 128u) prefetch_l2(pl.hi + (size_t)r * ld, ld);
+        cr.rid[i] = r;
+        cr.scale[i] = v ? __ldg(pl.scale + r) : 0.f;
+        cr.ih0[i] = (v && metric == DOT_PRODUCT) ? ih0[r] : 0.f;
+    }
+    __syncthreads();
     const uint32_t nq = ld >> 4;                       // 16-byte words per plane row
     const int nsteps = (int)((nq + 7) >> 3);
     const uint4* LA = reinterpret_cast<const uint4*>(limbs);
     const uint4* LB = LA + nq;
-    // ---- stage 1: the hi plane of every row ----
+    // ---- stage 1: the hi plane of every row; the next block's hi rows are prefetched into L2 while this block's are read ----
     for (uint32_t pbase = base; pbase < end; pbase += 128) {
+        if (tid < 128 && pbase + 128u + tid < end) prefetch_l2(pl.hi + (size_t)cr.rid[pbase + 128u - base + tid] * ld, ld);
         uint32_t pos[4], rid[4];
         const uint4* S[4];
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
             pos[r] = pbase + warp * 16 + grp * 4 + r;
-            rid[r] = pos[r] < end ? (jb.rows ? __ldcg(jb.rows + pos[r]) : pos[r]) : 0u;
+            rid[r] = cr.rid[pos[r] - base];
             S[r] = reinterpret_cast<const uint4*>(pl.hi + (size_t)rid[r] * ld) + g8;
         }
         int sa[4], sb[4];
@@ -376,14 +404,17 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
 #pragma unroll
             for (int o = 1; o < 8; o <<= 1) { sa[r] += __shfl_xor_sync(0xffffffffu, sa[r], o); sb[r] += __shfl_xor_sync(0xffffffffu, sb[r], o); }
             const bool valid = pos[r] < end;
-            const float s = valid ? __ldg(pl.scale + rid[r]) : 0.f;
+            const float s = cr.scale[pos[r] - base];
             const double t1 = (double)(254ll * sa[r] + sb[r]);
-            const double mt = __dadd_rn(__dmul_rn(__dmul_rn(t1, (double)s), k1), prefilter_c(metric, nh0, (metric == DOT_PRODUCT && valid) ? ih0[rid[r]] : 0.f));
+            const double mt = __dadd_rn(__dmul_rn(__dmul_rn(t1, (double)s), k1), prefilter_c(metric, nh0, cr.ih0[pos[r] - base]));
             const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, w1), wa);      // false for NaN / Inf scales and NaN factors
             const bool leader = g8 == 0 && valid;
             const int side = mt > 0.0 ? 1 : 0;
             if (leader && certain) jb.flags[pos[r]] = (uint8_t)side;
-            if (leader && !certain) sm_list[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = pos[r];
+            if (leader && !certain) {   // stage 2 reads this row's lo plane from L2
+                sm_list[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = pos[r];
+                prefetch_l2(pl.lo + (size_t)rid[r] * ld, ld);
+            }
             const unsigned lefts = __ballot_sync(0xffffffffu, leader && certain && side == 0);
             // the four groups of a warp hold positions of the same unit (16 consecutive positions per warp)
             if (lane == 0 && lefts) atomicAdd(&sm_cnt[(pbase + warp * 16 - base) / SCAN_UNIT], (uint32_t)__popc(lefts));
@@ -398,7 +429,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
         const bool act = idx < n1;
         const uint32_t p = act ? sm_list[idx] : base;
-        const uint32_t r = jb.rows ? __ldcg(jb.rows + p) : p;
+        const uint32_t r = cr.rid[p - base];
         const uint4* Hr = reinterpret_cast<const uint4*>(pl.hi + (size_t)r * ld) + g8;
         const uint4* Lr = reinterpret_cast<const uint4*>(pl.lo + (size_t)r * ld) + g8;
         int ha = 0, hb = 0, hc = 0, la = 0, lb = 0, lc = 0;
@@ -427,8 +458,8 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         double a = (double)(254ull * hu + lu);
 #pragma unroll
         for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
-        const float s = __ldg(pl.scale + r);
-        const double mt = __dadd_rn(__dmul_rn(__dmul_rn(m, (double)s), pn->k2), prefilter_c(metric, nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f));
+        const float s = cr.scale[p - base];
+        const double mt = __dadd_rn(__dmul_rn(__dmul_rn(m, (double)s), pn->k2), prefilter_c(metric, nh0, cr.ih0[p - base]));
         const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, __dadd_rn(pn->w2, __dmul_rn(pn->rel2, a))), pn->wa);
         const int side = mt > 0.0 ? 1 : 0;
         if (act && g8 == 0) {
@@ -450,7 +481,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
         const bool act = idx < nl;
         const uint32_t p = act ? sm_list2[idx] : base;
-        const uint32_t r = jb.rows ? __ldcg(jb.rows + p) : p;
+        const uint32_t r = cr.rid[p - base];
         const float4* A = reinterpret_cast<const float4*>(items + (size_t)r * ld);
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         int c = 0;
@@ -471,7 +502,7 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
         float da = group8_hsum(acc);
         const float* row = items + (size_t)r * ld;
         for (uint32_t i = (uint32_t)nch * 32u; i < d; ++i) da = __fadd_rn(da, __fmul_rn(row[i], sm_normal[i]));
-        const int sa = side_of(margin_finish(metric, da, nh0, (metric == DOT_PRODUCT) ? ih0[r] : 0.f));
+        const int sa = side_of(margin_finish(metric, da, nh0, cr.ih0[p - base]));
         if (act && g8 == 0) { jb.flags[p] = (uint8_t)sa; if (sa == 0) atomicAdd(&sm_cnt[(p - base) / SCAN_UNIT], 1u); }
     }
     __syncthreads();
@@ -680,6 +711,7 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
     __shared__ uint32_t sm_w[16];
     __shared__ uint32_t sm_list[SCAN_UNIT * PLANES_CHUNK], sm_list2[SCAN_UNIT * PLANES_CHUNK];
     __shared__ uint32_t sm_cnt[PLANES_CHUNK + 2];
+    __shared__ PlanesClaimRows sm_cr;
     __shared__ PlanesScratch sm_sc;
     __shared__ PlanesNormal sm_pn;
     auto via_shadow = [&](const Job& jb) { return jb.kind == JOB_SCAN && jb.margins == nullptr && (jb.len + SCAN_UNIT - 1) / SCAN_UNIT > min_units; };
@@ -732,7 +764,7 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
             if (via_shadow(jb)) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
                 scan_claim_planes(jb, item * PLANES_CHUNK, min(units, (item + 1u) * PLANES_CHUNK), items, planes, ih0, d, ld, metric, sm_normal, sm_limbs, &sm_pn, nh0,
-                                  sm_list, sm_list2, sm_cnt, stats);
+                                  sm_list, sm_list2, sm_cnt, sm_cr, stats);
             } else scan_unit<true>(jb, item, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
         } else {
             partition_block(jb.rows, jb.flags, jb.dst, item * PART_UNIT, jb.len, jb.unit_left[item * (PART_UNIT / SCAN_UNIT)], jb.total_left, sm_w);
