@@ -71,6 +71,7 @@ SIGNATURES = [
     ("arroy_b200_arena_get", C.c_int32, [C.c_void_p, C.c_uint32, C.POINTER(_u8p), _u64p]),
     ("arroy_b200_build_breakdown", C.c_int32, [C.c_void_p, C.POINTER(C.c_double)]),
     ("arroy_b200_counters", C.c_int32, [C.c_void_p, _u64p]),
+    ("arroy_b200_plane_rerank_stats", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_rerank_stats", C.c_int32, [C.c_void_p, _u64p]),
     ("arroy_b200_rerank_breakdown", C.c_int32, [C.c_void_p, C.POINTER(C.c_double)]),
     ("arroy_b200_search_breakdown", C.c_int32, [C.c_void_p, C.POINTER(C.c_double)]),
@@ -534,6 +535,12 @@ class Context:
         out = (C.c_uint64 * 4)()
         self._ck(self.lib.arroy_b200_counters(self.h, out))
         return {"launches": out[0], "h2d_bytes": out[1], "d2h_bytes": out[2], "fused_rerank_batches": out[3] >> 32, "fused_rerank_fallbacks": out[3] & 0xffffffff}
+
+    def plane_rerank_stats(self):
+        """The plane pre-filter of host-placed indexes' batched re-ranks, since create (arroy_b200_plane_rerank_stats)."""
+        out = (C.c_uint64 * 4)()
+        self._ck(self.lib.arroy_b200_plane_rerank_stats(self.h, out))
+        return {"batches": out[0], "fallbacks": out[1], "rows_estimated": out[2], "rows_rescored": out[3]}
 
     def prefilter_scores(self, queries, rows, engine=0):
         queries = np.ascontiguousarray(queries, dtype=np.float32)

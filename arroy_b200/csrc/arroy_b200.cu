@@ -210,6 +210,10 @@ struct arroy_ctx {
     // first build after staging
     DevBuf pl_hi, pl_lo, pl_scale;
     bool planes_valid = false;
+    // the plane pre-filter of host-placed items' re-rank (frerank_kernel<FR_PLANES>): device counters of candidates estimated
+    // and survivors re-scored, allocated by the first such batch; batches and fallbacks since create
+    DevBuf pr_counts;
+    uint64_t pr_batches = 0, pr_fallbacks = 0;
     uint64_t fr_batches = 0, fr_fallbacks = 0;   // last search_batch call, ms: bitmap clear + tree walk, candidate sort, distances, top-k   // last rerank_shared call, ms: prep, score GEMM, select, re-score, top-k, exact dense path
 };
 
@@ -1102,7 +1106,7 @@ int xf_engine() { const char* e = getenv("ARROY_B200_XGEMM"); return (e && strcm
 bool frerank_enabled(arroy_ctx* c, uint32_t k) {
     const char* e = getenv("ARROY_B200_FRERANK");
     const bool off = e != nullptr && atoi(e) == 0;
-    // (host-placed items have no bf16 shadow: their re-rank takes the plain distance + top-k kernels)
+    // (host-placed items have no bf16 shadow: their re-rank takes plane_rerank_enabled's kernel)
     return !off && c->metric != MANHATTAN && !is_bq(c->metric) && !c->host_items && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
 }
 
@@ -1160,17 +1164,49 @@ void frerank_launch(arroy_ctx* c, uint32_t m, const float* d_q, const uint32_t* 
     P.out_rows = c->s_orows.as<uint32_t>(); P.out_dist = c->s_odist.as<float>(); P.out_len = c->s_olen.as<uint32_t>(); P.status = c->fr_status.as<int32_t>();
     const size_t smem = frerank_smem(c->ld);
     static std::atomic<size_t> configured{0};
-    if (smem > 48 * 1024 && smem > configured.load()) { CK(cudaFuncSetAttribute(frerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured = smem; }
-    frerank_kernel<<<m, FR_THREADS, smem, c->stream>>>(P);
+    if (smem > 48 * 1024 && smem > configured.load()) { CK(cudaFuncSetAttribute(frerank_kernel<FR_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured = smem; }
+    frerank_kernel<FR_BF16><<<m, FR_THREADS, smem, c->stream>>>(P);
     CK(cudaGetLastError());
     c->n_launches += 1;
     c->fr_batches += 1;
 }
 
-bool frerank_ok(arroy_ctx* c, uint32_t m) {   // after the stream is idle: did every query finish in the fused kernel?
+// Host-placed items: the same per-query kernel with estimates from the build's 8-bit planes (frerank.cuh, FR_PLANES). It reads
+// the planes, scales and headers on the device and only the survivors' rows from host memory; it needs nothing prepared.
+bool plane_rerank_enabled(arroy_ctx* c, uint32_t k) {
+    const char* e = getenv("ARROY_B200_FRERANK");
+    const bool off = e != nullptr && atoi(e) == 0;
+    return !off && c->host_items && c->planes_valid && !is_bq(c->metric) && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
+}
+
+void plane_rerank_launch(arroy_ctx* c, uint32_t m, const float* d_q, const uint32_t* d_qrows, const float* d_qh0, const uint32_t* d_rows,
+                         const uint64_t* d_beg, const uint64_t* d_end, uint32_t k) {
+    c->fr_status.ensure(4ull * m);
+    if (!c->pr_counts.p) { c->pr_counts.ensure(16); CK(cudaMemsetAsync(c->pr_counts.p, 0, 16, c->stream)); }
+    FrParams P{};
+    P.items = items_f32(c); P.ih0 = c->h0.as<float>();
+    P.d = c->dim; P.ld = c->ld; P.metric = c->metric;
+    P.queries = d_q; P.qrows = d_qrows; P.qh0 = d_qh0;
+    P.rows = d_rows; P.seg_beg = d_beg; P.seg_end = d_end;
+    P.k = k; P.hmin = cos_header_min(c->dim);
+    P.out_rows = c->s_orows.as<uint32_t>(); P.out_dist = c->s_odist.as<float>(); P.out_len = c->s_olen.as<uint32_t>(); P.status = c->fr_status.as<int32_t>();
+    P.hi = c->pl_hi.as<int8_t>(); P.lo = c->pl_lo.as<int8_t>(); P.scale = c->pl_scale.as<float>();
+    fr_plane_consts(c->metric, c->dim, P);
+    P.counts = c->pr_counts.as<unsigned long long>();
+    const size_t smem = frerank_smem(c->ld);
+    static std::atomic<size_t> configured{0};
+    if (smem > 48 * 1024 && smem > configured.load()) { CK(cudaFuncSetAttribute(frerank_kernel<FR_PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured = smem; }
+    frerank_kernel<FR_PLANES><<<m, FR_THREADS, smem, c->stream>>>(P);
+    CK(cudaGetLastError());
+    c->n_launches += 1;
+    c->pr_batches += 1;
+}
+
+// after the stream is idle: did every query finish in the fused kernel? (counts a fallback batch in `fallbacks`)
+bool frerank_ok(arroy_ctx* c, uint32_t m, uint64_t& fallbacks) {
     std::vector<int32_t> st(m);
     CK(cudaMemcpy(st.data(), c->fr_status.p, 4ull * m, cudaMemcpyDeviceToHost));
-    for (int32_t x : st) if (x != 0) { c->fr_fallbacks += 1; return false; }
+    for (int32_t x : st) if (x != 0) { fallbacks += 1; return false; }
     return true;
 }
 
@@ -1246,7 +1282,11 @@ void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32
     if (try_fused && frerank_enabled(c, k)) {   // one fused kernel per query: bf16 pre-filter + exact re-score + top-k (frerank.cuh)
         frerank_launch(c, m, Q.vecs, Q.rows, Q.h0, rows, beg, end, k);
         CK(cudaStreamSynchronize(c->stream));
-        if (frerank_ok(c, m)) { if (mark) (*mark)(); return; }
+        if (frerank_ok(c, m, c->fr_fallbacks)) { if (mark) (*mark)(); return; }
+    } else if (try_fused && plane_rerank_enabled(c, k)) {   // host-placed items: the same kernel on the 8-bit planes
+        plane_rerank_launch(c, m, Q.vecs, Q.rows, Q.h0, rows, beg, end, k);
+        CK(cudaStreamSynchronize(c->stream));
+        if (frerank_ok(c, m, c->pr_fallbacks)) { if (mark) (*mark)(); return; }
     }
     if (max_len) {
         // (Manhattan sums one row per lane, the bit-string rows take four lanes per row, the other metrics eight)
@@ -1414,7 +1454,7 @@ void arroy_b200_destroy(arroy_ctx* c) {
                       &c->s_keys, &c->s_keys2, &c->s_dists, &c->s_q, &c->s_qh0, &c->s_off, &c->s_orows, &c->s_odist, &c->s_olen, &c->s_misc};
     for (auto* b : bufs) b->release();
     c->host_rows.release();
-    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag,
+    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->pr_counts, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag,
                       &c->x_gh0, &c->x_iota}; for (auto* b : xb) b->release(); }
     if (c->blas) cublasDestroy(c->blas);
     for (auto& e : c->xev) if (e) cudaEventDestroy(e);
@@ -2700,6 +2740,19 @@ int32_t arroy_b200_build_breakdown(arroy_ctx* c, double out[8]) {
 
 int32_t arroy_b200_counters(arroy_ctx* c, uint64_t out[4]) {
     return guarded(c, [&] { out[0] = c->n_launches; out[1] = c->h2d_bytes; out[2] = c->d2h_bytes; out[3] = (c->fr_batches << 32) | (c->fr_fallbacks & 0xffffffffull); });
+}
+
+int32_t arroy_b200_plane_rerank_stats(arroy_ctx* c, uint64_t out[4]) {
+    return guarded(c, [&] {
+        if (!out) throw ArgError("null argument");
+        uint64_t rows[2] = {0, 0};
+        if (c->pr_counts.p) {
+            set_device(c);
+            CK(cudaStreamSynchronize(c->stream));
+            CK(cudaMemcpy(rows, c->pr_counts.p, 16, cudaMemcpyDeviceToHost));
+        }
+        out[0] = c->pr_batches; out[1] = c->pr_fallbacks; out[2] = rows[0]; out[3] = rows[1];
+    });
 }
 
 int32_t arroy_b200_prefilter_scores(arroy_ctx* c, uint32_t nq, const float* queries, const uint32_t* rows, uint64_t n_rows, int32_t engine, float* out_scores) {

@@ -82,7 +82,9 @@ const char* arroy_b200_version(void);
  * library-owned mapped pinned host memory: the rows are decoded straight into it and cross PCIe once, in chunks, to a device
  * bounce buffer where the build's 8-bit planes and scales (and, for _flat's Cosine default headers, the norms) are written; the
  * device then holds 2 ld + 4 bytes per item plus headers, and no f32 rows. Builds scan through the planes and read the f32 rows
- * they cannot decide from host memory; queries and re-ranks read host rows too. Results are identical either way. A failed
+ * they cannot decide from host memory. Batched queries and re-ranks estimate their candidates from the planes and read only
+ * the rows that can still reach the top-k from host memory (arroy_b200_plane_rerank_stats); single queries and
+ * arroy_b200_rerank_shared read all their candidates' host rows. Results are identical either way. A failed
  * pinned allocation is ARROY_B200_ERR_CUDA and leaves nothing staged. ARROY_B200_HOST_ITEMS=1 forces host placement for
  * eligible indexes (tests and measurements). */
 int32_t arroy_b200_stage_items(arroy_ctx* ctx, int32_t metric, uint32_t dim, uint64_t n,
@@ -404,6 +406,15 @@ int32_t arroy_b200_build_breakdown(arroy_ctx* ctx, double out[8]);
  * out[1] = bytes copied host->device, out[2] = bytes copied device->host, out[3] = (query batches re-ranked by
  * the fused bf16-pre-filter kernel << 32) | batches that fell back to the plain distance + top-k kernels. */
 int32_t arroy_b200_counters(arroy_ctx* ctx, uint64_t out[4]);
+
+/* The plane pre-filter of host-placed indexes' re-rank, counted since arroy_b200_create. Batched searches and re-ranks of an
+ * index whose f32 rows are in host memory (arroy_b200_item_placement) estimate every candidate from the build's 8-bit planes on
+ * the device, with a proven error bound, and re-score only the rows that can still reach the top-k from the host rows (in the
+ * reference's order: results are identical). out[0] = query batches that went through it, out[1] = of those, batches that fell
+ * back to the plain kernels (a query with more than 8192 candidates or 2048 survivors; such a batch reads all its candidates
+ * from host memory again), out[2] = candidate rows estimated from the planes, out[3] = rows it re-scored from the f32 rows, i.e.
+ * read from host memory. ARROY_B200_FRERANK=0 turns it off. Device-placed indexes leave all four at 0. */
+int32_t arroy_b200_plane_rerank_stats(arroy_ctx* ctx, uint64_t out[4]);
 
 /* The score matrix of the pre-filter, for tests and profiling: out_scores[q * n_rows + i] ~ dot(query q,
  * item rows[i]) computed with TF32 inputs and FP32 accumulation on the tensor cores; guaranteed within

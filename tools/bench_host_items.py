@@ -7,6 +7,12 @@
       12 rows per create_split call, 4 ld bytes each; reads of the same row by several trees are counted each time), 1000-query
       batched search QPS (by vector, 10 neighbours) and the p50 of single-query calls. The forests of both placements must be
       byte-identical, and so must the query results.
+  Re-rank (--rerank): C2 staged once with forced host placement and built once; then the batched queries alternate between
+      the plane pre-filter of the re-rank (default) and ARROY_B200_FRERANK=0 (every candidate row read from host memory), three
+      runs each: 1000-query batched QPS by vector and by item at top-10 and top-100, the p50 of single-query calls (a path the
+      switch does not touch), and rows read from host memory per query (arroy_b200_plane_rerank_stats out[3] / queries) against
+      the candidates per query (out[2] / queries). Both sides' results must be byte-identical. One device-placed run of the
+      same queries is printed for comparison.
   Out of core: 11M x 1536 Cosine, 10 trees, staged with the automatic choice: 67.6 GB of f32 rows and 33.8 GB of planes, so an
       80 GB card must choose host. It runs only if MemAvailable covers the caller's copy plus the library's (about 140 GB);
       otherwise it prints "not run: host memory".
@@ -153,6 +159,66 @@ def c2(ctx, runs):
             assert rec["forest_identical"] and rec["results_identical"], rec
 
 
+def timed_qps(fn, nq, reps=3):
+    fn()   # warm-up
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        res = fn()
+    return res, round(reps * nq / (time.perf_counter() - t0), 1)
+
+
+def rerank_side(ctx, qv, qh, qrows, plane):
+    if plane:
+        os.environ.pop("ARROY_B200_FRERANK", None)
+    else:
+        os.environ["ARROY_B200_FRERANK"] = "0"
+    rec, res = {}, {}
+    for k in (10, 100):
+        s0 = ctx.plane_rerank_stats()
+        res["vec%d" % k], rec["qps_by_vector_top%d" % k] = timed_qps(lambda: ctx.search_batch(k, queries=qv, qhdr0=qh), len(qv))
+        res["item%d" % k], rec["qps_by_item_top%d" % k] = timed_qps(lambda: ctx.search_batch(k, query_rows=qrows), len(qrows))
+        s1 = ctx.plane_rerank_stats()
+        nq = 2 * 4 * len(qv)   # (warm-up + 3 timed calls) x (by vector, by item)
+        rec["top%d_rows_estimated_per_query" % k] = round((s1["rows_estimated"] - s0["rows_estimated"]) / nq, 1)
+        rec["top%d_rows_from_host_per_query" % k] = round((s1["rows_rescored"] - s0["rows_rescored"]) / nq, 2)
+        rec["top%d_fallback_batches" % k] = s1["fallbacks"] - s0["fallbacks"]
+    lat = []
+    for i in range(200):
+        t0 = time.perf_counter()
+        ctx.search_batch(10, queries=qv[i:i + 1], qhdr0=qh[i:i + 1])
+        lat.append((time.perf_counter() - t0) * 1e3)
+    rec["single_query_p50_ms"] = round(float(np.percentile(lat, 50)), 3)
+    os.environ.pop("ARROY_B200_FRERANK", None)
+    return res, rec
+
+
+def host_rerank(ctx, runs):
+    n, d, T = 1_000_000, 768, 50
+    rows = synth_host(ctx, n, d)
+    rng = np.random.default_rng(3)
+    qv = (rows[rng.choice(n, 1000)] + rng.standard_normal((1000, d)).astype(np.float32) * np.float32(0.05)).astype(np.float32)
+    qh = np.array([oracle.new_header(oracle.COSINE, v)[0] for v in qv], dtype=np.float32)
+    qrows = rng.choice(n, 1000).astype(np.uint32)
+    counts, rec = stage_and_build(ctx, rows, T, host=False)
+    nodes = emit(ctx, counts, T)
+    arrays = forest_arrays(nodes, d)
+    ctx.load_forest(roots=np.arange(T, dtype=np.uint32), **arrays)
+    dev_res, dev_rec = rerank_side(ctx, qv, qh, qrows, plane=True)
+    print(json.dumps({"workload": "C2 re-rank", "placement": rec["placement"], **dev_rec}), flush=True)
+    counts, rec = stage_and_build(ctx, rows, T, host=True)
+    assert rec["placement"] == "host", rec
+    assert emit(ctx, counts, T) == nodes
+    ctx.load_forest(roots=np.arange(T, dtype=np.uint32), **arrays)
+    for r in range(runs):
+        for plane in (True, False):
+            res, side = rerank_side(ctx, qv, qh, qrows, plane)
+            same = all(np.asarray(a).tobytes() == np.asarray(b).tobytes() for key in res for a, b in zip(res[key], dev_res[key]))
+            print(json.dumps({"workload": "C2 re-rank", "placement": "host", "path": "planes" if plane else "ARROY_B200_FRERANK=0", "run": r,
+                              **side, "results_identical_to_device_placement": same}), flush=True)
+            assert same
+
+
 def mem_available():
     with open("/proc/meminfo") as f:
         for line in f:
@@ -185,9 +251,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--skip-out-of-core", action="store_true")
+    ap.add_argument("--rerank", action="store_true", help="only the host-placed re-rank comparison")
     args = ap.parse_args()
     print(json.dumps({"card": card()}), flush=True)
     ctx = ab.Context(0)
+    if args.rerank:
+        host_rerank(ctx, args.runs)
+        ctx.close()
+        return
     c2(ctx, args.runs)
     if not args.skip_out_of_core:
         out_of_core(ctx)
