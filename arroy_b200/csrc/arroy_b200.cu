@@ -211,10 +211,9 @@ struct arroy_ctx {
     DevBuf pl_hi, pl_lo, pl_scale;
     bool planes_valid = false;
     // the plane pre-filter of host-placed items' re-rank (frerank_kernel<FR_PLANES>): device counters of candidates estimated
-    // and survivors re-scored, allocated by the first such batch; batches and fallbacks since create
+    // and survivors re-scored, allocated by the first such batch
     DevBuf pr_counts;
-    uint64_t pr_batches = 0, pr_fallbacks = 0;
-    uint64_t fr_batches = 0, fr_fallbacks = 0;   // last search_batch call, ms: bitmap clear + tree walk, candidate sort, distances, top-k   // last rerank_shared call, ms: prep, score GEMM, select, re-score, top-k, exact dense path
+    uint64_t fr_batches[2] = {0, 0}, fr_fallbacks[2] = {0, 0};   // fused re-rank batches and fallbacks since create, per FrSource
 };
 
 namespace {
@@ -265,15 +264,19 @@ void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
     c->n_launches += 1;
 }
 
+// norms_kernel over n rows of d = c->dim in a matrix of pitch c->ld (one 8-lane group per row); max_bits: their atomic max, or null
+void launch_norms(arroy_ctx* c, const float* rows, uint64_t n, float* out, uint32_t* max_bits) {
+    const uint64_t warps = (n + 3) / 4;
+    const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16));
+    norms_kernel<<<grid, 256, 0, c->stream>>>(rows, n, c->dim, c->ld, out, max_bits);
+    CK(cudaGetLastError());
+}
+
 void compute_norms(arroy_ctx* c, bool with_max) {
     c->norms.ensure(c->n * 4);
     c->maxbits.ensure(4);
     if (with_max) CK(cudaMemsetAsync(c->maxbits.p, 0, 4, c->stream));
-    uint64_t warps = (c->n + 3) / 4;
-    int grid = (int)std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16);
-    if (grid < 1) grid = 1;
-    norms_kernel<<<grid, 256, 0, c->stream>>>(items_f32(c), c->n, c->dim, c->ld, c->norms.as<float>(), with_max ? c->maxbits.as<uint32_t>() : nullptr);
-    CK(cudaGetLastError());
+    launch_norms(c, items_f32(c), c->n, c->norms.as<float>(), with_max ? c->maxbits.as<uint32_t>() : nullptr);
     c->n_launches += 1;
 }
 
@@ -1085,8 +1088,7 @@ const float* xf_candidates(arroy_ctx* c, const uint32_t* rows, uint32_t nc) {
 // kernel of tcgemm.cuh; engine 1: cuBLAS (kept as the cross-check of the hand-written kernel)
 void xf_scores(arroy_ctx* c, const float* q, uint32_t m, const float* cand, uint32_t nc, float* S, uint32_t lds, TgEpilogue ep, int engine) {
     if (engine == 0) {
-        const int mc = (getenv("ARROY_B200_XGEMM_MC") && atoi(getenv("ARROY_B200_XGEMM_MC")) == 1) ? 1 : 2;
-        if (!tcgemm_tf32(q, m, cand, nc, c->ld, S, lds, ep, c->sm_count, c->stream, mc)) throw CudaError(std::string("tcgemm_tf32 launch failed: ") + cudaGetErrorString(cudaGetLastError()));
+        if (!tcgemm_tf32(q, m, cand, nc, c->ld, S, lds, ep, c->sm_count, c->stream)) throw CudaError(std::string("tcgemm_tf32 launch failed: ") + cudaGetErrorString(cudaGetLastError()));
         c->n_launches += 1;
         return;
     }
@@ -1102,12 +1104,24 @@ void xf_scores(arroy_ctx* c, const float* q, uint32_t m, const float* cand, uint
 
 int xf_engine() { const char* e = getenv("ARROY_B200_XGEMM"); return (e && strcmp(e, "cublas") == 0) ? 1 : 0; }
 
+// A call's queries on the device: by item their rows (vecs == nullptr), by vector their vectors (rows == nullptr), and their
+// first header. Binary-quantized metrics: always their +-1 vectors (rows == nullptr), and their bit strings.
+struct DevQueries {
+    const float* vecs = nullptr;
+    const uint32_t* rows = nullptr;
+    const float* h0 = nullptr;
+    const uint4* bits = nullptr;
+};
+
 // ---- fused re-rank (frerank.cuh) -------------------------------------------------------------------
-bool frerank_enabled(arroy_ctx* c, uint32_t k) {
+// The estimate source of the fused re-rank for this context and k: device-placed items estimate from the bf16 shadow (Manhattan
+// has none), host-placed items from the build's 8-bit planes, which reads only the survivors' rows from host memory.
+// FR_NONE: the plain kernels re-rank (ARROY_B200_FRERANK=0, binary-quantized metrics, k or rows beyond the kernel's buffers).
+int frerank_source(arroy_ctx* c, uint32_t k) {
     const char* e = getenv("ARROY_B200_FRERANK");
-    const bool off = e != nullptr && atoi(e) == 0;
-    // (host-placed items have no bf16 shadow: their re-rank takes plane_rerank_enabled's kernel)
-    return !off && c->metric != MANHATTAN && !is_bq(c->metric) && !c->host_items && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
+    if ((e != nullptr && atoi(e) == 0) || is_bq(c->metric) || k > (uint32_t)FR_SURV || frerank_smem(c->ld) > 200 * 1024) return FR_NONE;
+    if (c->host_items) return c->planes_valid ? FR_PLANES : FR_NONE;
+    return c->metric != MANHATTAN ? FR_BF16 : FR_NONE;
 }
 
 // bf16 copy of the staged items (round to nearest even; padding stays zero) for the fused re-rank
@@ -1135,13 +1149,13 @@ void planes_prepare(arroy_ctx* c) {
     c->planes_valid = true;
 }
 
+// the bf16 source's per-item norms and gmax, built with the shadow
 void frerank_prepare(arroy_ctx* c) {
     if (c->fr_valid) return;
     shadow_prepare(c);
     c->fr_norm.ensure(std::max<size_t>(16, c->n * 4));
     c->fr_gmax.ensure(4);
-    { uint64_t warps = (c->n + 3) / 4; int g = (int)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16));
-      norms_kernel<<<g, 256, 0, c->stream>>>(c->items.as<float>(), c->n, c->dim, c->ld, c->fr_norm.as<float>(), nullptr); CK(cudaGetLastError()); }
+    launch_norms(c, c->items.as<float>(), c->n, c->fr_norm.as<float>(), nullptr);
     CK(cudaMemsetAsync(c->fr_gmax.p, 0, 4, c->stream));
     fr_gmax_kernel<<<(unsigned)((c->n + 255) / 256), 256, 0, c->stream>>>(c->fr_norm.as<float>(), c->h0.as<float>(), c->n, c->metric, c->fr_gmax.as<uint32_t>());
     CK(cudaGetLastError());
@@ -1149,64 +1163,44 @@ void frerank_prepare(arroy_ctx* c) {
     c->fr_valid = true;
 }
 
-// launches the fused kernel for m queries whose sorted candidate rows are rows[beg[q] .. end[q]); results in s_orows / s_odist /
-// s_olen, per-query status in fr_status (0 = done, 1 = needs the plain kernels)
-void frerank_launch(arroy_ctx* c, uint32_t m, const float* d_q, const uint32_t* d_qrows, const float* d_qh0, const uint32_t* d_rows,
-                    const uint64_t* d_beg, const uint64_t* d_end, uint32_t k) {
-    frerank_prepare(c);
+// launches the fused kernel with estimates from `src` for m queries whose sorted candidate rows are rows[beg[q] .. end[q]);
+// results in s_orows / s_odist / s_olen, per-query status in fr_status (0 = done, 1 = needs the plain kernels). The plane source
+// reads the planes, scales and headers on the device and needs nothing prepared.
+void frerank_launch(arroy_ctx* c, int src, uint32_t m, const DevQueries& Q, const uint32_t* d_rows, const uint64_t* d_beg, const uint64_t* d_end,
+                    uint32_t k) {
     c->fr_status.ensure(4ull * m);
-    FrParams P{};
-    P.items = c->items.as<float>(); P.shadow = c->fr_shadow.as<__nv_bfloat16>(); P.ih0 = c->h0.as<float>(); P.cnorm = c->fr_norm.as<float>();
-    P.d = c->dim; P.ld = c->ld; P.metric = c->metric;
-    P.queries = d_q; P.qrows = d_qrows; P.qh0 = d_qh0;
-    P.rows = d_rows; P.seg_beg = d_beg; P.seg_end = d_end;
-    P.k = k; P.rel = fr_rel(c->dim); P.sub = fr_sub(c->dim); P.hmin = cos_header_min(c->dim); P.gmax_bits = c->fr_gmax.as<uint32_t>();
-    P.out_rows = c->s_orows.as<uint32_t>(); P.out_dist = c->s_odist.as<float>(); P.out_len = c->s_olen.as<uint32_t>(); P.status = c->fr_status.as<int32_t>();
-    const size_t smem = frerank_smem(c->ld);
-    static std::atomic<size_t> configured{0};
-    if (smem > 48 * 1024 && smem > configured.load()) { CK(cudaFuncSetAttribute(frerank_kernel<FR_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured = smem; }
-    frerank_kernel<FR_BF16><<<m, FR_THREADS, smem, c->stream>>>(P);
-    CK(cudaGetLastError());
-    c->n_launches += 1;
-    c->fr_batches += 1;
-}
-
-// Host-placed items: the same per-query kernel with estimates from the build's 8-bit planes (frerank.cuh, FR_PLANES). It reads
-// the planes, scales and headers on the device and only the survivors' rows from host memory; it needs nothing prepared.
-bool plane_rerank_enabled(arroy_ctx* c, uint32_t k) {
-    const char* e = getenv("ARROY_B200_FRERANK");
-    const bool off = e != nullptr && atoi(e) == 0;
-    return !off && c->host_items && c->planes_valid && !is_bq(c->metric) && k <= (uint32_t)FR_SURV && frerank_smem(c->ld) <= 200 * 1024;
-}
-
-void plane_rerank_launch(arroy_ctx* c, uint32_t m, const float* d_q, const uint32_t* d_qrows, const float* d_qh0, const uint32_t* d_rows,
-                         const uint64_t* d_beg, const uint64_t* d_end, uint32_t k) {
-    c->fr_status.ensure(4ull * m);
-    if (!c->pr_counts.p) { c->pr_counts.ensure(16); CK(cudaMemsetAsync(c->pr_counts.p, 0, 16, c->stream)); }
     FrParams P{};
     P.items = items_f32(c); P.ih0 = c->h0.as<float>();
     P.d = c->dim; P.ld = c->ld; P.metric = c->metric;
-    P.queries = d_q; P.qrows = d_qrows; P.qh0 = d_qh0;
+    P.queries = Q.vecs; P.qrows = Q.rows; P.qh0 = Q.h0;
     P.rows = d_rows; P.seg_beg = d_beg; P.seg_end = d_end;
     P.k = k; P.hmin = cos_header_min(c->dim);
     P.out_rows = c->s_orows.as<uint32_t>(); P.out_dist = c->s_odist.as<float>(); P.out_len = c->s_olen.as<uint32_t>(); P.status = c->fr_status.as<int32_t>();
-    P.hi = c->pl_hi.as<int8_t>(); P.lo = c->pl_lo.as<int8_t>(); P.scale = c->pl_scale.as<float>();
-    fr_plane_consts(c->metric, c->dim, P);
-    P.counts = c->pr_counts.as<unsigned long long>();
+    if (src == FR_BF16) {
+        frerank_prepare(c);
+        P.shadow = c->fr_shadow.as<__nv_bfloat16>(); P.cnorm = c->fr_norm.as<float>();
+        P.rel = fr_rel(c->dim); P.sub = fr_sub(c->dim); P.gmax_bits = c->fr_gmax.as<uint32_t>();
+    } else {
+        if (!c->pr_counts.p) { c->pr_counts.ensure(16); CK(cudaMemsetAsync(c->pr_counts.p, 0, 16, c->stream)); }
+        P.hi = c->pl_hi.as<int8_t>(); P.lo = c->pl_lo.as<int8_t>(); P.scale = c->pl_scale.as<float>();
+        fr_plane_consts(c->metric, c->dim, P);
+        P.counts = c->pr_counts.as<unsigned long long>();
+    }
+    const auto kernel = src == FR_BF16 ? frerank_kernel<FR_BF16> : frerank_kernel<FR_PLANES>;
     const size_t smem = frerank_smem(c->ld);
-    static std::atomic<size_t> configured{0};
-    if (smem > 48 * 1024 && smem > configured.load()) { CK(cudaFuncSetAttribute(frerank_kernel<FR_PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured = smem; }
-    frerank_kernel<FR_PLANES><<<m, FR_THREADS, smem, c->stream>>>(P);
+    static std::atomic<size_t> configured[2] = {0, 0};
+    if (smem > 48 * 1024 && smem > configured[src].load()) { CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured[src] = smem; }
+    kernel<<<m, FR_THREADS, smem, c->stream>>>(P);
     CK(cudaGetLastError());
     c->n_launches += 1;
-    c->pr_batches += 1;
+    c->fr_batches[src] += 1;
 }
 
-// after the stream is idle: did every query finish in the fused kernel? (counts a fallback batch in `fallbacks`)
-bool frerank_ok(arroy_ctx* c, uint32_t m, uint64_t& fallbacks) {
+// after the stream is idle: did every query of the batch from `src` finish in the fused kernel? (else counts a fallback)
+bool frerank_ok(arroy_ctx* c, int src, uint32_t m) {
     std::vector<int32_t> st(m);
     CK(cudaMemcpy(st.data(), c->fr_status.p, 4ull * m, cudaMemcpyDeviceToHost));
-    for (int32_t x : st) if (x != 0) { fallbacks += 1; return false; }
+    for (int32_t x : st) if (x != 0) { c->fr_fallbacks[src] += 1; return false; }
     return true;
 }
 
@@ -1224,15 +1218,6 @@ struct Marks {
     int n = 0;
     void operator()() { if (!c->xev[n]) CK(cudaEventCreate(&c->xev[n])); CK(cudaEventRecord(c->xev[n], c->stream)); ++n; }
     void add_to(double* b) const { for (int i = 0; i + 1 < n; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); b[i] += ms; } }
-};
-
-// A call's queries on the device: by item their rows (vecs == nullptr), by vector their vectors (rows == nullptr), and their
-// first header. Binary-quantized metrics: always their +-1 vectors (rows == nullptr), and their bit strings.
-struct DevQueries {
-    const float* vecs = nullptr;
-    const uint32_t* rows = nullptr;
-    const float* h0 = nullptr;
-    const uint4* bits = nullptr;
 };
 
 // Uploads queries q0 .. q0 + m of a call: by item their rows into w_qrows, by vector their vectors into s_q (rows padded to ld
@@ -1279,14 +1264,11 @@ DevQueries upload_queries(arroy_ctx* c, uint32_t q0, uint32_t m, const uint32_t*
 // (beg / end are not const: the key sort stays the CUB instantiation with uint64_t* offsets, as the walk's candidate sort)
 void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32_t* rows, uint64_t* beg, uint64_t* end,
                      uint64_t n_keys, uint64_t max_len, uint32_t k, bool try_fused, Marks* mark) {
-    if (try_fused && frerank_enabled(c, k)) {   // one fused kernel per query: bf16 pre-filter + exact re-score + top-k (frerank.cuh)
-        frerank_launch(c, m, Q.vecs, Q.rows, Q.h0, rows, beg, end, k);
+    const int src = try_fused ? frerank_source(c, k) : FR_NONE;
+    if (src != FR_NONE) {   // one fused kernel per query: pre-filter + exact re-score + top-k (frerank.cuh)
+        frerank_launch(c, src, m, Q, rows, beg, end, k);
         CK(cudaStreamSynchronize(c->stream));
-        if (frerank_ok(c, m, c->fr_fallbacks)) { if (mark) (*mark)(); return; }
-    } else if (try_fused && plane_rerank_enabled(c, k)) {   // host-placed items: the same kernel on the 8-bit planes
-        plane_rerank_launch(c, m, Q.vecs, Q.rows, Q.h0, rows, beg, end, k);
-        CK(cudaStreamSynchronize(c->stream));
-        if (frerank_ok(c, m, c->pr_fallbacks)) { if (mark) (*mark)(); return; }
+        if (frerank_ok(c, src, m)) { if (mark) (*mark)(); return; }
     }
     if (max_len) {
         // (Manhattan sums one row per lane, the bit-string rows take four lanes per row, the other metrics eight)
@@ -1313,7 +1295,7 @@ void rerank_segments(arroy_ctx* c, uint32_t m, const DevQueries& Q, const uint32
         take_sorted_kernel<<<m, 256, 0, c->stream>>>(c->s_keys2.as<unsigned long long>(), c->s_dists.as<float>(), rows, beg, end, k, c->metric,
                                                      c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
     } else
-        topk_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), rows, beg, end, k, c->metric,
+        topk_kernel<false><<<m, TOPK_THREADS, 0, c->stream>>>(c->s_keys.as<unsigned long long>(), c->s_dists.as<float>(), rows, beg, end, 0, k, c->metric,
                                                        c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
     CK(cudaGetLastError());
 }
@@ -2030,8 +2012,7 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
         if (filter) {
             cand = xf_candidates(c, rows, nc);
             c->x_cnorm.ensure(4ull * nc);
-            { uint64_t warps = ((uint64_t)nc + 3) / 4; int g = (int)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16));
-              norms_kernel<<<g, 256, 0, c->stream>>>(cand, nc, c->dim, ld, c->x_cnorm.as<float>(), nullptr); CK(cudaGetLastError()); }
+            launch_norms(c, cand, nc, c->x_cnorm.as<float>(), nullptr);
             c->x_ca.ensure(4ull * nc); c->x_cb.ensure(4ull * nc); c->x_gmax.ensure(4);
             CK(cudaMemsetAsync(c->x_gmax.p, 0, 4, c->stream));
             xf_cand_prep_kernel<<<(nc + 255) / 256, 256, 0, c->stream>>>(c->x_cnorm.as<float>(), c->h0.as<float>(), c->s_rows.as<uint32_t>(), nc, c->metric, cos_header_min(c->dim),
@@ -2055,8 +2036,7 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
                 c->x_S.ensure(4ull * m * lds); c->x_qnorm.ensure(4ull * m); c->x_qa.ensure(4ull * m); c->x_qb.ensure(4ull * m); c->x_twoe.ensure(4ull * m);
                 c->x_sel.ensure(4ull * m * cap); c->x_beg.ensure(8ull * m); c->x_end.ensure(8ull * m);
                 c->s_dists.ensure(4ull * m * cap); c->s_keys.ensure(8ull * m * cap);
-                { uint64_t warps = ((uint64_t)m + 3) / 4; int g = (int)std::max<uint64_t>(1, std::min<uint64_t>((warps + 7) / 8, (uint64_t)c->sm_count * 16));
-                  norms_kernel<<<g, 256, 0, c->stream>>>(Q.vecs, m, c->dim, ld, c->x_qnorm.as<float>(), nullptr); CK(cudaGetLastError()); }
+                launch_norms(c, Q.vecs, m, c->x_qnorm.as<float>(), nullptr);
                 xf_query_prep_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(c->x_qnorm.as<float>(), Q.h0, m, c->metric, xf_rel(c->dim), c->dim, c->x_gmax.as<uint32_t>(),
                                                                              c->x_qa.as<float>(), c->x_qb.as<float>(), c->x_twoe.as<float>());
                 CK(cudaGetLastError());
@@ -2106,7 +2086,7 @@ int32_t arroy_b200_rerank_shared(arroy_ctx* c, uint32_t nq, const float* queries
                 else
                     xrerank_kernel<false><<<grid, XTHREADS, 0, c->stream>>>(x_items, x_h0, c->dim, ld, c->metric, Q.vecs, Q.h0, m, x_rows, nc, c->s_dists.as<float>());
                 CK(cudaGetLastError());
-                topk_dense_kernel<<<m, TOPK_THREADS, 0, c->stream>>>(c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), nc, k, c->metric,
+                topk_kernel<true><<<m, TOPK_THREADS, 0, c->stream>>>(nullptr, c->s_dists.as<float>(), c->s_rows.as<uint32_t>(), nullptr, nullptr, nc, k, c->metric,
                                                                      c->s_orows.as<uint32_t>(), c->s_odist.as<float>(), c->s_olen.as<uint32_t>());
                 CK(cudaGetLastError());
                 c->n_launches += 2;
@@ -2739,7 +2719,7 @@ int32_t arroy_b200_build_breakdown(arroy_ctx* c, double out[8]) {
 }
 
 int32_t arroy_b200_counters(arroy_ctx* c, uint64_t out[4]) {
-    return guarded(c, [&] { out[0] = c->n_launches; out[1] = c->h2d_bytes; out[2] = c->d2h_bytes; out[3] = (c->fr_batches << 32) | (c->fr_fallbacks & 0xffffffffull); });
+    return guarded(c, [&] { out[0] = c->n_launches; out[1] = c->h2d_bytes; out[2] = c->d2h_bytes; out[3] = (c->fr_batches[FR_BF16] << 32) | (c->fr_fallbacks[FR_BF16] & 0xffffffffull); });
 }
 
 int32_t arroy_b200_plane_rerank_stats(arroy_ctx* c, uint64_t out[4]) {
@@ -2751,7 +2731,7 @@ int32_t arroy_b200_plane_rerank_stats(arroy_ctx* c, uint64_t out[4]) {
             CK(cudaStreamSynchronize(c->stream));
             CK(cudaMemcpy(rows, c->pr_counts.p, 16, cudaMemcpyDeviceToHost));
         }
-        out[0] = c->pr_batches; out[1] = c->pr_fallbacks; out[2] = rows[0]; out[3] = rows[1];
+        out[0] = c->fr_batches[FR_PLANES]; out[1] = c->fr_fallbacks[FR_PLANES]; out[2] = rows[0]; out[3] = rows[1];
     });
 }
 

@@ -39,17 +39,17 @@
 //   is rel qn gmax.
 //
 // One CTA per query, everything in shared memory:
-//   1. estimates of all candidates (8 lanes per row, 16-byte loads of 8 bf16)
+//   1. estimates of all candidates (fr_estimates_bf16: 8 lanes per row, 16-byte loads of 8 bf16)
 //   2. t = k-th smallest estimate (linear-range histograms), threshold t + 2E
 //   3. survivors (estimate <= threshold, or not finite) in candidate order = ascending ids
-//   4. exact distances of the survivors (distance_kernel's code), 64-bit keys, bitonic sort,
-//      first k -> out_rows / normalized distances (what topk_kernel returns)
+//   4. exact distances of the survivors (distance_kernel's row_sum8; Manhattan in the reference's sequential order), 64-bit
+//      keys, bitonic sort, first k -> out_rows / normalized distances (what topk_kernel returns)
 // A query with more candidates than FR_CAP or more survivors than FR_SURV sets its status to 1 and
 // the host re-runs the batch on the plain kernels.
 //
 // Host-placed items (frerank_kernel<FR_PLANES>): the f32 rows are in mapped host memory and there is no bf16 shadow, but the
-// build's two 8-bit planes and row scales are on the device (kernels.cuh planes_encode_kernel). Phase 1 then estimates every
-// candidate from its planes (2 bytes per element; nothing reads an f32 row, a norm or a gmax, each of which would be a pass over
+// build's two 8-bit planes and row scales are on the device (kernels.cuh planes_encode_kernel). Phase 1 (fr_estimates_planes)
+// then estimates every candidate from its planes (2 bytes per element; nothing reads an f32 row, a norm or a gmax, each of which would be a pass over
 // PCIe), phases 2-3 are the same, and phase 4 re-scores only the survivors from the host rows — about k rows per query instead
 // of all of its candidates. The estimate and its bound, with u = 2^-24:
 //   * dequantization: y_i = 254 h_i + l_i is an exact integer (|y_i| <= 32385), turned into a float exactly (the 1.5 2^23 bias
@@ -94,7 +94,7 @@ constexpr int FR_THREADS = 256;
 constexpr int FR_CAP = 8192;      // candidates per query held in shared memory
 constexpr int FR_SURV = 2048;     // survivors per query
 constexpr int FR_BINS = 2048;
-enum FrSource { FR_BF16 = 0, FR_PLANES = 1 };   // where phase 1's estimates come from
+enum FrSource { FR_NONE = -1, FR_BF16 = 0, FR_PLANES = 1 };   // where phase 1's estimates come from (FR_NONE: the fused kernel does not run)
 
 inline float fr_rel(uint32_t d) { return 0.004150390625f + (float)d * 2.384185791015625e-07f; }   // 1.0625 * 2^-8 + d 2^-22
 inline float fr_sub(uint32_t d) { return sqrtf((float)d + 64.0f) * 5.293955920339377e-23f; }  // sqrt(d + 64) 2^-74
@@ -108,21 +108,6 @@ __global__ void fr_shadow_kernel(const float4* __restrict__ items, uint2* __rest
         o.x = *reinterpret_cast<uint32_t*>(&a); o.y = *reinterpret_cast<uint32_t*>(&b);
         shadow[i] = o;
     }
-}
-
-__device__ __forceinline__ uint32_t fr_block_scan(uint32_t v, uint32_t* sm /* 9 */, uint32_t* total) {   // exclusive scan over FR_THREADS
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    __syncthreads();
-    if (lane == 31) sm[warp] = inc;
-    __syncthreads();
-    uint32_t base = 0, tot = 0;
-#pragma unroll
-    for (int i = 0; i < FR_THREADS / 32; ++i) { const uint32_t y = sm[i]; if (i < warp) base += y; tot += y; }
-    *total = tot;
-    return base + inc - v;
 }
 
 struct FrParams {
@@ -171,42 +156,17 @@ __device__ __forceinline__ void fr_plane_row(const int8_t* __restrict__ hi, cons
     if (g8 < tail) step(__ldg(H + nch * 8 + g8), __ldg(L + nch * 8 + g8), sq + nch * 128 + g8 * 16);
 }
 
-template <int SRC>
-__global__ void __launch_bounds__(FR_THREADS)
-frerank_kernel(FrParams P) {
-    extern __shared__ __align__(16) unsigned char fr_smem[];
-    // shared memory: [query ld floats][region A: FR_CAP estimates; in phase 4 re-used for FR_SURV keys + FR_SURV distances]
-    //                [FR_BINS histogram words; from phase 3 on the survivor positions] — 43 KB at d = 768, five CTAs per SM
-    float* sq = reinterpret_cast<float*>(fr_smem);
-    float* est = sq + P.ld;
-    unsigned long long* keys = reinterpret_cast<unsigned long long*>(est);          // phase 4 (the estimates are dead by then)
-    float* sdist = est + 2 * FR_SURV;                                               // phase 4: exact distance per survivor
-    uint32_t* hist = reinterpret_cast<uint32_t*>(est + FR_CAP);
-    __shared__ uint32_t sm_scan[9];
-    __shared__ uint32_t sh_min, sh_max, sh_bin, sh_before;
-    const uint32_t q = blockIdx.x;
+// Phase 1 from the bf16 shadow: est[p] for every candidate p, the CTA's smallest and largest key in sh_min / sh_max; returns 2E.
+__device__ __forceinline__ float fr_estimates_bf16(const FrParams& P, const float* __restrict__ sq, float* __restrict__ est, const uint32_t* __restrict__ rows,
+                                                   uint32_t nc, float qh, uint32_t* sh_min, uint32_t* sh_max) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
-    const uint64_t beg = P.seg_beg[q], end = P.seg_end[q];
-    const uint32_t nc = (uint32_t)(end - beg);
-    const uint32_t* rows = P.rows + beg;
-    const uint32_t k = P.k, kk = nc < k ? nc : k;
-    const float* qv = P.qrows ? P.items + (size_t)P.qrows[q] * P.ld : P.queries + (size_t)q * P.ld;
-    const float qh = P.qh0 ? P.qh0[q] : 0.f;
     const int metric = P.metric;
-    if (tid == 0) { sh_min = 0xffffffffu; sh_max = 0u; P.status[q] = 0; }
-    if (nc > FR_CAP) { if (tid == 0) { P.status[q] = 1; P.out_len[q] = 0; } return; }
-    for (uint32_t i = tid; i < P.ld; i += FR_THREADS) sq[i] = qv[i];
-    __syncthreads();
-
-    float two_e;
-    bool e_ok;
-    if constexpr (SRC == FR_BF16) {
     // |q| (any order: it only enters the bound) and the per-query constants of the estimate
+    __shared__ float sm_f[FR_THREADS / 32];
     float part = 0.f;
     for (uint32_t i = tid; i < P.d; i += FR_THREADS) part = fmaf(sq[i], sq[i], part);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    __shared__ float sm_f[FR_THREADS / 32];
     if (lane == 0) sm_f[warp] = part;
     __syncthreads();
     float qq = 0.f;
@@ -219,10 +179,8 @@ frerank_kernel(FrParams P) {
     if (metric == DOT_PRODUCT) e = eps;
     else if (metric == EUCLIDEAN) { qa = qq; e = fmaf(((float)(P.d / 32u) + 16.0f) * 2.384185791015625e-07f, qq + gmax * gmax, 2.0f * eps); }
     else { if (qh >= 1e-30f) { qa = 1.0f / qh; e = fmaf(0.5f * eps, qa, 1.9073486328125e-06f); } else { qa = __uint_as_float(0x7fc00000u); e = 1.9073486328125e-06f; } }
-    two_e = 2.0f * e * 1.001f;
-    e_ok = two_e >= 0.0f && two_e <= 3.0e38f;
 
-    // ---- 1. estimates from the bf16 shadow ------------------------------------------------------
+    // estimates: 8 lanes per row, 16-byte loads of 8 bf16
     const int nch = (int)(P.ld >> 6);                      // chunks of 64 elements (8 lanes x 8 bf16); ld % 32 == 0
     const bool half_chunk = (P.ld & 32u) != 0;             // a trailing chunk of 32 elements (lanes 0..3 of the group)
     uint32_t mn = 0xffffffffu, mx = 0u;
@@ -260,9 +218,17 @@ frerank_kernel(FrParams P) {
         }
     }
     mn = __reduce_min_sync(0xffffffffu, mn); mx = __reduce_max_sync(0xffffffffu, mx);
-    if (lane == 0) { atomicMin(&sh_min, mn); atomicMax(&sh_max, mx); }
+    if (lane == 0) { atomicMin(sh_min, mn); atomicMax(sh_max, mx); }
     __syncthreads();
-    } else {
+    return 2.0f * e * 1.001f;
+}
+
+// Phase 1 from the 8-bit planes: est[p] for every candidate p and the largest per-row bound E, the CTA's smallest and largest
+// key in sh_min / sh_max; returns 2E.
+__device__ __forceinline__ float fr_estimates_planes(const FrParams& P, const float* __restrict__ sq, float* __restrict__ est, const uint32_t* __restrict__ rows,
+                                                     uint32_t nc, float qh, uint32_t* sh_min, uint32_t* sh_max) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
+    const int metric = P.metric;
     // |q|_1 (any order: it only enters the bound) and 1 / qh
     __shared__ float sm_f[FR_THREADS / 32];
     __shared__ uint32_t sh_e;
@@ -279,7 +245,6 @@ frerank_kernel(FrParams P) {
     l1q *= 1.001f;
     const float qa = metric == COSINE ? (qh >= 1e-30f ? 1.0f / qh : __uint_as_float(0x7fc00000u)) : 0.f;
 
-    // ---- 1. estimates from the 8-bit planes, and the largest per-row bound --------------------------------------------------
     uint32_t mn = 0xffffffffu, mx = 0u, eb = 0u;
     for (uint32_t p0 = (uint32_t)warp * 4u; p0 < nc; p0 += (FR_THREADS / 32) * 4u) {
         const uint32_t p = p0 + (uint32_t)grp;
@@ -319,44 +284,50 @@ frerank_kernel(FrParams P) {
         }
     }
     mn = __reduce_min_sync(0xffffffffu, mn); mx = __reduce_max_sync(0xffffffffu, mx); eb = __reduce_max_sync(0xffffffffu, eb);
-    if (lane == 0) { atomicMin(&sh_min, mn); atomicMax(&sh_max, mx); atomicMax(&sh_e, eb); }
+    if (lane == 0) { atomicMin(sh_min, mn); atomicMax(sh_max, mx); atomicMax(&sh_e, eb); }
     __syncthreads();
-    two_e = 2.0f * __uint_as_float(sh_e) * 1.001f;
-    e_ok = two_e >= 0.0f && two_e <= 3.0e38f;
-    }
+    return 2.0f * __uint_as_float(sh_e) * 1.001f;
+}
+
+template <int SRC>
+__global__ void __launch_bounds__(FR_THREADS)
+frerank_kernel(FrParams P) {
+    extern __shared__ __align__(16) unsigned char fr_smem[];
+    // shared memory: [query ld floats][region A: FR_CAP estimates; in phase 4 re-used for FR_SURV keys + FR_SURV distances]
+    //                [FR_BINS histogram words; from phase 3 on the survivor positions] — 43 KB at d = 768, five CTAs per SM
+    float* sq = reinterpret_cast<float*>(fr_smem);
+    float* est = sq + P.ld;
+    unsigned long long* keys = reinterpret_cast<unsigned long long*>(est);          // phase 4 (the estimates are dead by then)
+    float* sdist = est + 2 * FR_SURV;                                               // phase 4: exact distance per survivor
+    uint32_t* hist = reinterpret_cast<uint32_t*>(est + FR_CAP);
+    __shared__ uint32_t sm_scan[FR_THREADS / 32];
+    __shared__ uint32_t sh_min, sh_max, sh_bin[2];
+    const uint32_t q = blockIdx.x;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
+    const uint64_t beg = P.seg_beg[q], end = P.seg_end[q];
+    const uint32_t nc = (uint32_t)(end - beg);
+    const uint32_t* rows = P.rows + beg;
+    const uint32_t k = P.k, kk = nc < k ? nc : k;
+    const float* qv = P.qrows ? P.items + (size_t)P.qrows[q] * P.ld : P.queries + (size_t)q * P.ld;
+    const float qh = P.qh0 ? P.qh0[q] : 0.f;
+    const int metric = P.metric;
+    if (tid == 0) { sh_min = 0xffffffffu; sh_max = 0u; P.status[q] = 0; }
+    if (nc > FR_CAP) { if (tid == 0) { P.status[q] = 1; P.out_len[q] = 0; } return; }
+    for (uint32_t i = tid; i < P.ld; i += FR_THREADS) sq[i] = qv[i];
+    __syncthreads();
+
+    // ---- 1. estimates of all candidates ---------------------------------------------------------
+    float two_e;
+    if constexpr (SRC == FR_BF16) two_e = fr_estimates_bf16(P, sq, est, rows, nc, qh, &sh_min, &sh_max);
+    else two_e = fr_estimates_planes(P, sq, est, rows, nc, qh, &sh_min, &sh_max);
 
     // ---- 2. k-th smallest estimate (upper bin edge) ---------------------------------------------
     uint32_t T = 0xffffffffu;   // key of the threshold t + 2E
-    if (nc > k && e_ok) {
-        uint32_t rlo = sh_min, rhi = sh_max, want = k;
-        for (int level = 0; level < 3 && rhi > rlo; ++level) {
-            for (int i = tid; i < FR_BINS; i += FR_THREADS) hist[i] = 0;
-            __syncthreads();
-            const uint32_t span = rhi - rlo;
-            const int shift = span < FR_BINS ? 0 : (32 - __clz(span)) - 11;
-            for (uint32_t p = tid; p < nc; p += FR_THREADS) { const uint32_t key = xf_key(est[p]); if (key >= rlo && key <= rhi) atomicAdd(&hist[(key - rlo) >> shift], 1u); }
-            __syncthreads();
-            // smallest bin whose cumulative count reaches `want`
-            constexpr int PER = FR_BINS / FR_THREADS;
-            uint32_t local = 0;
-#pragma unroll
-            for (int i = 0; i < PER; ++i) local += hist[tid * PER + i];
-            uint32_t total;
-            const uint32_t ex = fr_block_scan(local, sm_scan, &total);
-            if (tid == 0) { sh_bin = FR_BINS - 1; sh_before = total; }
-            __syncthreads();
-            if (ex < want && ex + local >= want) {
-                uint32_t cum = ex;
-                for (int i = 0; i < PER; ++i) { const uint32_t h = hist[tid * PER + i]; if (cum + h >= want) { sh_bin = tid * PER + i; sh_before = cum; break; } cum += h; }
-            }
-            __syncthreads();
-            const uint32_t b = sh_bin, in_bin = hist[b];
-            const uint32_t top = (uint32_t)min((unsigned long long)rhi, (unsigned long long)rlo + (((unsigned long long)b + 1ull) << shift) - 1ull);
-            want -= sh_before; rlo = rlo + (b << shift); rhi = top;
-            __syncthreads();
-            if (in_bin <= 8u || shift == 0) break;
-        }
-        T = xf_widen(rhi, two_e);
+    if (nc > k && two_e >= 0.0f && two_e <= 3.0e38f) {
+        const uint32_t t = hist_narrow<FR_THREADS, FR_BINS>(sh_min, sh_max, k, 8u, [&](auto add) {
+            for (uint32_t p = tid; p < nc; p += FR_THREADS) add(xf_key(est[p]));
+        }, hist, sm_scan, sh_bin);
+        T = xf_widen(t, two_e);
     }
 
     // ---- 3. survivors in candidate order ----------------------------------------------------------
@@ -367,7 +338,7 @@ frerank_kernel(FrParams P) {
         uint32_t keep = 0;
         if (p < nc) { const uint32_t key = xf_key(est[p]); keep = (key <= T || key == 0xffffffffu) ? 1u : 0u; }
         uint32_t total;
-        const uint32_t pos = count + fr_block_scan(keep, sm_scan, &total);
+        const uint32_t pos = count + block_exclusive_scan<FR_THREADS>(keep, sm_scan, &total);
         if (keep && pos < FR_SURV) surv[pos] = p;
         count += total;
     }
@@ -386,59 +357,26 @@ frerank_kernel(FrParams P) {
         const bool v = s < count;
         const uint32_t p = v ? surv[s] : 0u;
         const uint32_t r = v ? rows[p] : 0u;
+        const float* row = P.items + (size_t)r * P.ld;
         float res;
         if (metric == MANHATTAN) {
-            res = 0.f;
-            if constexpr (SRC == FR_PLANES) {
-                const float* row = P.items + (size_t)r * P.ld;
-                // Manhattan's survivors (FR_PLANES only: the bf16 path never takes Manhattan): the reference's strictly sequential
-                // sum in element order. The group's 8 lanes load the row in 16-byte pieces, all in flight at once (the row is read
-                // over PCIe), and lane 0 adds the terms in order from their registers.
-                const float4* A = reinterpret_cast<const float4*>(row);
-                const float4* Q = reinterpret_cast<const float4*>(sq);
-                const int src = lane & ~7, n32 = (int)(P.d >> 5);
-#pragma unroll 4
-                for (int c = 0; c < n32; ++c) {
-                    const float4 x = Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
-                    const float t[4] = {fabsf(__fsub_rn(x.x, y.x)), fabsf(__fsub_rn(x.y, y.y)), fabsf(__fsub_rn(x.z, y.z)), fabsf(__fsub_rn(x.w, y.w))};
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) res = __fadd_rn(res, __shfl_sync(0xffffffffu, t[e], src + j));
-                }
-                if (g8 == 0) for (uint32_t i = (uint32_t)n32 * 32u; i < P.d; ++i) res = __fadd_rn(res, fabsf(__fsub_rn(sq[i], row[i])));
-            } else {   // not reached (frerank_enabled keeps Manhattan off the bf16 path); kept for completeness
-                if (g8 == 0) { const float* row = P.items + (size_t)r * P.ld; for (uint32_t i = 0; i < P.d; ++i) res = __fadd_rn(res, fabsf(__fsub_rn(sq[i], row[i]))); }
-            }
-        } else if (P.d >= 32) {
-            const float4* A = reinterpret_cast<const float4*>(P.items + (size_t)r * P.ld);
+            // the reference's strictly sequential sum in element order. The group's 8 lanes load the row in 16-byte pieces, all in
+            // flight at once (host-placed rows are read over PCIe), and lane 0 adds the terms in order from their registers.
+            const float4* A = reinterpret_cast<const float4*>(row);
             const float4* Q = reinterpret_cast<const float4*>(sq);
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int n32 = (int)(P.d >> 5);
-            if (metric == EUCLIDEAN) {
-#pragma unroll 4
-                for (int c = 0; c < n32; ++c) {
-                    const float4 x = Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
-                    const float t0 = __fsub_rn(x.x, y.x), t1 = __fsub_rn(x.y, y.y), t2 = __fsub_rn(x.z, y.z), t3 = __fsub_rn(x.w, y.w);
-                    acc.x = fmaf(t0, t0, acc.x); acc.y = fmaf(t1, t1, acc.y); acc.z = fmaf(t2, t2, acc.z); acc.w = fmaf(t3, t3, acc.w);
-                }
-            } else {
-#pragma unroll 4
-                for (int c = 0; c < n32; ++c) {
-                    const float4 x = Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
-                    acc.x = fmaf(x.x, y.x, acc.x); acc.y = fmaf(x.y, y.y, acc.y); acc.z = fmaf(x.z, y.z, acc.z); acc.w = fmaf(x.w, y.w, acc.w);
-                }
-            }
-            res = group8_hsum(acc);
-            const float* row = P.items + (size_t)r * P.ld;
-            for (uint32_t i = (uint32_t)n32 * 32u; i < P.d; ++i) {
-                if (metric == EUCLIDEAN) { const float t = __fsub_rn(sq[i], row[i]); res = __fadd_rn(res, __fmul_rn(t, t)); }
-                else res = __fadd_rn(res, __fmul_rn(sq[i], row[i]));
-            }
-        } else {
+            const int src = lane & ~7, n32 = (int)(P.d >> 5);
             res = 0.f;
-            if (g8 == 0 && v) { const float* row = P.items + (size_t)r * P.ld; res = (metric == EUCLIDEAN) ? exact_thread<true>(sq, row, (int)P.d) : exact_thread<false>(sq, row, (int)P.d); }
-        }
+#pragma unroll 4
+            for (int c = 0; c < n32; ++c) {
+                const float4 x = Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
+                const float t[4] = {fabsf(__fsub_rn(x.x, y.x)), fabsf(__fsub_rn(x.y, y.y)), fabsf(__fsub_rn(x.z, y.z)), fabsf(__fsub_rn(x.w, y.w))};
+#pragma unroll
+                for (int j = 0; j < 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) res = __fadd_rn(res, __shfl_sync(0xffffffffu, t[e], src + j));
+            }
+            if (g8 == 0) for (uint32_t i = (uint32_t)n32 * 32u; i < P.d; ++i) res = __fadd_rn(res, fabsf(__fsub_rn(sq[i], row[i])));
+        } else res = row_sum8<false>(metric == EUCLIDEAN, sq, row, P.d, g8, v);
         if (v && g8 == 0) {
             const float dist = built_finish(metric, res, qh, (metric == COSINE) ? P.ih0[r] : 0.f);
             sdist[s] = dist;

@@ -11,6 +11,7 @@
 // reference's exact summation order (exact.cuh), no tensor cores.
 #pragma once
 #include "exact.cuh"
+#include "select.cuh"
 
 namespace ab {
 
@@ -849,6 +850,39 @@ __device__ __forceinline__ float built_finish(int metric, float acc, float qh0, 
     return 0.0f;
 }
 
+// The raw sum of built_distance (Euclidean: the sum of squared differences, else the dot product) of the query q and one row,
+// in the reference's summation order, by the 8 lanes g8 of a group. d >= 32: every lane of the warp takes part (the AVX order
+// over 16-byte loads, group8_hsum, then the separately rounded tail). d < 32: lane g8 == 0 alone, when v (exact_thread). The
+// result is valid in lane g8 == 0. Q_LDG: q is read through the read-only cache (global memory), else with plain loads.
+template <bool Q_LDG>
+__device__ __forceinline__ float row_sum8(bool euclid, const float* q, const float* row, uint32_t d, int g8, bool v) {
+    if (d < 32) return (g8 == 0 && v) ? (euclid ? exact_thread<true>(q, row, (int)d) : exact_thread<false>(q, row, (int)d)) : 0.f;
+    const float4* A = reinterpret_cast<const float4*>(row);
+    const float4* Q = reinterpret_cast<const float4*>(q);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int nch = (int)(d >> 5);
+    if (euclid) {
+#pragma unroll 4
+        for (int c = 0; c < nch; ++c) {
+            const float4 x = Q_LDG ? __ldg(Q + c * 8 + g8) : Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
+            const float t0 = __fsub_rn(x.x, y.x), t1 = __fsub_rn(x.y, y.y), t2 = __fsub_rn(x.z, y.z), t3 = __fsub_rn(x.w, y.w);
+            acc.x = fmaf(t0, t0, acc.x); acc.y = fmaf(t1, t1, acc.y); acc.z = fmaf(t2, t2, acc.z); acc.w = fmaf(t3, t3, acc.w);
+        }
+    } else {
+#pragma unroll 4
+        for (int c = 0; c < nch; ++c) {
+            const float4 x = Q_LDG ? __ldg(Q + c * 8 + g8) : Q[c * 8 + g8], y = ldg_stream(A + c * 8 + g8);
+            acc.x = fmaf(x.x, y.x, acc.x); acc.y = fmaf(x.y, y.y, acc.y); acc.z = fmaf(x.z, y.z, acc.z); acc.w = fmaf(x.w, y.w, acc.w);
+        }
+    }
+    float res = group8_hsum(acc);
+    for (uint32_t i = (uint32_t)nch * 32u; i < d; ++i) {
+        if (euclid) { const float t = __fsub_rn(q[i], row[i]); res = __fadd_rn(res, __fmul_rn(t, t)); }
+        else res = __fadd_rn(res, __fmul_rn(q[i], row[i]));
+    }
+    return res;
+}
+
 __global__ void __launch_bounds__(256)
 distance_kernel(const float* __restrict__ items, const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric,
                 const float* __restrict__ queries, const uint32_t* __restrict__ qrows, const float* __restrict__ qh0, uint32_t nq,
@@ -875,56 +909,15 @@ distance_kernel(const float* __restrict__ items, const float* __restrict__ ih0, 
         }
         return;
     }
-    for (uint64_t p0 = beg + warp_global * 4; p0 < end; p0 += nwarps * 4) {
-        float res;
-        uint64_t p;
-        bool v, writer;
-        uint32_t r = 0;
-        if (d >= 32) {
-            const int g8 = lane & 7, grp = lane >> 3;
-            p = p0 + grp;
-            v = p < end;
-            writer = g8 == 0;
-            if (v) r = rows[p];
-            const float4* A = reinterpret_cast<const float4*>(items + (size_t)r * ld);
-            const float4* Q = reinterpret_cast<const float4*>(qv);
-            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int nch = d >> 5;
-            if (metric == EUCLIDEAN || metric == BQ_EUCLIDEAN) {
-#pragma unroll 4
-                for (int c = 0; c < nch; ++c) {
-                    float4 x = __ldg(Q + c * 8 + g8);
-                    float4 y = ldg_stream(A + c * 8 + g8);
-                    float t0 = __fsub_rn(x.x, y.x), t1 = __fsub_rn(x.y, y.y), t2 = __fsub_rn(x.z, y.z), t3 = __fsub_rn(x.w, y.w);
-                    acc.x = fmaf(t0, t0, acc.x); acc.y = fmaf(t1, t1, acc.y); acc.z = fmaf(t2, t2, acc.z); acc.w = fmaf(t3, t3, acc.w);
-                }
-            } else {
-#pragma unroll 4
-                for (int c = 0; c < nch; ++c) {
-                    float4 x = __ldg(Q + c * 8 + g8);
-                    float4 y = ldg_stream(A + c * 8 + g8);
-                    acc.x = fmaf(x.x, y.x, acc.x); acc.y = fmaf(x.y, y.y, acc.y); acc.z = fmaf(x.z, y.z, acc.z); acc.w = fmaf(x.w, y.w, acc.w);
-                }
-            }
-            res = group8_hsum(acc);
-            const float* row = items + (size_t)r * ld;
-            for (uint32_t i = nch * 32; i < d; ++i) {
-                if (metric == EUCLIDEAN || metric == BQ_EUCLIDEAN) { float t = __fsub_rn(qv[i], row[i]); res = __fadd_rn(res, __fmul_rn(t, t)); }
-                else res = __fadd_rn(res, __fmul_rn(qv[i], row[i]));
-            }
-        } else {
-            p = p0 + lane;
-            v = lane < 4 && p < end;
-            writer = true;
-            res = 0.f;
-            if (v) {
-                r = rows[p];
-                const float* row = items + (size_t)r * ld;
-                res = (metric == EUCLIDEAN || metric == BQ_EUCLIDEAN) ? exact_thread<true>(qv, row, (int)d) : exact_thread<false>(qv, row, (int)d);
-            }
-        }
-        if (v && writer) {
-            float dist = built_finish(metric, res, qhdr, (metric == COSINE || metric == BQ_COSINE) ? ih0[r] : 0.f);
+    const bool euclid = metric == EUCLIDEAN || metric == BQ_EUCLIDEAN;
+    const int g8 = lane & 7, grp = lane >> 3;
+    for (uint64_t p0 = beg + warp_global * 4; p0 < end; p0 += nwarps * 4) {   // one row per 8-lane group
+        const uint64_t p = p0 + grp;
+        const bool v = p < end;
+        const uint32_t r = v ? rows[p] : 0u;
+        const float res = row_sum8<true>(euclid, qv, items + (size_t)r * ld, d, g8, v);
+        if (v && g8 == 0) {
+            const float dist = built_finish(metric, res, qhdr, (metric == COSINE || metric == BQ_COSINE) ? ih0[r] : 0.f);
             dists[p] = dist;
             keys[p] = ((unsigned long long)ordered_key(dist) << 32) | (unsigned long long)(uint32_t)(p - beg);
         }
@@ -936,24 +929,11 @@ distance_kernel(const float* __restrict__ items, const float* __restrict__ ih0, 
 // [0,k) (sorted) and is refilled with up to CAP-k new keys that beat the current k-th key, then
 // bitonic-sorted. Equivalent to sort-ascending-take-k on (OrderedFloat, id) — which is what
 // median_based_top_k returns (src/reader.rs:607-640, tests/reader.rs:283-299).
+// The query's keys: DENSE, formed here from its row of a dense distance matrix (dists + q * nc) over one candidate list `rows`
+// that all queries share, key = ordered_key(dist) << 32 | position; else distance_kernel's keys[seg_beg[q] .. seg_end[q]) over
+// the query's own candidates rows + seg_beg[q].
 constexpr int TOPK_CAP = 4096;
 constexpr int TOPK_THREADS = 256;
-
-__device__ __forceinline__ void bitonic_sort_shared(unsigned long long* buf, int n /* power of two */) {
-    for (int size = 2; size <= n; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            for (int t = threadIdx.x; t < (n >> 1); t += blockDim.x) {
-                int i = 2 * t - (t & (stride - 1));
-                int j = i + stride;
-                bool up = ((i & size) == 0);
-                unsigned long long a = buf[i], b = buf[j];
-                if ((a > b) == up) { buf[i] = b; buf[j] = a; }
-            }
-        }
-    }
-    __syncthreads();
-}
 
 __device__ __forceinline__ float normalized_distance_dev(int metric, float dist) {
     if (metric == EUCLIDEAN) return __fsqrt_rn(dist);  // mod.rs:59-61
@@ -962,17 +942,18 @@ __device__ __forceinline__ float normalized_distance_dev(int metric, float dist)
     return (dist != dist) ? 0.0f : (dist > 0.0f ? dist : 0.0f);  // manhattan.rs:48-50 (f32::max)
 }
 
+template <bool DENSE>
 __global__ void __launch_bounds__(TOPK_THREADS)
 topk_kernel(const unsigned long long* __restrict__ keys, const float* __restrict__ dists, const uint32_t* __restrict__ rows,
-            const uint64_t* __restrict__ seg_beg, const uint64_t* __restrict__ seg_end, uint32_t k, int metric,
+            const uint64_t* __restrict__ seg_beg, const uint64_t* __restrict__ seg_end, uint32_t nc, uint32_t k, int metric,
             uint32_t* __restrict__ out_rows, float* __restrict__ out_dist, uint32_t* __restrict__ out_len) {
     __shared__ unsigned long long buf[TOPK_CAP];
     __shared__ uint32_t fill;
     const uint32_t q = blockIdx.x;
-    const uint64_t beg = seg_beg[q], end = seg_end[q];
-    const uint64_t n = end - beg;
+    const uint64_t beg = DENSE ? (uint64_t)q * nc : seg_beg[q];
+    const uint64_t n = DENSE ? (uint64_t)nc : seg_end[q] - beg;
+    const uint32_t* qrows = DENSE ? rows : rows + beg;
     const uint32_t kk = (uint32_t)(n < (uint64_t)k ? n : (uint64_t)k);
-    for (int i = threadIdx.x; i < TOPK_CAP; i += blockDim.x) buf[i] = ~0ull;
     unsigned long long threshold = ~0ull;  // keys >= threshold cannot enter the top k any more
     uint64_t pos = 0;
     bool have = false;
@@ -984,7 +965,8 @@ topk_kernel(const unsigned long long* __restrict__ keys, const float* __restrict
         if (threadIdx.x == 0) fill = base;
         __syncthreads();
         for (uint32_t i = threadIdx.x; i < take; i += blockDim.x) {
-            unsigned long long key = keys[beg + pos + i];
+            const uint32_t j = (uint32_t)pos + i;
+            const unsigned long long key = DENSE ? ((unsigned long long)ordered_key(dists[beg + j]) << 32) | (unsigned long long)j : keys[beg + j];
             if (key < threshold) { uint32_t s = atomicAdd(&fill, 1u); buf[s] = key; }
         }
         pos += take;
@@ -1001,7 +983,7 @@ topk_kernel(const unsigned long long* __restrict__ keys, const float* __restrict
     if (threadIdx.x == 0) out_len[q] = kk;
     for (uint32_t i = threadIdx.x; i < kk; i += blockDim.x) {
         uint32_t p = (uint32_t)(buf[i] & 0xffffffffull);
-        out_rows[(size_t)q * k + i] = rows[beg + p];
+        out_rows[(size_t)q * k + i] = qrows[p];
         out_dist[(size_t)q * k + i] = normalized_distance_dev(metric, dists[beg + p]);
     }
 }

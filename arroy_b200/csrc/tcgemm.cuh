@@ -150,12 +150,13 @@ __device__ __forceinline__ float tg_finish(int mode, float s, float qa, float qb
     return pnqn == pnqn ? 0.0f : pnqn;
 }
 
-// MC = 1: independent CTAs. MC = 2: clusters of two CTAs that work on the same 256 candidates and two
-// neighbouring blocks of 128 queries; each CTA fetches one half of the candidate tile and TMA-multicasts it
-// into both CTAs' shared memory, so the operand traffic L2 -> SM per CTA drops from 48 to 32 KB per stage.
-// A stage is released to both producers by the consumer warpgroups of both CTAs (remote mbarrier arrivals
-// on the `empty` barriers, which therefore count 2 * MC arrivals).
-template <int MC>
+// Clusters of TG_MC = 2 CTAs that work on the same 256 candidates and two neighbouring blocks of 128 queries;
+// each CTA fetches one half of the candidate tile and TMA-multicasts it into both CTAs' shared memory, so the
+// operand traffic L2 -> SM per CTA drops from 48 to 32 KB per stage. A stage is released to both producers by
+// the consumer warpgroups of both CTAs (remote mbarrier arrivals on the `empty` barriers, which therefore count
+// 2 * TG_MC arrivals).
+constexpr int TG_MC = 2;
+
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_c,
                    float* __restrict__ S, uint32_t m, uint32_t nc, uint32_t lds, uint32_t nk, TgEpilogue ep) {
@@ -167,20 +168,20 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     auto empty = [&](int s) { return bars + 8u * (TG_STAGES + s); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t crank = MC > 1 ? cooperative_groups::this_cluster().block_rank() : 0u;
-    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + MC - 1) / MC, num_n = (nc + TG_BN - 1) / TG_BN;   // m-blocks per cluster step
-    const uint32_t tiles = num_mb * num_n, first = blockIdx.x / MC, stride = gridDim.x / MC;
-    auto tile_m0 = [&](uint32_t t) { return ((t % num_mb) * MC + crank) * TG_BM; };   // may lie beyond m: zero rows, nothing stored
+    const uint32_t crank = cooperative_groups::this_cluster().block_rank();
+    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + TG_MC - 1) / TG_MC, num_n = (nc + TG_BN - 1) / TG_BN;   // m-blocks per cluster step
+    const uint32_t tiles = num_mb * num_n, first = blockIdx.x / TG_MC, stride = gridDim.x / TG_MC;
+    auto tile_m0 = [&](uint32_t t) { return ((t % num_mb) * TG_MC + crank) * TG_BM; };   // may lie beyond m: zero rows, nothing stored
     auto tile_n0 = [&](uint32_t t) { return (t / num_mb) * TG_BN; };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TG_STAGES; ++s) { tg_mbar_init(full(s), 1); tg_mbar_init(empty(s), 2 * MC); }
+        for (int s = 0; s < TG_STAGES; ++s) { tg_mbar_init(full(s), 1); tg_mbar_init(empty(s), 2 * TG_MC); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_c) : "memory");
     }
     __syncthreads();
-    if (MC > 1) cooperative_groups::this_cluster().sync();   // the peer's barriers exist before anything is multicast to them
+    cooperative_groups::this_cluster().sync();   // the peer's barriers exist before anything is multicast to them
 
     if (warp < 4) {
         if (threadIdx.x == 0) {
@@ -192,8 +193,7 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                     tg_mbar_expect_tx(full(stage), TG_STAGE_BYTES);
                     const uint32_t sa = base + stage * TG_STAGE_BYTES, sb = sa + TG_A_BYTES;
                     tg_tma_load_2d(sa, &map_q, full(stage), (int)(kb * TG_BK), m0);
-                    if (MC == 1) tg_tma_load_2d(sb, &map_c, full(stage), (int)(kb * TG_BK), n0);
-                    else tg_tma_load_2d_mc(sb + crank * (TG_B_BYTES / MC), &map_c, full(stage), (int)(kb * TG_BK), n0 + (int)(crank * (TG_BN / MC)), (uint16_t)((1u << MC) - 1u));
+                    tg_tma_load_2d_mc(sb + crank * (TG_B_BYTES / TG_MC), &map_c, full(stage), (int)(kb * TG_BK), n0 + (int)(crank * (TG_BN / TG_MC)), (uint16_t)((1u << TG_MC) - 1u));
                     if (++stage == TG_STAGES) { stage = 0; phase ^= 1u; }
                 }
             }
@@ -204,7 +204,7 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         const uint32_t wc = (uint32_t)(lane & 3) * 2u;                 // fragment columns 8 j + wc, + 1
         auto release = [&](int s) {                                    // one arrival per warpgroup on every CTA's barrier
             if ((threadIdx.x & 127u) == 0)
-                for (uint32_t r = 0; r < (uint32_t)MC; ++r) tg_mbar_arrive_cluster(empty(s), r);
+                for (uint32_t r = 0; r < (uint32_t)TG_MC; ++r) tg_mbar_arrive_cluster(empty(s), r);
         };
         int stage = 0; uint32_t phase = 0;
         float acc[TG_BN / 2];
@@ -257,7 +257,7 @@ tcgemm_tf32_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         }
     }
     __syncthreads();
-    if (MC > 1) cooperative_groups::this_cluster().sync();   // no CTA leaves while its peer can still multicast or arrive into it
+    cooperative_groups::this_cluster().sync();   // no CTA leaves while its peer can still multicast or arrive into it
 }
 
 // the same epilogue as a separate pass (used after the cuBLAS cross-check engine)
@@ -299,37 +299,32 @@ inline bool tg_make_map(CUtensorMap* map, const float* ptr, uint64_t rows, uint3
 }
 
 // S[m x nc] (pitch lds, lds % 4 == 0) = Q[m x ld] . C[nc x ld]^T; false if the tensor maps cannot be built
-inline bool tcgemm_tf32(const float* Q, uint32_t m, const float* C, uint32_t nc, uint32_t ld, float* S, uint32_t lds, TgEpilogue ep, int sm_count, cudaStream_t stream, int mc = 2) {
-    if (mc != 1 && mc != 2) mc = 2;
+inline bool tcgemm_tf32(const float* Q, uint32_t m, const float* C, uint32_t nc, uint32_t ld, float* S, uint32_t lds, TgEpilogue ep, int sm_count, cudaStream_t stream) {
     CUtensorMap mq, mcand;
-    if (!tg_make_map(&mq, Q, m, ld, TG_BM) || !tg_make_map(&mcand, C, nc, ld, TG_BN / mc)) return false;
+    if (!tg_make_map(&mq, Q, m, ld, TG_BM) || !tg_make_map(&mcand, C, nc, ld, TG_BN / TG_MC)) return false;
     static bool configured = false;
-    static int max_clusters[3] = {0, 0, 0};   // clusters of 1 / 2 CTAs that can be resident at once (GPCs need not hold an even SM count)
+    static int max_clusters = 0;   // clusters that can be resident at once (GPCs need not hold an even SM count)
     if (!configured) {
-        if (cudaFuncSetAttribute(tcgemm_tf32_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
-        if (cudaFuncSetAttribute(tcgemm_tf32_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
+        if (cudaFuncSetAttribute(tcgemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
         configured = true;
     }
     cudaLaunchConfig_t cfg{};
     cfg.blockDim = dim3(TG_THREADS); cfg.dynamicSmemBytes = TG_SMEM; cfg.stream = stream;
     cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)mc; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = (unsigned)TG_MC; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    if (max_clusters[mc] == 0) {
-        cfg.gridDim = dim3((unsigned)(sm_count / mc * mc));
+    if (max_clusters == 0) {
+        cfg.gridDim = dim3((unsigned)(sm_count / TG_MC * TG_MC));
         int nclu = 0;
-        const cudaError_t oe = mc == 1 ? cudaOccupancyMaxActiveClusters(&nclu, tcgemm_tf32_kernel<1>, &cfg) : cudaOccupancyMaxActiveClusters(&nclu, tcgemm_tf32_kernel<2>, &cfg);
-        if (oe != cudaSuccess || nclu <= 0) return false;
-        max_clusters[mc] = nclu;
+        if (cudaOccupancyMaxActiveClusters(&nclu, tcgemm_tf32_kernel, &cfg) != cudaSuccess || nclu <= 0) return false;
+        max_clusters = nclu;
     }
-    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + mc - 1) / mc;
+    const uint32_t num_mb = ((m + TG_BM - 1) / TG_BM + TG_MC - 1) / TG_MC;
     const uint32_t tiles = num_mb * ((nc + TG_BN - 1) / TG_BN);
-    const uint32_t units = (uint32_t)std::min(sm_count / mc, max_clusters[mc]);
-    cfg.gridDim = dim3((unsigned)((tiles < units ? tiles : units) * mc));
+    const uint32_t units = (uint32_t)std::min(sm_count / TG_MC, max_clusters);
+    cfg.gridDim = dim3((unsigned)((tiles < units ? tiles : units) * TG_MC));
     const uint32_t nk = ld / TG_BK;
-    cudaError_t e = mc == 1 ? cudaLaunchKernelEx(&cfg, tcgemm_tf32_kernel<1>, mq, mcand, S, m, nc, lds, nk, ep)
-                            : cudaLaunchKernelEx(&cfg, tcgemm_tf32_kernel<2>, mq, mcand, S, m, nc, lds, nk, ep);
-    return e == cudaSuccess;
+    return cudaLaunchKernelEx(&cfg, tcgemm_tf32_kernel, mq, mcand, S, m, nc, lds, nk, ep) == cudaSuccess;
 }
 
 }  // namespace ab

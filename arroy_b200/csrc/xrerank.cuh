@@ -159,48 +159,6 @@ xrerank_kernel(const float* __restrict__ items, const float* __restrict__ ih0, u
     }
 }
 
-// top-k per query straight from a dense distance row: key = ordered_key(dist) << 32 | position
-__global__ void __launch_bounds__(TOPK_THREADS)
-topk_dense_kernel(const float* __restrict__ dist, const uint32_t* __restrict__ rows, uint32_t nc, uint32_t k, int metric,
-                  uint32_t* __restrict__ out_rows, float* __restrict__ out_dist, uint32_t* __restrict__ out_len) {
-    __shared__ unsigned long long buf[TOPK_CAP];
-    __shared__ uint32_t fill;
-    const uint32_t q = blockIdx.x;
-    const float* dq = dist + (size_t)q * nc;
-    const uint32_t kk = nc < k ? nc : k;
-    unsigned long long threshold = ~0ull;
-    uint32_t pos = 0;
-    bool have = false;
-    while (pos < nc) {
-        const uint32_t base = have ? kk : 0u;
-        const uint32_t room = TOPK_CAP - base;
-        const uint32_t take = nc - pos < room ? nc - pos : room;
-        __syncthreads();
-        if (threadIdx.x == 0) fill = base;
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < take; i += blockDim.x) {
-            unsigned long long key = ((unsigned long long)ordered_key(dq[pos + i]) << 32) | (unsigned long long)(pos + i);
-            if (key < threshold) { uint32_t s = atomicAdd(&fill, 1u); buf[s] = key; }
-        }
-        pos += take;
-        __syncthreads();
-        const uint32_t f = fill;
-        int mm = 2;
-        while ((uint32_t)mm < f) mm <<= 1;
-        for (int i = (int)f + threadIdx.x; i < mm; i += blockDim.x) buf[i] = ~0ull;
-        bitonic_sort_shared(buf, mm);
-        have = true;
-        threshold = (f >= kk && kk > 0) ? buf[kk - 1] : ~0ull;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) out_len[q] = kk;
-    for (uint32_t i = threadIdx.x; i < kk; i += blockDim.x) {
-        uint32_t p = (uint32_t)(buf[i] & 0xffffffffull);
-        out_rows[(size_t)q * k + i] = rows[p];
-        out_dist[(size_t)q * k + i] = normalized_distance_dev(metric, dq[p]);
-    }
-}
-
 // =================================================================================================
 // Tensor-core pre-filter for the shared-candidate re-rank (SURVEY.md §8a row 9: "tensor-core
 // pre-filter + exact AVX-order re-score of the top-(k + margin)").
@@ -290,80 +248,6 @@ __global__ void xf_query_prep_kernel(const float* __restrict__ qnorm, const floa
     two_e[q] = __fmul_rn(__fmul_rn(2.0f, e), 1.0009765625f);
 }
 
-// monotone float -> uint32 key for finite estimates; NaN / infinite estimates are "unknown" = max
-__device__ __forceinline__ uint32_t xf_key(float a) {
-    const uint32_t b = __float_as_uint(a);
-    return fabsf(a) <= 3.0e38f ? (b ^ ((b & 0x80000000u) ? 0xffffffffu : 0x80000000u)) : 0xffffffffu;
-}
-__device__ __forceinline__ float xf_unkey(uint32_t k) {   // inverse of xf_key for finite values
-    return __uint_as_float(k ^ ((k & 0x80000000u) ? 0x80000000u : 0xffffffffu));
-}
-__device__ __forceinline__ bool xf_unknown(float a) { return !(fabsf(a) <= 3.0e38f); }
-__device__ __forceinline__ uint32_t xf_widen(uint32_t key, float two_e) {   // key of (value + 2E), max if not finite
-    if (key == 0xffffffffu) return key;
-    return xf_key(__fadd_rn(xf_unkey(key), two_e));
-}
-
-// exclusive scan of one value per thread over the CTA (XF_THREADS threads); returns the exclusive
-// prefix, *total = sum. sm: 17 uint32.
-__device__ __forceinline__ uint32_t xf_block_scan(uint32_t v, uint32_t* sm, uint32_t* total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    __syncthreads();
-    if (lane == 31) sm[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t w = lane < (XF_THREADS / 32) ? sm[lane] : 0u, winc = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += t; }
-        if (lane < (XF_THREADS / 32)) sm[lane] = winc - w;
-        if (lane == 31) sm[16] = winc;
-    }
-    __syncthreads();
-    const uint32_t res = sm[warp] + inc - v;
-    *total = sm[16];
-    return res;
-}
-
-// smallest bin b with (number of entries in bins <= b) >= want; *before = entries in bins < b
-__device__ __forceinline__ uint32_t xf_find_bin(const uint32_t* hist, uint32_t want, uint32_t* sm, uint32_t* sh_out /* 2 uint32 */, uint32_t* before) {
-    constexpr int PER = XF_BINS / XF_THREADS;
-    uint32_t local = 0;
-#pragma unroll
-    for (int i = 0; i < PER; ++i) local += hist[threadIdx.x * PER + i];
-    uint32_t total;
-    uint32_t ex = xf_block_scan(local, sm, &total);
-    if (threadIdx.x == 0) { sh_out[0] = XF_BINS - 1; sh_out[1] = total; }   // fewer than `want` entries: last bin
-    __syncthreads();
-    if (ex < want && ex + local >= want) {
-        uint32_t cum = ex;
-        for (int i = 0; i < PER; ++i) {
-            uint32_t h = hist[threadIdx.x * PER + i];
-            if (cum + h >= want) { sh_out[0] = threadIdx.x * PER + i; sh_out[1] = cum; break; }
-            cum += h;
-        }
-    }
-    __syncthreads();
-    *before = sh_out[1];
-    return sh_out[0];
-}
-
-__device__ __forceinline__ void xf_bitonic_u32(uint32_t* buf, int n /* power of two */) {
-    for (int size = 2; size <= n; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            __syncthreads();
-            for (int t = threadIdx.x; t < (n >> 1); t += XF_THREADS) {
-                int i = 2 * t - (t & (stride - 1)), j = i + stride;
-                bool up = ((i & size) == 0);
-                uint32_t a = buf[i], b = buf[j];
-                if ((a > b) == up) { buf[i] = b; buf[j] = a; }
-            }
-        }
-    __syncthreads();
-}
-
 // One CTA per query, over the query's row of estimates A[q][0..nc).
 //  1. t0: a loose upper bound of the k-th smallest estimate, from a sample (every 4th group of 32
 //     candidates): the r-th smallest sample key, r = k p + 4 sqrt(k p) + 4 (p = sample fraction),
@@ -379,7 +263,7 @@ xf_select_kernel(const float* __restrict__ A, uint32_t lds, uint32_t nc, uint32_
                  uint32_t* __restrict__ sel_rows, uint64_t* __restrict__ seg_beg, uint64_t* __restrict__ seg_end, int* __restrict__ overflow) {
     __shared__ uint32_t u_mem[XF_BINS];               // histogram, later sort buffers
     __shared__ uint32_t st_key[XF_STAGE], st_pos[XF_STAGE];
-    __shared__ uint32_t sm_scan[17];
+    __shared__ uint32_t sm_scan[XF_THREADS / 32];
     __shared__ uint32_t sh_out[2];
     __shared__ uint32_t sh_min, sh_max, sh_ns, sh_cnt, sh_nlow, sh_cnt2;
     const uint32_t q = blockIdx.x;
@@ -404,7 +288,7 @@ xf_select_kernel(const float* __restrict__ A, uint32_t lds, uint32_t nc, uint32_
         if (lane == 0) { atomicMin(&sh_min, mn); atomicMax(&sh_max, mx); atomicAdd(&sh_ns, cnt); }
         __syncthreads();
         const uint32_t ns = sh_ns;
-        uint32_t rlo = sh_min, rhi = sh_max;
+        const uint32_t rlo = sh_min, rhi = sh_max;
         uint32_t want;
         if (sf == 1u) want = k;
         else {
@@ -412,30 +296,12 @@ xf_select_kernel(const float* __restrict__ A, uint32_t lds, uint32_t nc, uint32_
             want = (uint32_t)(mean + 4.0f * sqrtf(mean) + 4.0f) + 1u;
         }
         if (want > ns) want = ns;
-        for (int level = 0; level < 3 && rhi > rlo; ++level) {
-            for (int i = threadIdx.x; i < XF_BINS; i += XF_THREADS) u_mem[i] = 0;
-            __syncthreads();
-            // bin = (key - rlo) >> shift with the smallest shift that keeps every key of the range below XF_BINS
-            const uint32_t span = rhi - rlo;
-            const int shift = span < XF_BINS ? 0 : (32 - __clz(span)) - 12;
+        t0 = hist_narrow<XF_THREADS, XF_BINS>(rlo, rhi, want, 32u, [&](auto add) {
             for (uint32_t j = warp; j < sgroups; j += XF_THREADS / 32) {
                 const uint32_t c = j * sf * 32u + lane;
-                if (c < nc) {
-                    const uint32_t key = xf_key(a[c]);
-                    if (key >= rlo && key <= rhi) atomicAdd(&u_mem[(key - rlo) >> shift], 1u);
-                }
+                if (c < nc) add(xf_key(a[c]));
             }
-            __syncthreads();
-            uint32_t before;
-            const uint32_t b = xf_find_bin(u_mem, want, sm_scan, sh_out, &before);
-            const uint32_t in_bin = u_mem[b];
-            __syncthreads();
-            const uint32_t nlo = rlo + (b << shift);
-            const uint32_t top = (uint32_t)min((unsigned long long)rhi, (unsigned long long)rlo + (((unsigned long long)b + 1ull) << shift) - 1ull);
-            want -= before; rlo = nlo; rhi = top;
-            if (in_bin <= 32u || shift == 0) break;
-        }
-        t0 = rhi;
+        }, u_mem, sm_scan, sh_out);
     }
     const bool all = t0 == 0xffffffffu;
     const float t0f = all ? 0.f : xf_unkey(t0);
@@ -470,7 +336,7 @@ xf_select_kernel(const float* __restrict__ A, uint32_t lds, uint32_t nc, uint32_
         int np2 = 2;
         while ((uint32_t)np2 < staged) np2 <<= 1;
         for (int i = threadIdx.x; i < np2; i += XF_THREADS) u_mem[i] = (uint32_t)i < staged ? st_key[i] : 0xffffffffu;
-        xf_bitonic_u32(u_mem, np2);
+        bitonic_sort_shared(u_mem, np2);
         T1 = xf_widen(u_mem[k - 1], two_e);
         __syncthreads();
     }
@@ -481,7 +347,7 @@ xf_select_kernel(const float* __restrict__ A, uint32_t lds, uint32_t nc, uint32_
     int kp2 = 2;
     while ((uint32_t)kp2 < keep) kp2 <<= 1;
     for (int i = keep + threadIdx.x; i < kp2; i += XF_THREADS) u_mem[i] = 0xffffffffu;
-    xf_bitonic_u32(u_mem, kp2);                       // back to candidate order (ties are broken by id)
+    bitonic_sort_shared(u_mem, kp2);                       // back to candidate order (ties are broken by id)
     uint32_t* out = sel_rows + (size_t)q * cap;
     for (uint32_t i = threadIdx.x; i < keep && i < cap; i += XF_THREADS) out[i] = rows[u_mem[i]];
     if (threadIdx.x == 0) {

@@ -94,7 +94,7 @@ def test_prefilter_nan_and_inf_inputs(ctx, monkeypatch):
 
 
 @pytest.mark.parametrize("d,nq,nc", [(768, 300, 5001), (33, 7, 258), (100, 129, 1000), (64, 1, 40)])
-def test_tensor_core_scores_are_within_the_bound(ctx, monkeypatch, d, nq, nc):
+def test_tensor_core_scores_are_within_the_bound(ctx, d, nq, nc):
     # the bound the whole pre-filter rests on: |S - q.c| <= 2^-8 |q| |c|, for the hand-written wgmma
     # kernel (engine 0, single-CTA and 2-CTA multicast variants) and optionally for cuBLAS (engine 1); ragged tile
     # edges in both directions
@@ -107,10 +107,8 @@ def test_tensor_core_scores_are_within_the_bound(ctx, monkeypatch, d, nq, nc):
     for rows in (np.arange(10, 10 + nc, dtype=np.uint32), np.sort(np.random.default_rng(1).choice(n, nc, replace=False)).astype(np.uint32)):
         exact = q.astype(np.float64) @ data[rows].astype(np.float64).T
         bound = np.linalg.norm(q.astype(np.float64), axis=1)[:, None] * np.linalg.norm(data[rows].astype(np.float64), axis=1)[None, :] / 256.0
-        for mc in ("1", "2"):
-            monkeypatch.setenv("ARROY_B200_XGEMM_MC", mc)
-            own = ctx.prefilter_scores(q, rows, engine=0)
-            assert np.all(np.abs(own - exact) <= bound), (mc, float(np.max(np.abs(own - exact) / bound)))
+        own = ctx.prefilter_scores(q, rows, engine=0)
+        assert np.all(np.abs(own - exact) <= bound), float(np.max(np.abs(own - exact) / bound))
         if CUBLAS:
             lib = ctx.prefilter_scores(q, rows, engine=1)
             assert np.all(np.abs(lib - exact) <= bound)
@@ -140,7 +138,7 @@ def _tf32_rows(signs, exps, low):
     return (signs * bits.astype(np.uint32).view(np.float32)).astype(np.float32)
 
 
-def test_tensor_core_scores_at_worst_case_rounding(ctx, monkeypatch, capsys):
+def test_tensor_core_scores_at_worst_case_rounding(ctx, capsys):
     # both operands just below a TF32 midpoint, with the rows' signs taken from the query: every element of the pair loses
     # 2^-11 of itself in the same direction, ~2^-10 |q| |c| in all, a quarter of the bound 2^-8 |q| |c|. The truncation pattern
     # reports which conversion wgmma does: ~0.5 of the bound if it truncates, ~0 if it rounds.
@@ -157,16 +155,14 @@ def test_tensor_core_scores_at_worst_case_rounding(ctx, monkeypatch, capsys):
         rows = np.arange(n, dtype=np.uint32)
         exact = q.astype(np.float64) @ rows_v.astype(np.float64).T
         bound = np.linalg.norm(q.astype(np.float64), axis=1)[:, None] * np.linalg.norm(rows_v.astype(np.float64), axis=1)[None, :] / 256.0
-        for mc in ("1", "2"):
-            monkeypatch.setenv("ARROY_B200_XGEMM_MC", mc)
-            own = ctx.prefilter_scores(q, rows, engine=0)
-            ratio = np.abs(own - exact) / bound
-            assert np.all(ratio <= 1.0), (d, mc, float(ratio.max()))
-            matched = ratio[np.arange(nq), np.arange(nq)]                  # query j against its own row j
-            assert matched[: nq // 2].min() >= 0.2, (d, mc, matched[: nq // 2])
-            with capsys.disabled():
-                print("\nTF32 scores d=%d mc=%s: midpoint rows %.3f of the bound, all-ones low bits %.3f (0.5: truncation, ~0: rounding)"
-                      % (d, mc, float(matched[: nq // 2].min()), float(matched[nq // 2:].max())))
+        own = ctx.prefilter_scores(q, rows, engine=0)
+        ratio = np.abs(own - exact) / bound
+        assert np.all(ratio <= 1.0), (d, float(ratio.max()))
+        matched = ratio[np.arange(nq), np.arange(nq)]                  # query j against its own row j
+        assert matched[: nq // 2].min() >= 0.2, (d, matched[: nq // 2])
+        with capsys.disabled():
+            print("\nTF32 scores d=%d: midpoint rows %.3f of the bound, all-ones low bits %.3f (0.5: truncation, ~0: rounding)"
+                  % (d, float(matched[: nq // 2].min()), float(matched[nq // 2:].max())))
 
 
 def _tf32_matrix(kind, metric, d, n_random=800):   # fewer candidates than the 1024 survivors a query may keep
@@ -202,7 +198,7 @@ def test_prefilter_on_adversarial_rows(ctx, monkeypatch, metric, d):
                 assert out_rows[i, :out_len[i]].tolist() == wr.tolist() and out_dist[i, :out_len[i]].tobytes() == wd.tobytes(), (kind, k, i)
 
 
-def test_tensor_core_scores_of_tiny_rows(ctx, monkeypatch, capsys):
+def test_tensor_core_scores_of_tiny_rows(ctx, capsys):
     # subnormal rows and rows whose squared norm underflows, against a large query: the scores must stay within the bound the
     # pre-filter charges, 2^-8 (|q| + sub) (|c| + sub) + 1e-30 with sub = sqrt(d + 64) 2^-74 (xf_query_prep_kernel), whether
     # the conversion keeps subnormal operands or flushes them (reported)
@@ -218,10 +214,8 @@ def test_tensor_core_scores_of_tiny_rows(ctx, monkeypatch, capsys):
         qn = np.linalg.norm(queries.astype(np.float64), axis=1)[:, None]
         cn = np.linalg.norm(rows_v.astype(np.float64), axis=1)[None, :]
         bound = (2.0 ** -8 + d * 2.0 ** -22) * (qn + sub) * (cn + sub) + 1e-30
-        for mc in ("1", "2"):
-            monkeypatch.setenv("ARROY_B200_XGEMM_MC", mc)
-            own = ctx.prefilter_scores(queries, np.arange(n, dtype=np.uint32), engine=0)
-            assert np.all(np.abs(own - exact) <= bound), (d, mc)
-            rel = np.abs(own[:, :adv.shape[0]] - exact[:, :adv.shape[0]]) / np.abs(exact[:, :adv.shape[0]])
-            with capsys.disabled():
-                print("\nTF32 scores of subnormal rows d=%d mc=%s: relative error up to %.3g (1: flushed to zero)" % (d, mc, float(rel.max())))
+        own = ctx.prefilter_scores(queries, np.arange(n, dtype=np.uint32), engine=0)
+        assert np.all(np.abs(own - exact) <= bound), d
+        rel = np.abs(own[:, :adv.shape[0]] - exact[:, :adv.shape[0]]) / np.abs(exact[:, :adv.shape[0]])
+        with capsys.disabled():
+            print("\nTF32 scores of subnormal rows d=%d: relative error up to %.3g (1: flushed to zero)" % (d, float(rel.max())))
