@@ -390,7 +390,7 @@ class Context:
 
     def build_prefilter_stats(self):
         """Rows of the last build through each stage of side()'s 8-bit pre-filter: all of them read the hi plane (d bytes), the
-        stage-1 leftovers read both planes, the stage-2 leftovers the f32 row."""
+        stage-1 leftovers read the lo plane, the stage-2 leftovers the f32 row."""
         out = (C.c_uint64 * 5)()
         self._ck(self.lib.arroy_b200_build_prefilter_stats(self.h, out))
         return {"rows_via_prefilter": int(out[0]), "rows_stage2": int(out[1]), "rows_rescored_f32": int(out[2]),

@@ -641,7 +641,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     // from start to end (10M x 100 trees) runs a little faster on work_kernel's three scanning CTAs per SM.
     if ((double)n * (double)tw <= 2.0e8 && !lockstep && use_smem && ld <= 8u * CTRL_THREADS && n < (1ull << 29)) {
         ctrlp = control_fn(true, 0, c->metric);
-        const size_t cand[2] = {ctrl_smem, (size_t)WS_VECS * ld * 4};
+        const size_t cand[2] = {persistent_smem(ctrl_smem, ld), persistent_smem((size_t)WS_VECS * ld * 4, ld)};
         for (int k = 0; k < 2 && !persist; ++k) {
             if (k == 1 && !P.spec) break;
             CK(cudaFuncSetAttribute(ctrlp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand[k]));

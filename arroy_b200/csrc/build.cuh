@@ -971,20 +971,23 @@ __device__ __noinline__ void proot(const BuildParams& P, float* smN) {
 // Returns when every tree is done (or on error). sm_normal: ld floats of dynamic shared memory.
 // BQ: the items are bit-string rows, the loaded normal's first words of sm_normal hold its bit string and the scans are
 // bq_scan_unit's (no fused root pass, no pre-filter planes).
-static_assert(sizeof(PlanesClaimRows) <= (WS_VECS - 2) * 4 * 64, "pworker: the claim rows fit behind the normal and its limbs at ld = 64");
+// The persistent kernel's dynamic shared memory around a two_means workspace of ws_bytes: a worker keeps the normal, its limbs
+// and its claim's rows there (pworker), 8 ld + 7 KB bytes: more than the workspace only at the smallest widths (ld = 64 with
+// the speculative two_means).
+inline size_t persistent_smem(size_t ws_bytes, uint32_t ld) { return std::max(ws_bytes, (size_t)8 * ld + sizeof(PlanesClaimRows)); }
 template <bool BQ>
 __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
     __shared__ uint32_t w_t, w_u0, w_n, w_seq, w_pseq, w_found, w_exit, w_count;
     __shared__ PSlot w_job;        // fields of the claimed job (first 64 bytes)
     __shared__ uint32_t w_sm[16];
-    __shared__ uint32_t w_list[SCAN_UNIT * PLANES_CHUNK], w_list2[SCAN_UNIT * PLANES_CHUNK];   // positions stage 1 / stage 2 could not decide
+    __shared__ uint32_t w_list2[SCAN_UNIT * PLANES_CHUNK];   // positions stage 2 could not decide
     __shared__ uint32_t w_cnt[PLANES_CHUNK + 2];
     __shared__ PlanesScratch w_sc;
     __shared__ PlanesNormal w_pn;                           // the loaded normal's pre-filter factors (scan_claim_planes)
     uint8_t* sm_limbs = reinterpret_cast<uint8_t*>(sm_normal + P.ld);   // and its limbs
-    // the claim's row ids, scales and headers (scan_claim_planes), after the limbs: the workspace this kernel is launched with
-    // (at least WS_VECS * ld floats) holds 2 ld floats + 3 KB whenever the planes are used (ld >= 64); kept out of static
-    // shared memory, which every control CTA pays for next to its two_means workspace
+    // the claim's row ids, scales, headers and the rows stage 1 leaves (scan_claim_planes), after the limbs: in the launch's
+    // dynamic shared memory (persistent_smem), not in static shared memory, which every control CTA pays for next to its
+    // two_means workspace
     PlanesClaimRows& w_cr = *reinterpret_cast<PlanesClaimRows*>(sm_normal + 2u * P.ld);
     const uint32_t T = P.n_trees;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1111,7 +1114,7 @@ __device__ __noinline__ void pworker(const BuildParams& P, float* sm_normal) {
                     if (P.planes.hi != nullptr && units > P.shadow_min_units)
                         for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); u += PLANES_CHUNK)
                             scan_claim_planes(jb, u, min(min(units, (g0 + 1u) * chunk), u + PLANES_CHUNK), P.items, P.planes, P.ih0, P.d, P.ld, P.metric, sm_normal, sm_limbs,
-                                              &w_pn, nh0, w_list, w_list2, w_cnt, w_cr, P.shadow_stats);
+                                              &w_pn, nh0, w_list2, w_cnt, w_cr, P.shadow_stats);
                     else
                         for (uint32_t u = g0 * chunk; u < min(units, (g0 + 1u) * chunk); ++u) scan_unit<true>(jb, u, P.items, P.ih0, P.d, P.ld, P.metric, sm_normal, nh0, &w_count);
                 }

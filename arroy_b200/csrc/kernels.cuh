@@ -170,7 +170,7 @@ __device__ __forceinline__ void scan_unit(const Job& jb, uint32_t unit, const fl
 //    The row is certain when |p + c| > s w1 + wa in f64, p = fl(fl(T1 s) k1), k1 = fl(sigma / 254), w1 = (N1 (E1 + 127.001
 //    gamma_R) + 127 D1) (1 + 2^-20) rounded up: the factor 1 + 2^-20 covers the relative errors of p (3 roundings on
 //    |p| <= 254 s N1) and of the test (2^-53 each; s w1 and wa are both positive, so the sum's rounding is relative too).
-//  stage 2, the rows stage 1 left (both planes; the hi row was just streamed by this CTA): y_i = 254 h_i + l_i (|y_i| <= 32385),
+//  stage 2, the rows stage 1 left (lo plane only: stage 1 kept their hi-plane sums): y_i = 254 h_i + l_i (|y_i| <= 32385),
 //    T2 = sum y_i (254^2 a_i + 254 b_i + c_i) from the six int32 sums of h, l times a, b, c (|T2| <= 2.2e15 < 2^53: exact in f64),
 //    so s sigma T2 / 254^3 = (s / 254) sum y_i n2_i, and with A = 254 sum |h_i| U_i + sum |l_i| U_i (sum |n_i| |y_i| <= sigma A / 2):
 //    |dot - (s/254) sum y_i n2_i| <= s E2 N1 + (s/254) 32385 D2 + gamma_R ((s/254) sigma A / 2 + s E2 N1) + wa
@@ -333,55 +333,67 @@ __device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(__cvta_generic_to_global(p)), "r"(bytes));
 }
 
-// What scan_claim_planes needs of each row of its claim, fetched once in its prologue (position base + i at index i; zeros past
-// the claim's end).
+// A row stage 1 of scan_claim_planes leaves to stage 2: its position and its hi-plane sums over the whole row,
+// mh = 254^3 sum h a + 254^2 sum h b + 254 sum h c (|mh| < 2^51) and hu = sum |h| U (< 2^32).
+struct __align__(16) PlanesLeft {
+    long long mh;
+    uint32_t hu, pos;
+};
+
+// What scan_claim_planes keeps of the rows of its claim (position base + i at index i): the ids, fetched once in its prologue
+// (zeros past the claim's end), and for the rows stage 1 leaves (the first sm_cnt[PLANES_CHUNK] entries of left) their scales
+// and headers.
 constexpr uint32_t PLANES_CLAIM_ROWS = SCAN_UNIT * PLANES_CHUNK;
 struct PlanesClaimRows {
     uint32_t rid[PLANES_CLAIM_ROWS];   // row ids
-    float scale[PLANES_CLAIM_ROWS];    // the rows' plane scales
-    float ih0[PLANES_CLAIM_ROWS];      // DotProduct: the rows' h0 (the other metrics: unused)
+    float scale[PLANES_CLAIM_ROWS];    // the plane scales of the rows stage 1 leaves
+    float ih0[PLANES_CLAIM_ROWS];      // DotProduct: their h0 (the other metrics: 0)
+    PlanesLeft left[PLANES_CLAIM_ROWS];
 };
 
-// scan units [u0, u1) (at most PLANES_CHUNK) of a job. sm_list, sm_list2: 64 * PLANES_CHUNK positions each (the rows stage 1,
-// stage 2 left); sm_cnt: PLANES_CHUNK + 2 counters. limbs, pn: the job's normal as planes_job_factors left it. stats (optional):
-// [0] rows through the pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
+// scan units [u0, u1) (at most PLANES_CHUNK) of a job. sm_list2: 64 * PLANES_CHUNK positions (the rows stage 2 left); sm_cnt:
+// PLANES_CHUNK + 2 counters. limbs, pn: the job's normal as planes_job_factors left it. stats (optional): [0] rows through the
+// pre-filter, [1] of them re-scored from the f32 row, [2] of them that went through stage 2.
 // Every read of a plane row is a device read (the planes never live in host memory), so their L2 prefetches are safe.
 __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, uint32_t u1, const float* __restrict__ items, const PlaneRows pl,
                                                   const float* __restrict__ ih0, uint32_t d, uint32_t ld, int metric, const float* sm_normal, const uint8_t* limbs,
-                                                  const PlanesNormal* pn, float nh0, uint32_t* sm_list, uint32_t* sm_list2, uint32_t* sm_cnt,
+                                                  const PlanesNormal* pn, float nh0, uint32_t* sm_list2, uint32_t* sm_cnt,
                                                   PlanesClaimRows& cr, unsigned long long* stats) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g8 = lane & 7, grp = lane >> 3;
     const uint32_t base = u0 * SCAN_UNIT, end = min(jb.len, u1 * SCAN_UNIT);
-    // ---- prologue: one round for the claim's row ids, one for their scales (and headers); the hi rows of the first 128
-    // positions start towards L2 as soon as their ids are known ----
+    // ---- prologue: one round for the claim's row ids; the hi rows of the first 128 positions start towards L2 as soon as
+    // their ids are known (the rows' scales and headers are loaded in stage 1, beside its hi-plane loads) ----
     if (tid <= (int)PLANES_CHUNK + 1) sm_cnt[tid] = 0;
     for (uint32_t i = tid; i < PLANES_CLAIM_ROWS; i += blockDim.x) {
         const bool v = base + i < end;
         const uint32_t r = v ? (jb.rows ? __ldcg(jb.rows + base + i) : base + i) : 0u;
         if (v && i < 128u) prefetch_l2(pl.hi + (size_t)r * ld, ld);
         cr.rid[i] = r;
-        cr.scale[i] = v ? __ldg(pl.scale + r) : 0.f;
-        cr.ih0[i] = (v && metric == DOT_PRODUCT) ? ih0[r] : 0.f;
     }
     __syncthreads();
     const uint32_t nq = ld >> 4;                       // 16-byte words per plane row
     const int nsteps = (int)((nq + 7) >> 3);
     const uint4* LA = reinterpret_cast<const uint4*>(limbs);
     const uint4* LB = LA + nq;
-    // ---- stage 1: the hi plane of every row; the next block's hi rows are prefetched into L2 while this block's are read ----
+    const uint4* LC = LB + nq;
+    const uint4* LU = LC + nq;
+    // ---- stage 1: the hi plane of every row, and with it every hi-plane sum stage 2 needs (kept for the rows it leaves); the
+    // next block's hi rows are prefetched into L2 while this block's are read ----
     for (uint32_t pbase = base; pbase < end; pbase += 128) {
         if (tid < 128 && pbase + 128u + tid < end) prefetch_l2(pl.hi + (size_t)cr.rid[pbase + 128u - base + tid] * ld, ld);
-        uint32_t pos[4], rid[4];
         const uint4* S[4];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            pos[r] = pbase + warp * 16 + grp * 4 + r;
-            rid[r] = cr.rid[pos[r] - base];
-            S[r] = reinterpret_cast<const uint4*>(pl.hi + (size_t)rid[r] * ld) + g8;
-        }
-        int sa[4], sb[4];
+        for (int r = 0; r < 4; ++r) S[r] = reinterpret_cast<const uint4*>(pl.hi + (size_t)cr.rid[pbase + warp * 16 + grp * 4 + r - base] * ld) + g8;
+        // the row this lane decides once its group's sums are reduced (below): row 2 b2 + b1 of the group's four, for the lane
+        // bits b2 b1 b0 of g8; its scale and header are in flight while the hi rows stream
+        const uint32_t pos = pbase + warp * 16 + grp * 4 + (uint32_t)(g8 >> 1), rid = cr.rid[pos - base];
+        const bool valid = pos < end;
+        const float s = valid ? __ldg(pl.scale + rid) : 0.f;
+        const float h0 = (valid && metric == DOT_PRODUCT) ? ih0[rid] : 0.f;
+        int sa[4], sb[4], hc[4];
+        uint32_t hu[4];
 #pragma unroll
-        for (int r = 0; r < 4; ++r) { sa[r] = 0; sb[r] = 0; }
+        for (int r = 0; r < 4; ++r) { sa[r] = 0; sb[r] = 0; hc[r] = 0; hu[r] = 0; }
         for (int c0 = 0; c0 < nsteps; c0 += 3) {
             uint4 v[3][4];
 #pragma unroll
@@ -394,71 +406,92 @@ __device__ __forceinline__ void scan_claim_planes(const Job& jb, uint32_t u0, ui
 #pragma unroll
             for (int sidx = 0; sidx < 3; ++sidx) {
                 const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                const uint4 la = q < nq ? LA[q] : make_uint4(0u, 0u, 0u, 0u), lb = q < nq ? LB[q] : make_uint4(0u, 0u, 0u, 0u);
+                const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+                const uint4 la = q < nq ? LA[q] : z, lb = q < nq ? LB[q] : z, lc = q < nq ? LC[q] : z, lu = q < nq ? LU[q] : z;
 #pragma unroll
-                for (int r = 0; r < 4; ++r) { sa[r] = dp16(v[sidx][r], la, sa[r]); sb[r] = dp16(v[sidx][r], lb, sb[r]); }
-            }
-        }
-        const double w1 = pn->w1, k1 = pn->k1, wa = pn->wa;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-#pragma unroll
-            for (int o = 1; o < 8; o <<= 1) { sa[r] += __shfl_xor_sync(0xffffffffu, sa[r], o); sb[r] += __shfl_xor_sync(0xffffffffu, sb[r], o); }
-            const bool valid = pos[r] < end;
-            const float s = cr.scale[pos[r] - base];
-            const double t1 = (double)(254ll * sa[r] + sb[r]);
-            const double mt = __dadd_rn(__dmul_rn(__dmul_rn(t1, (double)s), k1), prefilter_c(metric, nh0, cr.ih0[pos[r] - base]));
-            const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, w1), wa);      // false for NaN / Inf scales and NaN factors
-            const bool leader = g8 == 0 && valid;
-            const int side = mt > 0.0 ? 1 : 0;
-            if (leader && certain) jb.flags[pos[r]] = (uint8_t)side;
-            if (leader && !certain) {   // stage 2 reads this row's lo plane from L2
-                sm_list[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = pos[r];
-                prefetch_l2(pl.lo + (size_t)rid[r] * ld, ld);
-            }
-            const unsigned lefts = __ballot_sync(0xffffffffu, leader && certain && side == 0);
-            // the four groups of a warp hold positions of the same unit (16 consecutive positions per warp)
-            if (lane == 0 && lefts) atomicAdd(&sm_cnt[(pbase + warp * 16 - base) / SCAN_UNIT], (uint32_t)__popc(lefts));
-        }
-    }
-    __syncthreads();
-    // ---- stage 2: both planes of the rows stage 1 left, one 8-lane group per row ----
-    const uint32_t n1 = sm_cnt[PLANES_CHUNK];
-    const uint4* LC = LB + nq;
-    const uint4* LU = LC + nq;
-    for (uint32_t it = 0; it * 32u < n1; ++it) {
-        const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
-        const bool act = idx < n1;
-        const uint32_t p = act ? sm_list[idx] : base;
-        const uint32_t r = cr.rid[p - base];
-        const uint4* Hr = reinterpret_cast<const uint4*>(pl.hi + (size_t)r * ld) + g8;
-        const uint4* Lr = reinterpret_cast<const uint4*>(pl.lo + (size_t)r * ld) + g8;
-        int ha = 0, hb = 0, hc = 0, la = 0, lb = 0, lc = 0;
-        uint32_t hu = 0, lu = 0;
-        for (int c0 = 0; c0 < nsteps; c0 += 3) {
-            uint4 vh[3], vl[3];
-#pragma unroll
-            for (int sidx = 0; sidx < 3; ++sidx) {
-                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                vh[sidx] = q < nq ? ldg_stream_u4(Hr + (c0 + sidx) * 8) : make_uint4(0u, 0u, 0u, 0u);
-                vl[sidx] = q < nq ? ldg_stream_u4(Lr + (c0 + sidx) * 8) : make_uint4(0u, 0u, 0u, 0u);
-            }
-#pragma unroll
-            for (int sidx = 0; sidx < 3; ++sidx) {
-                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
-                if (q < nq) {   // the rows' words past nq were loaded as zeros
-                    const uint4 na = LA[q], nb = LB[q], nc = LC[q], nu = LU[q];
-                    ha = dp16(vh[sidx], na, ha); hb = dp16(vh[sidx], nb, hb); hc = dp16(vh[sidx], nc, hc);
-                    la = dp16(vl[sidx], na, la); lb = dp16(vl[sidx], nb, lb); lc = dp16(vl[sidx], nc, lc);
-                    hu = dp16u(abs_bytes(vh[sidx]), nu, hu); lu = dp16u(abs_bytes(vl[sidx]), nu, lu);
+                for (int r = 0; r < 4; ++r) {
+                    sa[r] = dp16(v[sidx][r], la, sa[r]); sb[r] = dp16(v[sidx][r], lb, sb[r]); hc[r] = dp16(v[sidx][r], lc, hc[r]);
+                    hu[r] = dp16u(abs_bytes(v[sidx][r]), lu, hu[r]);
                 }
             }
         }
-        // this lane's share of T2 and A: integers below 2^53, so the doubles and their butterfly are exact
-        double m = (double)(16387064ll * ha + 64516ll * (hb + la) + 254ll * (hc + lb) + lc);
-        double a = (double)(254ull * hu + lu);
+        // reduce the 16 sums (4 rows x sa, sb, hc, hu) over the group by halving: lanes b2 = 0 keep rows 0, 1 and b2 = 1 rows 2, 3
+        // (xor 4), then b1 picks one of the two (xor 2), and the lane pair b0 = 0, 1 sums its row's four (xor 1): 16 shuffles
+        int x[2][4];
 #pragma unroll
-        for (int o = 1; o < 8; o <<= 1) { m += __shfl_xor_sync(0xffffffffu, m, o); a += __shfl_xor_sync(0xffffffffu, a, o); }
+        for (int j = 0; j < 2; ++j) {
+            const int lo4[4] = {sa[j], sb[j], hc[j], (int)hu[j]}, hi4[4] = {sa[j + 2], sb[j + 2], hc[j + 2], (int)hu[j + 2]};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const bool up = (g8 & 4) != 0;
+                x[j][k] = (up ? hi4[k] : lo4[k]) + __shfl_xor_sync(0xffffffffu, up ? lo4[k] : hi4[k], 4);
+            }
+        }
+        int y[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const bool up = (g8 & 2) != 0;
+            y[k] = (up ? x[1][k] : x[0][k]) + __shfl_xor_sync(0xffffffffu, up ? x[0][k] : x[1][k], 2);
+            y[k] += __shfl_xor_sync(0xffffffffu, y[k], 1);
+        }
+        const long long t1 = 254ll * y[0] + y[1];
+        const double mt = __dadd_rn(__dmul_rn(__dmul_rn((double)t1, (double)s), pn->k1), prefilter_c(metric, nh0, h0));
+        const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, pn->w1), pn->wa);     // false for NaN / Inf scales and NaN factors
+        const bool leader = (g8 & 1) == 0 && valid;
+        const int side = mt > 0.0 ? 1 : 0;
+        if (leader && certain) jb.flags[pos] = (uint8_t)side;
+        if (leader && !certain) {   // stage 2 reads this row's lo plane from L2, and its scale and header from cr
+            PlanesLeft e;
+            e.mh = 64516ll * t1 + 254ll * y[2]; e.hu = (uint32_t)y[3]; e.pos = pos;
+            cr.left[atomicAdd(&sm_cnt[PLANES_CHUNK], 1u)] = e;
+            cr.scale[pos - base] = s;
+            cr.ih0[pos - base] = h0;
+            prefetch_l2(pl.lo + (size_t)rid * ld, ld);
+        }
+        const unsigned lefts = __ballot_sync(0xffffffffu, leader && certain && side == 0);
+        // the four groups of a warp hold positions of the same unit (16 consecutive positions per warp)
+        if (lane == 0 && lefts) atomicAdd(&sm_cnt[(pbase + warp * 16 - base) / SCAN_UNIT], (uint32_t)__popc(lefts));
+    }
+    __syncthreads();
+    // ---- stage 2: the lo plane of the rows stage 1 left, one 8-lane group per row; six words per lane in flight (the one
+    // round of a row of ld <= 768) ----
+    const uint32_t n1 = sm_cnt[PLANES_CHUNK];
+    for (uint32_t it = 0; it * 32u < n1; ++it) {
+        const uint32_t idx = it * 32u + (uint32_t)(warp * 4 + grp);
+        const bool act = idx < n1;
+        PlanesLeft e;
+        if (act) e = cr.left[idx];
+        else { e.mh = 0; e.hu = 0u; e.pos = base; }
+        const uint32_t p = e.pos;
+        const uint32_t r = cr.rid[p - base];
+        const uint4* Lr = reinterpret_cast<const uint4*>(pl.lo + (size_t)r * ld) + g8;
+        int la = 0, lb = 0, lc = 0;
+        uint32_t lu = 0;
+        for (int c0 = 0; c0 < nsteps; c0 += 6) {
+            uint4 vl[6];
+#pragma unroll
+            for (int sidx = 0; sidx < 6; ++sidx) {
+                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
+                vl[sidx] = q < nq ? ldg_stream_u4(Lr + (c0 + sidx) * 8) : make_uint4(0u, 0u, 0u, 0u);
+            }
+#pragma unroll
+            for (int sidx = 0; sidx < 6; ++sidx) {
+                const uint32_t q = (uint32_t)(c0 + sidx) * 8u + (uint32_t)g8;
+                if (q < nq) {   // the row's words past nq were loaded as zeros
+                    const uint4 na = LA[q], nb = LB[q], nc = LC[q], nu = LU[q];
+                    la = dp16(vl[sidx], na, la); lb = dp16(vl[sidx], nb, lb); lc = dp16(vl[sidx], nc, lc);
+                    lu = dp16u(abs_bytes(vl[sidx]), nu, lu);
+                }
+            }
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) {
+            la += __shfl_xor_sync(0xffffffffu, la, o); lb += __shfl_xor_sync(0xffffffffu, lb, o);
+            lc += __shfl_xor_sync(0xffffffffu, lc, o); lu += __shfl_xor_sync(0xffffffffu, lu, o);
+        }
+        // T2 and A: integers below 2^53 (the lo-plane group sums fit int32 / uint32 like the hi-plane ones), so the doubles are exact
+        const double m = (double)(e.mh + 64516ll * la + 254ll * lb + lc);
+        const double a = (double)(254ull * e.hu + lu);
         const float s = cr.scale[p - base];
         const double mt = __dadd_rn(__dmul_rn(__dmul_rn(m, (double)s), pn->k2), prefilter_c(metric, nh0, cr.ih0[p - base]));
         const bool certain = fabs(mt) > __dadd_rn(__dmul_rn((double)s, __dadd_rn(pn->w2, __dmul_rn(pn->rel2, a))), pn->wa);
@@ -710,7 +743,7 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
     uint32_t* sm_prefix = reinterpret_cast<uint32_t*>(sm_limbs + PLANES_LIMBS * ld);
     __shared__ uint32_t sm_count;
     __shared__ uint32_t sm_w[16];
-    __shared__ uint32_t sm_list[SCAN_UNIT * PLANES_CHUNK], sm_list2[SCAN_UNIT * PLANES_CHUNK];
+    __shared__ uint32_t sm_list2[SCAN_UNIT * PLANES_CHUNK];
     __shared__ uint32_t sm_cnt[PLANES_CHUNK + 2];
     __shared__ PlanesClaimRows sm_cr;
     __shared__ PlanesScratch sm_sc;
@@ -765,7 +798,7 @@ work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restr
             if (via_shadow(jb)) {
                 const uint32_t units = (jb.len + SCAN_UNIT - 1) / SCAN_UNIT;
                 scan_claim_planes(jb, item * PLANES_CHUNK, min(units, (item + 1u) * PLANES_CHUNK), items, planes, ih0, d, ld, metric, sm_normal, sm_limbs, &sm_pn, nh0,
-                                  sm_list, sm_list2, sm_cnt, sm_cr, stats);
+                                  sm_list2, sm_cnt, sm_cr, stats);
             } else scan_unit<true>(jb, item, items, ih0, d, ld, metric, sm_normal, nh0, &sm_count);
         } else {
             partition_block(jb.rows, jb.flags, jb.dst, item * PART_UNIT, jb.len, jb.unit_left[item * (PART_UNIT / SCAN_UNIT)], jb.total_left, sm_w);

@@ -269,7 +269,7 @@ int32_t arroy_b200_build_stats(arroy_ctx* ctx, double stats[8]);
  * read out[3] rows from the item matrix for all of them. Flags are identical either way. */
 int32_t arroy_b200_build_shadow_stats(arroy_ctx* ctx, uint64_t out[4]);
 /* The same accounting with the stages of the pre-filter apart: out[0] = rows that went through it (its first stage reads the
- * hi plane, one byte per element), out[1] = of them, rows its first stage could not decide (second stage: both planes),
+ * hi plane, one byte per element), out[1] = of them, rows its first stage could not decide (second stage: the lo plane),
  * out[2] = of them, rows the second stage could not decide either (scored from the f32 row), out[3], out[4] = out[2], out[3] of
  * arroy_b200_build_shadow_stats. */
 int32_t arroy_b200_build_prefilter_stats(arroy_ctx* ctx, uint64_t out[5]);
