@@ -27,6 +27,7 @@ CANCEL_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p)
 # every symbol include/arroy_b200.h declares: (name, restype, argtypes)
 SIGNATURES = [
     ("arroy_b200_version", C.c_char_p, []),
+    ("arroy_b200_allocations", C.c_int32, [_u64p]),
     ("arroy_b200_create", C.c_int32, [C.c_int32, C.POINTER(C.c_void_p)]),
     ("arroy_b200_destroy", None, [C.c_void_p]),
     ("arroy_b200_last_error", C.c_char_p, [C.c_void_p]),
@@ -156,6 +157,13 @@ def stage_delta_plan(old_ids, new_ids, changed_ids):
     src = np.empty(new.size, dtype=np.int64)
     n = load().arroy_b200_stage_delta_plan(_up(old), old.size, _up(new), new.size, _up(ch), ch.size, src.ctypes.data_as(C.POINTER(C.c_int64)))
     return src, int(n)
+
+
+def allocations():
+    """What the library holds now, in the whole process (arroy_b200_allocations; no CUDA call)."""
+    out = (C.c_uint64 * 5)()
+    load().arroy_b200_allocations(out)
+    return dict(zip(["device_buffers", "device_bytes", "pinned_buffers", "pinned_bytes", "handles"], (int(v) for v in out)))
 
 
 def item_placement_plan(metric, dim, n, free_bytes):

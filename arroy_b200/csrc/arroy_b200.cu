@@ -9,10 +9,12 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "../../include/arroy_b200.h"
@@ -43,27 +45,38 @@ struct NotStaged : std::runtime_error { using std::runtime_error::runtime_error;
                             std::to_string(__LINE__) + ")");                                          \
     } while (0)
 
+// Live allocations of the owning types below, in the whole process (arroy_b200_allocations): device buffers and their bytes,
+// pinned host buffers and their bytes, CUDA handles. Kept on the allocate and free paths only.
+enum { LIVE_DEV, LIVE_DEV_BYTES, LIVE_PIN, LIVE_PIN_BYTES, LIVE_HANDLES, LIVE_N };
+std::atomic<uint64_t> g_live[LIVE_N];
+void live_add(int kind, size_t bytes) { g_live[kind].fetch_add(1, std::memory_order_relaxed); g_live[kind + 1].fetch_add(bytes, std::memory_order_relaxed); }
+void live_sub(int kind, size_t bytes) { g_live[kind].fetch_sub(1, std::memory_order_relaxed); g_live[kind + 1].fetch_sub(bytes, std::memory_order_relaxed); }
+
+// The buffers below free their memory when they are destroyed and are move-only. Destructors ignore return codes: a context may
+// be destroyed at interpreter exit, after the CUDA runtime has begun unloading.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept { *this = std::move(o); }
+    DevBuf& operator=(DevBuf&& o) noexcept { if (this != &o) { release(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); } return *this; }
+    ~DevBuf() { release(); }
     void ensure(size_t bytes) {
         if (bytes <= cap) return;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        size_t want = bytes + bytes / 4 + 256;
-        CK(cudaMalloc(&p, want));
-        cap = want;
+        release();
+        alloc(bytes + bytes / 4 + 256);
     }
     // exactly `bytes` (no slack, nothing larger kept): for the planes of host-placed items, which are most of what such an index
     // holds on the device
     void ensure_exact(size_t bytes) {
         if (bytes == cap) return;
         release();
-        CK(cudaMalloc(&p, bytes));
-        cap = bytes;
+        alloc(bytes);
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    void release() { if (p) { cudaFree(p); live_sub(LIVE_DEV, cap); } p = nullptr; cap = 0; }
     template <class T> T* as() { return static_cast<T*>(p); }
+  private:
+    void alloc(size_t bytes) { CK(cudaMalloc(&p, bytes)); cap = bytes; if (p) live_add(LIVE_DEV, cap); }
 };
 // The f32 item matrix of a host-placed index: mapped pinned host memory, read by the kernels through its device address (UVA).
 // Allocated to size; a buffer more than twice the size asked for is given back rather than kept pinned.
@@ -71,6 +84,13 @@ struct MappedBuf {
     void* p = nullptr;
     void* dev = nullptr;
     size_t cap = 0;
+    MappedBuf() = default;
+    MappedBuf(MappedBuf&& o) noexcept { *this = std::move(o); }
+    MappedBuf& operator=(MappedBuf&& o) noexcept {
+        if (this != &o) { release(); p = std::exchange(o.p, nullptr); dev = std::exchange(o.dev, nullptr); cap = std::exchange(o.cap, 0); }
+        return *this;
+    }
+    ~MappedBuf() { release(); }
     void ensure(size_t bytes) {
         if (bytes <= cap && cap / 2 <= bytes) return;
         release();
@@ -81,31 +101,52 @@ struct MappedBuf {
             throw CudaError("cudaHostAlloc of " + std::to_string(bytes) + " bytes of pinned host memory for the item rows failed: " + cudaGetErrorString(e));
         }
         cap = bytes;
+        live_add(LIVE_PIN, cap);
         CK(cudaHostGetDevicePointer(&dev, p, 0));
     }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; dev = nullptr; cap = 0; }
+    void release() { if (p) { cudaFreeHost(p); live_sub(LIVE_PIN, cap); } p = nullptr; dev = nullptr; cap = 0; }
 };
 struct PinBuf {
     void* p = nullptr;
     size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(PinBuf&& o) noexcept { *this = std::move(o); }
+    PinBuf& operator=(PinBuf&& o) noexcept { if (this != &o) { release(); p = std::exchange(o.p, nullptr); cap = std::exchange(o.cap, 0); } return *this; }
+    ~PinBuf() { release(); }
     void ensure(size_t bytes) {
         if (bytes <= cap) return;
-        if (p) cudaFreeHost(p);
-        p = nullptr; cap = 0;
+        release();
         CK(cudaMallocHost(&p, bytes));
         cap = bytes;
+        live_add(LIVE_PIN, cap);
     }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+    void release() { if (p) { cudaFreeHost(p); live_sub(LIVE_PIN, cap); } p = nullptr; cap = 0; }
     template <class T> T* as() { return static_cast<T*>(p); }
 };
 
+// A CUDA or cuBLAS handle that destroys itself. It converts to the raw handle, so it is passed to the API as one.
+template <class T, auto Destroy>
+struct Handle {
+    T h = nullptr;
+    Handle() = default;
+    explicit Handle(T raw) : h(raw) { if (h) g_live[LIVE_HANDLES].fetch_add(1, std::memory_order_relaxed); }
+    Handle(Handle&& o) noexcept { *this = std::move(o); }
+    Handle& operator=(Handle&& o) noexcept { if (this != &o) { reset(); h = std::exchange(o.h, nullptr); } return *this; }
+    ~Handle() { reset(); }
+    operator T() const { return h; }
+    void reset() { if (h) { Destroy(h); g_live[LIVE_HANDLES].fetch_sub(1, std::memory_order_relaxed); } h = nullptr; }
+};
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Graph = Handle<cudaGraph_t, cudaGraphDestroy>;
+using GraphExec = Handle<cudaGraphExec_t, cudaGraphExecDestroy>;
+using Blas = Handle<cublasHandle_t, cublasDestroy>;
+
+Stream new_stream() { cudaStream_t s = nullptr; CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return Stream(s); }
+Event new_event(unsigned flags = cudaEventDefault) { cudaEvent_t e = nullptr; CK(cudaEventCreateWithFlags(&e, flags)); return Event(e); }
+
 struct Wave {  // device buffers of one wave of trees; kept across builds
     DevBuf st, frames, recs, perm0, perm1, flags, unit_left, pool, pool_counter, jobs, scratch, active, error, final_ids, keys, sub_rows, sub_off, slots, abort, cur_normal, start_pos, root, shadow_stats;
-    void release() {
-        sub_rows.release(); sub_off.release(); slots.release(); abort.release(); cur_normal.release(); start_pos.release(); root.release(); shadow_stats.release();
-        st.release(); frames.release(); recs.release(); perm0.release(); perm1.release(); flags.release(); unit_left.release();
-        pool.release(); pool_counter.release(); jobs.release(); scratch.release(); active.release(); error.release(); final_ids.release(); keys.release();
-    }
 };
 struct BuiltTreeView {  // views into the pinned HostWave buffers of the context
     const void* recs = nullptr;
@@ -114,14 +155,13 @@ struct BuiltTreeView {  // views into the pinned HostWave buffers of the context
     const float* pool = nullptr;
 };
 struct StageWorker {  // one H2D lane of the staging pipeline: own stream, two pinned bounce buffers
-    cudaStream_t st = nullptr;
+    Stream st;
     PinBuf pin[2];
     DevBuf dev[2];   // host placement: the device bounce buffers the chunk encoder reads
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    Event ev[2];
 };
 struct HostWave {  // pinned host copies of one wave's results; kept across builds
     PinBuf recs, final_rows, pool;
-    void release() { recs.release(); final_rows.release(); pool.release(); }
 };
 
 }  // namespace
@@ -129,7 +169,7 @@ struct HostWave {  // pinned host copies of one wave's results; kept across buil
 struct arroy_ctx {
     int device = 0;
     int sm_count = 132;
-    cudaStream_t stream = nullptr;
+    Stream stream;   // declared first, destroyed last: ~arroy_ctx synchronises it and the other members free themselves
     std::mutex mu;
     std::string err;
     // staged items
@@ -149,14 +189,14 @@ struct arroy_ctx {
     // scratch
     DevBuf s_rows, s_flags, s_margins, s_normal, s_unit, s_job, s_keys, s_keys2, s_dists, s_q, s_qbits, s_qh0, s_off, s_orows, s_odist, s_olen, s_misc;
     PinBuf pin;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    cudaStream_t side_stream = nullptr;   // host -> device flags while the persistent build kernel occupies `stream`
-    cudaEvent_t ev_done = nullptr, ev_p0 = nullptr, ev_p1 = nullptr;   // ev_p0 / ev_p1 bracket the persistent build kernel
+    Event ev0, ev1;
+    Stream side_stream;   // host -> device flags while the persistent build kernel occupies `stream`
+    Event ev_done, ev_p0, ev_p1;   // ev_p0 / ev_p1 bracket the persistent build kernel
     double stats[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     uint64_t shadow_rows = 0, shadow_rescored = 0, shadow_stage2 = 0, fused_root_rows = 0, fused_root_read = 0;
     uint64_t wave_key[4] = {0, 0, 0, 0}, wave_max = 0, wave_trees_ok = 0; bool wave_key_valid = false;   // shapes of the last successful build (do_build_begin)   // last build: rows scanned through the bf16 shadow / re-scored from f32
     uint64_t n_launches = 0, h2d_bytes = 0, d2h_bytes = 0;  // since create (arroy_b200_counters)
-    cudaEvent_t tev0 = nullptr, tev1 = nullptr;
+    Event tev0, tev1;
     std::vector<StageWorker> stage_workers;
     bool staging_open = false;             // between arroy_b200_stage_begin and arroy_b200_stage_end
     std::vector<float> stage_h0, stage_h1;  // headers decoded from the leaf values staged so far
@@ -187,19 +227,19 @@ struct arroy_ctx {
     std::vector<uint32_t> pending_wave_t0;
     uint32_t pending_pool_stride = 0, pending_n_trees = 0;
     Wave wave;
-    cudaGraph_t cached_graph = nullptr;
-    cudaGraphExec_t cached_exec = nullptr;
+    Graph cached_graph;
+    GraphExec cached_exec;
     std::vector<uint8_t> cached_graph_key;  // BuildParams bytes + schedule the cached graph was captured for
     std::vector<HostWave> host_waves;
     double breakdown[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    std::vector<cudaStream_t> tree_streams;   // one per tree of a wave (asynchronous per-tree chains)
-    std::vector<cudaEvent_t> tree_events;     // join events, [0] = fork
+    std::vector<Stream> tree_streams;   // one per tree of a wave (asynchronous per-tree chains)
+    std::vector<Event> tree_events;     // join events, [0] = fork
     // tensor-core pre-filter of rerank_shared
-    cublasHandle_t blas = nullptr;
+    Blas blas;
     DevBuf x_gather, x_cnorm, x_ca, x_cb, x_gmax, x_qa, x_qb, x_twoe, x_qnorm, x_S, x_sel, x_beg, x_end, x_flag;
     DevBuf x_gh0, x_iota;   // host placement: the gathered candidates' headers and their positions for the exact dense path
     uint64_t xf_calls = 0, xf_fallbacks = 0, xf_selected = 0, xf_queries = 0;
-    cudaEvent_t xev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    Event xev[8];
     double xbreak[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     double sbreak[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     // fused re-rank with a bf16 shadow of the items (frerank.cuh); built lazily by the first query after staging
@@ -214,6 +254,11 @@ struct arroy_ctx {
     // and survivors re-scored, allocated by the first such batch
     DevBuf pr_counts;
     uint64_t fr_batches[2] = {0, 0}, fr_fallbacks[2] = {0, 0};   // fused re-rank batches and fallbacks since create, per FrSource
+
+    ~arroy_ctx() {
+        cudaSetDevice(device);
+        if (stream) cudaStreamSynchronize(stream);
+    }
 };
 
 namespace {
@@ -280,9 +325,15 @@ void compute_norms(arroy_ctx* c, bool with_max) {
     c->n_launches += 1;
 }
 
-// Stage epochs are unique in the process, not per context: an owner that remembers (context, epoch) is not fooled by a new
-// context that was created at the address of a destroyed one.
-uint64_t next_stage_epoch() { static std::atomic<uint64_t> last{0}; return ++last; }
+// A (re)staging forgets everything derived from the previous items: the bf16 shadow, the 8-bit planes and the device forest (its
+// descendant rows were validated against the previous item count). Their buffers are kept for reuse. Stage epochs are unique in
+// the process, not per context: an owner that remembers (context, epoch) is not fooled by a new context that was created at the
+// address of a destroyed one.
+void forget_staged(arroy_ctx* c) {
+    static std::atomic<uint64_t> last_epoch{0};
+    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false; c->staging_open = false;
+    c->stage_epoch = ++last_epoch;
+}
 
 // Where the f32 rows of a staging go (may_host: the staging calls that can write host-placed rows, arroy_b200_stage_items and
 // _flat). The plan sees the free device memory plus what this context already holds for items, their derived copies and the wave
@@ -311,10 +362,7 @@ void alloc_items(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, const uint3
     if (is_bq(metric)) dim = (dim + 63u) / 64u * 64u;   // the bit string's length (binary_quantized.rs:80-92)
     if (n > 0xffffffffull) throw ArgError("too many items");
     for (uint64_t i = 1; i < n; ++i) if (ids[i] <= ids[i - 1]) throw ArgError("ids must be strictly ascending");
-    // a restage invalidates everything derived from the previous items: the bf16 shadow, the 8-bit planes and the device forest
-    // (its descendant rows were validated against the previous item count)
-    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false; c->staging_open = false;
-    c->stage_epoch = next_stage_epoch();
+    forget_staged(c);
     c->metric = metric; c->dim = dim; c->ld = (dim + 31u) & ~31u; c->n = n;
     c->row_bytes = is_bq(metric) ? 16u * bq_row_u4(dim) : 4u * c->ld;
     c->ids.assign(ids, ids + n);
@@ -373,11 +421,11 @@ void stage_rows_pipeline(arroy_ctx* c, uint64_t n, uint32_t dim, uint32_t row_by
     if (c->stage_workers.size() < W) c->stage_workers.resize(W);
     for (unsigned w = 0; w < W; ++w) {
         StageWorker& sw = c->stage_workers[w];
-        if (!sw.st) CK(cudaStreamCreateWithFlags(&sw.st, cudaStreamNonBlocking));
+        if (!sw.st) sw.st = new_stream();
         for (int k = 0; k < 2; ++k) {
             if (host) sw.dev[k].ensure(chunk_rows * row_bytes);
             else sw.pin[k].ensure(chunk_rows * row_bytes);
-            if (!sw.ev[k]) CK(cudaEventCreateWithFlags(&sw.ev[k], cudaEventDisableTiming));
+            if (!sw.ev[k]) sw.ev[k] = new_event(cudaEventDisableTiming);
         }
     }
     CK(cudaStreamSynchronize(c->stream));  // the destination buffer must not be in use
@@ -700,11 +748,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         memcpy(key.data() + sizeof(BuildParams), shape, 12);
         if (c->cached_exec && key == c->cached_graph_key) gexec = c->cached_exec;
         else {
-            if (c->cached_exec) { cudaGraphExecDestroy(c->cached_exec); c->cached_exec = nullptr; }
-            if (c->cached_graph) { cudaGraphDestroy(c->cached_graph); c->cached_graph = nullptr; }
             c->cached_graph_key.clear();
-            while (c->tree_streams.size() < tw) { cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); c->tree_streams.push_back(st); }
-            while (c->tree_events.size() < (size_t)tw + 1) { cudaEvent_t ev; CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)); c->tree_events.push_back(ev); }
+            while (c->tree_streams.size() < tw) c->tree_streams.push_back(new_stream());
+            while (c->tree_events.size() < (size_t)tw + 1) c->tree_events.push_back(new_event(cudaEventDisableTiming));
             const size_t wsmem1 = work_smem(ld, 1);
             cudaGraph_t graph = nullptr;
             CK(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
@@ -721,9 +767,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
                 CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
             }
             CK(cudaStreamEndCapture(c->stream, &graph));
-            c->cached_graph = graph;
+            c->cached_graph = Graph(graph);
             CK(cudaGraphInstantiate(&gexec, graph, 0));
-            c->cached_exec = gexec;
+            c->cached_exec = GraphExec(gexec);
             c->cached_graph_key = key;
         }
     }
@@ -733,9 +779,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     c->pin.ensure(64);
     volatile uint32_t* h_active = c->pin.as<uint32_t>();
     volatile int32_t* h_error = reinterpret_cast<volatile int32_t*>(c->pin.as<uint32_t>() + 1);
-    std::vector<cudaEvent_t> pev;
-    struct EvGuard { std::vector<cudaEvent_t>& v; ~EvGuard() { for (auto e : v) cudaEventDestroy(e); } } evg{pev};
-    if (profile) { pev.resize(2 * LOCKSTEP_BATCH); for (auto& e : pev) CK(cudaEventCreate(&e)); }
+    std::vector<Event> pev;
+    if (profile) for (int i = 0; i < 2 * LOCKSTEP_BATCH; ++i) pev.push_back(new_event());
     uint64_t steps = 0;
     // safety net against a stuck state machine (never hit by a correct build): every step each
     // live tree completes one attempt or one partition
@@ -1092,7 +1137,7 @@ void xf_scores(arroy_ctx* c, const float* q, uint32_t m, const float* cand, uint
         c->n_launches += 1;
         return;
     }
-    if (!c->blas) { if (cublasCreate(&c->blas) != CUBLAS_STATUS_SUCCESS) throw CudaError("cublasCreate failed"); }
+    if (!c->blas) { cublasHandle_t b = nullptr; if (cublasCreate(&b) != CUBLAS_STATUS_SUCCESS) throw CudaError("cublasCreate failed"); c->blas = Blas(b); }
     if (cublasSetStream(c->blas, c->stream) != CUBLAS_STATUS_SUCCESS) throw CudaError("cublasSetStream failed");
     const float one = 1.0f, zero = 0.0f;
     cublasStatus_t st = cublasGemmEx(c->blas, CUBLAS_OP_T, CUBLAS_OP_N, (int)nc, (int)m, (int)c->ld, &one, cand, CUDA_R_32F, (int)c->ld,
@@ -1216,7 +1261,7 @@ void bq_normalize(arroy_ctx* c, float* d_dist, uint64_t count) {
 struct Marks {
     arroy_ctx* c;
     int n = 0;
-    void operator()() { if (!c->xev[n]) CK(cudaEventCreate(&c->xev[n])); CK(cudaEventRecord(c->xev[n], c->stream)); ++n; }
+    void operator()() { if (!c->xev[n]) c->xev[n] = new_event(); CK(cudaEventRecord(c->xev[n], c->stream)); ++n; }
     void add_to(double* b) const { for (int i = 0; i + 1 < n; ++i) { float ms = 0; CK(cudaEventElapsedTime(&ms, c->xev[i], c->xev[i + 1])); b[i] += ms; } }
 };
 
@@ -1393,75 +1438,46 @@ extern "C" {
 
 const char* arroy_b200_version(void) { return "arroy_b200 0.1.0 (sm_90a)"; }
 
+int32_t arroy_b200_allocations(uint64_t out[5]) {
+    if (!out) return ARROY_B200_ERR_INVALID;
+    for (int i = 0; i < LIVE_N; ++i) out[i] = g_live[i].load(std::memory_order_relaxed);
+    return ARROY_B200_OK;
+}
+
 int32_t arroy_b200_create(int32_t device, arroy_ctx** out) {
     if (!out) return ARROY_B200_ERR_INVALID;
     *out = nullptr;
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count) { cudaGetLastError(); return ARROY_B200_ERR_CUDA; }
-    arroy_ctx* c = nullptr;
     try {
-        c = new arroy_ctx();
+        auto c = std::make_unique<arroy_ctx>();
         c->device = device;
         CK(cudaSetDevice(device));
         cudaDeviceProp prop;
         CK(cudaGetDeviceProperties(&prop, device));
         c->sm_count = prop.multiProcessorCount;
-        CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-        CK(cudaEventCreate(&c->ev0));
-        CK(cudaEventCreate(&c->ev1));
-        CK(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming));
-        CK(cudaEventCreate(&c->ev_p0));
-        CK(cudaEventCreate(&c->ev_p1));
-        CK(cudaEventCreate(&c->tev0));
-        CK(cudaEventCreate(&c->tev1));
+        c->stream = new_stream();
+        c->ev0 = new_event();
+        c->ev1 = new_event();
+        c->side_stream = new_stream();
+        c->ev_done = new_event(cudaEventDisableTiming);
+        c->ev_p0 = new_event();
+        c->ev_p1 = new_event();
+        c->tev0 = new_event();
+        c->tev1 = new_event();
         // fail loudly if the kernels were not built for this device
         cudaFuncAttributes fa;
         CK(cudaFuncGetAttributes(&fa, work_kernel<false>));
+        *out = c.release();
     } catch (const std::exception& e) {
         fprintf(stderr, "arroy_b200_create: %s\n", e.what());
-        delete c;
         cudaGetLastError();
         return ARROY_B200_ERR_CUDA;
     }
-    *out = c;
     return ARROY_B200_OK;
 }
 
-void arroy_b200_destroy(arroy_ctx* c) {
-    if (!c) return;
-    cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    DevBuf* bufs[] = {&c->items, &c->h0, &c->h1, &c->norms, &c->maxbits, &c->s_rows, &c->s_flags, &c->s_margins, &c->s_normal, &c->s_unit, &c->s_job,
-                      &c->s_keys, &c->s_keys2, &c->s_dists, &c->s_q, &c->s_qh0, &c->s_off, &c->s_orows, &c->s_odist, &c->s_olen, &c->s_misc};
-    for (auto* b : bufs) b->release();
-    c->host_rows.release();
-    { DevBuf* xb[] = {&c->pl_hi, &c->pl_lo, &c->pl_scale, &c->fr_shadow, &c->fr_norm, &c->fr_gmax, &c->fr_status, &c->pr_counts, &c->x_gather, &c->x_cnorm, &c->x_ca, &c->x_cb, &c->x_gmax, &c->x_qa, &c->x_qb, &c->x_twoe, &c->x_qnorm, &c->x_S, &c->x_sel, &c->x_beg, &c->x_end, &c->x_flag,
-                      &c->x_gh0, &c->x_iota}; for (auto* b : xb) b->release(); }
-    if (c->blas) cublasDestroy(c->blas);
-    for (auto& e : c->xev) if (e) cudaEventDestroy(e);
-    if (c->cached_exec) cudaGraphExecDestroy(c->cached_exec);
-    if (c->cached_graph) cudaGraphDestroy(c->cached_graph);
-    for (auto& sw : c->stage_workers) { sw.pin[0].release(); sw.pin[1].release(); sw.dev[0].release(); sw.dev[1].release(); if (sw.ev[0]) cudaEventDestroy(sw.ev[0]); if (sw.ev[1]) cudaEventDestroy(sw.ev[1]); if (sw.st) cudaStreamDestroy(sw.st); }
-    { DevBuf* fb[] = {&c->f_kind, &c->f_left, &c->f_right, &c->f_nidx, &c->f_nh0, &c->f_doff, &c->f_dlen, &c->f_normals, &c->f_desc, &c->f_roots, &c->f_rec, &c->f_nofn,
-                      &c->w_heaps, &c->w_cand, &c->w_cand2, &c->w_count, &c->w_bitmap, &c->w_status, &c->w_beg, &c->w_end, &c->w_qrows, &c->w_tmp, &c->w_pre};
-      for (auto* b : fb) b->release(); }
-    c->pin.release();
-    c->wave.release(); c->wave_key_valid = false;
-    for (auto& hw : c->host_waves) hw.release();
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->ev1) cudaEventDestroy(c->ev1);
-    if (c->ev_done) cudaEventDestroy(c->ev_done);
-    if (c->ev_p0) cudaEventDestroy(c->ev_p0);
-    if (c->ev_p1) cudaEventDestroy(c->ev_p1);
-    if (c->side_stream) cudaStreamDestroy(c->side_stream);
-    if (c->tev0) cudaEventDestroy(c->tev0);
-    if (c->tev1) cudaEventDestroy(c->tev1);
-    for (auto st : c->tree_streams) cudaStreamDestroy(st);
-    for (auto ev : c->tree_events) cudaEventDestroy(ev);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
-}
+void arroy_b200_destroy(arroy_ctx* c) { delete c; }
 
 const char* arroy_b200_last_error(arroy_ctx* c) { return c ? c->err.c_str() : "null context"; }
 
@@ -1536,9 +1552,8 @@ bool stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, c
     const int hf = metric_header_floats(metric);
     std::vector<float> h0, h1;
     decode_leaf_headers(leaf_values, n, hf, h0, h1);
-    // scratch for one window, released again below: a card filled by its index has no room to lend for longer
+    // scratch for one window, freed when this call returns: a card filled by its index has no room to lend for longer
     DevBuf scratch, d_pieces;
-    struct Release { DevBuf &a, &b; ~Release() { a.release(); b.release(); } } release{scratch, d_pieces};
     const uint64_t n_pieces = mv.pieces.size() + up.pieces.size();
     if (n_pieces) {
         try {
@@ -1546,11 +1561,9 @@ bool stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, c
             d_pieces.ensure(n_pieces * sizeof(RestagePiece));
         } catch (const CudaError&) { cudaGetLastError(); return false; }   // no room for the scratch: the full staging needs none
     }
-    // from here on the context changes: what alloc_items invalidates is invalid here too (the bf16 shadow, the 8-bit planes and
-    // the device forest follow rows, not ids)
+    // from here on the context changes: the derived state follows rows, not ids
     const uint64_t h2d0 = c->h2d_bytes;
-    c->staged = false; c->fr_valid = false; c->shadow_valid = false; c->planes_valid = false; c->forest_loaded = false;
-    c->stage_epoch = next_stage_epoch();
+    forget_staged(c);
     c->n = n;
     c->ids.assign(ids, ids + n);
     CK(cudaStreamSynchronize(c->stream));   // h0 / h1 may be reallocated: nothing may still read them
@@ -1581,7 +1594,7 @@ bool stage_items_delta(arroy_ctx* c, int32_t metric, uint32_t dim, uint64_t n, c
             k0 += rows;
         }
     }
-    upload_headers(c, h0, h1);   // ends in a stream synchronise: the scratch buffer is idle when it is released
+    upload_headers(c, h0, h1);   // ends in a stream synchronise: the scratch buffer is idle when it is freed
     c->staged = true;
     c->stage_stats[0] = n_upload; c->stage_stats[1] = mv.rows; c->stage_stats[2] = 1; c->stage_stats[3] = c->h2d_bytes - h2d0;
     return true;

@@ -42,11 +42,17 @@ struct arroy_group {
     std::vector<arroy_ctx*> ctx;
     std::vector<int> dev;
     std::vector<void*> comm;
-    std::vector<cudaStream_t> bstream;   // broadcast streams, one per device
+    std::vector<Stream> bstream;   // broadcast streams, one per device
     NcclApi nccl;
     std::string err;
     std::mutex mu;
     double stage_ms[4] = {0, 0, 0, 0};   // last group_stage_items: [0] total wall, [1] waiting for the last broadcast after the last H2D
+
+    ~arroy_group() {   // communicators, then the broadcast streams, then the member contexts
+        for (void* cm : comm) if (cm) nccl.CommDestroy(cm);
+        for (size_t r = 0; r < bstream.size(); ++r) { cudaSetDevice(dev[r]); bstream[r].reset(); }
+        for (auto* c : ctx) delete c;
+    }
 };
 
 namespace {
@@ -94,17 +100,16 @@ int32_t arroy_b200_create_group(int32_t n_dev, const int32_t* devices, arroy_gro
             if (arroy_b200_create(devices[i], &c) != ARROY_B200_OK) throw CudaError("arroy_b200_create failed for device " + std::to_string(devices[i]));
             g->ctx.push_back(c); g->dev.push_back(devices[i]);
             CK(cudaSetDevice(devices[i]));
-            cudaStream_t st; CK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-            g->bstream.push_back(st);
+            g->bstream.push_back(new_stream());
         }
         if (n_dev > 1) {
             if (!g->nccl.load()) throw CudaError(g->nccl.err);
-            g->comm.assign(n_dev, nullptr);
-            nccl_ck(g, g->nccl.CommInitAll(g->comm.data(), n_dev, g->dev.data()), "ncclCommInitAll");
+            std::vector<void*> comm(n_dev, nullptr);   // kept only once all of them exist
+            nccl_ck(g, g->nccl.CommInitAll(comm.data(), n_dev, g->dev.data()), "ncclCommInitAll");
+            g->comm = std::move(comm);
         }
     } catch (const std::exception& e) {
         fprintf(stderr, "arroy_b200_create_group: %s\n", e.what());
-        for (auto* c : g->ctx) arroy_b200_destroy(c);
         delete g;
         cudaGetLastError();
         return ARROY_B200_ERR_CUDA;
@@ -113,13 +118,7 @@ int32_t arroy_b200_create_group(int32_t n_dev, const int32_t* devices, arroy_gro
     return ARROY_B200_OK;
 }
 
-void arroy_b200_destroy_group(arroy_group* g) {
-    if (!g) return;
-    for (size_t r = 0; r < g->comm.size(); ++r) if (g->comm[r]) g->nccl.CommDestroy(g->comm[r]);
-    for (size_t r = 0; r < g->bstream.size(); ++r) { cudaSetDevice(g->dev[r]); cudaStreamDestroy(g->bstream[r]); }
-    for (auto* c : g->ctx) arroy_b200_destroy(c);
-    delete g;
-}
+void arroy_b200_destroy_group(arroy_group* g) { delete g; }
 
 const char* arroy_b200_group_last_error(arroy_group* g) { return g ? g->err.c_str() : "null group"; }
 int32_t arroy_b200_group_size(arroy_group* g) { return g ? (int32_t)g->ctx.size() : 0; }

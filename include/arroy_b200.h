@@ -67,6 +67,10 @@ void arroy_b200_destroy(arroy_ctx* ctx);
 const char* arroy_b200_last_error(arroy_ctx* ctx);
 /* library version string and the SM architecture the kernels were compiled for */
 const char* arroy_b200_version(void);
+/* What the library holds now, in the whole process (no context, no CUDA call): out[0] = live device buffers, out[1] = their
+ * bytes, out[2] = live pinned host buffers, out[3] = their bytes, out[4] = live CUDA streams, events, graphs, graph execs and
+ * cuBLAS handles. Destroying every context and group brings all five back to where they were before they were created. */
+int32_t arroy_b200_allocations(uint64_t out[5]);
 
 /* ---- item staging: replaces ImmutableLeafs::new (src/parallel.rs:271-293) ------------- */
 
