@@ -536,7 +536,7 @@ class Context:
     def build_breakdown(self):
         st = (C.c_double * 8)()
         self._ck(self.lib.arroy_b200_build_breakdown(self.h, st))
-        keys = ["setup_ms", "graph_ms", "loop_ms", "d2h_ms", "encode_ms", "graph_launches", "schedules", "r7"]
+        keys = ["setup_ms", "graph_ms", "loop_ms", "d2h_ms", "encode_ms", "graph_launches", "schedules", "late_pool_slots"]
         return dict(zip(keys, list(st)))
 
     def counters(self):

@@ -78,8 +78,9 @@ struct DevBuf {
   private:
     void alloc(size_t bytes) { CK(cudaMalloc(&p, bytes)); cap = bytes; if (p) live_add(LIVE_DEV, cap); }
 };
-// The f32 item matrix of a host-placed index: mapped pinned host memory, read by the kernels through its device address (UVA).
-// Allocated to size; a buffer more than twice the size asked for is given back rather than kept pinned.
+// Mapped pinned host memory that kernels address through `dev`: the f32 item matrix of a host-placed index, and the host result
+// buffers the build kernels write (HostWave). Allocated to size; a buffer more than twice the size asked for is given back rather
+// than kept pinned.
 struct MappedBuf {
     void* p = nullptr;
     void* dev = nullptr;
@@ -98,13 +99,14 @@ struct MappedBuf {
         if (e != cudaSuccess) {
             p = nullptr;
             cudaGetLastError();
-            throw CudaError("cudaHostAlloc of " + std::to_string(bytes) + " bytes of pinned host memory for the item rows failed: " + cudaGetErrorString(e));
+            throw CudaError("cudaHostAlloc of " + std::to_string(bytes) + " bytes of mapped pinned host memory failed: " + cudaGetErrorString(e));
         }
         cap = bytes;
         live_add(LIVE_PIN, cap);
         CK(cudaHostGetDevicePointer(&dev, p, 0));
     }
     void release() { if (p) { cudaFreeHost(p); live_sub(LIVE_PIN, cap); } p = nullptr; dev = nullptr; cap = 0; }
+    template <class T> T* as() { return static_cast<T*>(p); }
 };
 struct PinBuf {
     void* p = nullptr;
@@ -146,9 +148,9 @@ Stream new_stream() { cudaStream_t s = nullptr; CK(cudaStreamCreateWithFlags(&s,
 Event new_event(unsigned flags = cudaEventDefault) { cudaEvent_t e = nullptr; CK(cudaEventCreateWithFlags(&e, flags)); return Event(e); }
 
 struct Wave {  // device buffers of one wave of trees; kept across builds
-    DevBuf st, frames, recs, perm0, perm1, flags, unit_left, pool, pool_counter, jobs, scratch, active, error, final_ids, keys, sub_rows, sub_off, slots, abort, cur_normal, start_pos, root, shadow_stats;
+    DevBuf st, frames, recs, perm0, perm1, flags, unit_left, pool, pool_counter, jobs, scratch, active, error, keys, sub_rows, sub_off, slots, abort, cur_normal, start_pos, root, shadow_stats;
 };
-struct BuiltTreeView {  // views into the pinned HostWave buffers of the context
+struct BuiltTreeView {  // views into the HostWave buffers of the context
     const void* recs = nullptr;
     uint32_t n_recs = 0;
     const uint32_t* final_rows = nullptr;  // n entries
@@ -160,8 +162,12 @@ struct StageWorker {  // one H2D lane of the staging pipeline: own stream, two p
     DevBuf dev[2];   // host placement: the device bounce buffers the chunk encoder reads
     Event ev[2];
 };
-struct HostWave {  // pinned host copies of one wave's results; kept across builds
-    PinBuf recs, final_rows, pool;
+// One wave's results in mapped pinned host memory, written by the control kernel while the wave builds (build.cuh
+// export_records); kept across builds. Records of tree t start at t * rec_cap, its ids in final order at t * n.
+struct HostWave {
+    MappedBuf recs, final_rows, pool;
+    uint64_t shape[5] = {0, 0, 0, 0, 0};   // (n, K, ld, trees, subsets) of the last build of this wave, the slot capacity of its
+    uint32_t slots = 0, pool_used = 0;     // host pool and the slots it used (build_wave sizes the next pool from them)
 };
 
 }  // namespace
@@ -281,7 +287,7 @@ bool host_placement_eligible(int metric, uint32_t dim) { return metric >= EUCLID
 uint64_t device_placement_bytes(uint32_t dim, uint64_t n) {
     const uint64_t ld = (dim + 31u) & ~31u;
     const uint64_t leaves_est = n / std::max<uint32_t>(dim, 1) + 1;
-    const uint64_t per_tree = n * (4 + 4 + 1 + 4) + (n / SCAN_UNIT + 1) * 4 + sizeof(Frame) * (uint64_t)MAX_DEPTH + 16ull * 8 * leaves_est +
+    const uint64_t per_tree = n * (4 + 4 + 1) + (n / SCAN_UNIT + 1) * 4 + sizeof(Frame) * (uint64_t)MAX_DEPTH + 16ull * 8 * leaves_est +
                               4ull * (ld + NORMAL_HDR) * 4 * leaves_est + 4096;
     return n * ld * 4 + 2 * n * ld + 4 * n + 8 * n + per_tree;
 }
@@ -347,7 +353,7 @@ bool choose_host_placement(arroy_ctx* c, int metric, uint32_t dim, uint64_t n, b
     CK(cudaMemGetInfo(&free_b, &total_b));
     const Wave& W = c->wave;
     const uint64_t held = c->items.cap + c->pl_hi.cap + c->pl_lo.cap + c->pl_scale.cap + c->fr_shadow.cap + c->fr_norm.cap + W.perm0.cap + W.perm1.cap +
-                          W.flags.cap + W.final_ids.cap + W.pool.cap + W.recs.cap;
+                          W.flags.cap + W.pool.cap + W.recs.cap;
     if (placement_plan(metric, dim, n, (uint64_t)free_b + held) == 1) return true;
     c->placed_metric = metric; c->placed_dim = dim; c->placed_n = n;
     return false;
@@ -613,6 +619,23 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     // cluster-resident nodes: up to ~6 MB of item rows per scan (2048 rows at d = 768, every node of a 10k x 64 index)
     P.small_max = (uint32_t)std::max<uint64_t>(2048, (6ull << 20) / (4ull * ld));
     P.max_inner = 1024u;   // attempts per launch; `cancel` is polled between launches
+    // host result buffers: the control kernel writes each record, leaf's ids and accepted normal there as it closes
+    // (build.cuh export_records), so no copy of the results follows the kernel. The host pool keeps the slot capacity of the
+    // last build of these shapes while that build's slots fit in it, and otherwise takes the slots it used plus an eighth; slots
+    // above the capacity are copied after the kernel. A capacity that stays put keeps BuildParams, and so the async schedule's
+    // cached graph, the same from build to build.
+    if (c->host_waves.size() <= wave_no) c->host_waves.resize(wave_no + 1);
+    HostWave& H = c->host_waves[wave_no];
+    const uint64_t shape[5] = {n, K, ld, tw, (uint64_t)(sub.rows ? 1 : 0)};
+    const bool same_shape = memcmp(shape, H.shape, sizeof shape) == 0;
+    uint64_t h_slots = !same_shape ? 2 * leaves_est * tw + 8ull * tw : H.pool_used <= H.slots ? H.slots : (uint64_t)H.pool_used + H.pool_used / 8;
+    h_slots = std::min<uint64_t>(h_slots, pool_cap);
+    if (const char* e = getenv("ARROY_B200_EXPORT_SLOTS")) h_slots = std::min<uint64_t>(h_slots, strtoull(e, nullptr, 10));
+    H.recs.ensure(sizeof(Record) * (size_t)rec_cap * tw);
+    H.final_rows.ensure(std::max<size_t>(16, 4ull * n * tw));
+    H.pool.ensure(std::max<size_t>(16, (size_t)h_slots * pool_stride * 4));
+    P.h_recs = static_cast<Record*>(H.recs.dev); P.h_rows = static_cast<uint32_t*>(H.final_rows.dev);
+    P.h_pool = static_cast<float*>(H.pool.dev); P.h_pool_slots = (uint32_t)h_slots;
     if (sub.rows) {   // this wave's subsets, offsets rebased to the wave
         const uint64_t b = sub.off[t0], e = sub.off[t0 + tw];
         std::vector<uint64_t> off(tw + 1);
@@ -643,7 +666,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     }
     init_trees_kernel<<<tw, 256, 0, c->stream>>>(P, W.keys.as<uint32_t>(), d_start);
     CK(cudaGetLastError());
-    c->n_launches += 2;  // + finalize_kernel below
+    c->n_launches += 1;
 
     const size_t ctrl_smem = use_smem ? ws_bytes : 0;
     if (ctrl_smem > 48 * 1024) CK(cudaFuncSetAttribute(control_fn(true, 1, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
@@ -862,34 +885,43 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     c->breakdown[5] += (double)(steps / steps_per_batch);
     auto t_d2h = std::chrono::steady_clock::now();
 
-    // results: merge the ping-pong id buffers, then bring everything to (pinned) host memory
-    W.final_ids.ensure(4ull * n * tw);
-    finalize_kernel<<<dim3(64, tw), 256, 0, c->stream>>>(P, W.final_ids.as<uint32_t>());
-    CK(cudaGetLastError());
+    // results: the kernel has written them to the host buffers; only the tree states, the pool's fill and the pre-filter's
+    // stage counters come back here
     std::vector<TreeState> st(tw);
     uint32_t pool_used = 0;
+    unsigned long long hs[3] = {0, 0, 0};
     CK(cudaMemcpyAsync(st.data(), W.st.p, sizeof(TreeState) * tw, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(&pool_used, W.pool_counter.p, 4, cudaMemcpyDeviceToHost, c->stream));
+    if (P.shadow_stats) CK(cudaMemcpyAsync(hs, P.shadow_stats, 24, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
-    if (c->host_waves.size() <= wave_no) c->host_waves.resize(wave_no + 1);
-    HostWave& H = c->host_waves[wave_no];
-    uint64_t total_recs = 0;
-    for (uint32_t t = 0; t < tw; ++t) total_recs += st[t].n_recs;
-    H.pool.ensure(std::max<size_t>(16, (size_t)pool_used * pool_stride * 4));
-    H.recs.ensure(std::max<size_t>(16, sizeof(Record) * total_recs));
-    H.final_rows.ensure(std::max<size_t>(16, 4ull * n * tw));
-    if (pool_used) CK(cudaMemcpyAsync(H.pool.p, W.pool.p, (size_t)pool_used * pool_stride * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(H.final_rows.p, W.final_ids.p, 4ull * n * tw, cudaMemcpyDeviceToHost, c->stream));
+    memcpy(H.shape, shape, sizeof shape); H.slots = (uint32_t)h_slots; H.pool_used = pool_used;
+    uint64_t late_bytes = 0;
+    if (pool_used > h_slots) {   // the slots the host pool had no room for: a bigger pool keeps the exported ones
+        const size_t kept = (size_t)h_slots * pool_stride * 4;
+        late_bytes = ((size_t)pool_used - h_slots) * pool_stride * 4;
+        MappedBuf grown;
+        grown.ensure(kept + late_bytes);
+        memcpy(grown.p, H.pool.p, kept);
+        H.pool = std::move(grown);
+        CK(cudaMemcpyAsync(static_cast<uint8_t*>(H.pool.p) + kept, W.pool.as<uint8_t>() + kept, late_bytes, cudaMemcpyDeviceToHost, c->stream));
+        c->breakdown[7] += (double)(pool_used - h_slots);
+    }
     out_pool_stride = pool_stride;
     out_trees.resize(tw);
-    uint64_t rec_off = 0;
+    // bytes the kernel wrote to host memory: every record, the ids of every row of the tree (its leaves partition them) and
+    // one normal per split that is not random ((n_recs - 1) / 2 splits), less the normals in slots the host copied itself
+    uint64_t exported = 0;
     for (uint32_t t = 0; t < tw; ++t) {
-        out_trees[t].recs = static_cast<const void*>(H.recs.as<Record>() + rec_off);
+        const Record* recs = H.recs.as<Record>() + (size_t)t * rec_cap;
+        out_trees[t].recs = static_cast<const void*>(recs);
         out_trees[t].n_recs = st[t].n_recs;
         out_trees[t].final_rows = H.final_rows.as<uint32_t>() + (size_t)t * n;
         out_trees[t].pool = H.pool.as<float>();
-        CK(cudaMemcpyAsync(H.recs.as<Record>() + rec_off, W.recs.as<Record>() + (size_t)t * rec_cap, sizeof(Record) * st[t].n_recs, cudaMemcpyDeviceToHost, c->stream));
-        rec_off += st[t].n_recs;
+        const uint64_t rows = sub.rows ? sub.off[t0 + t + 1] - sub.off[t0 + t] : n;
+        uint64_t normals = (st[t].n_recs - 1) / 2 - st[t].n_random;
+        if (late_bytes)
+            for (uint32_t i = 0; i < st[t].n_recs; ++i) normals -= recs[i].kind == REC_SPLIT && recs[i].c != NO_SLOT && recs[i].c >= h_slots;
+        exported += sizeof(Record) * (uint64_t)st[t].n_recs + 4 * rows + 4ull * pool_stride * normals;
         c->stats[0] += (double)st[t].scanned;
         c->stats[2] += (double)st[t].n_splits_tried;
         c->stats[3] += (double)st[t].n_random;
@@ -897,14 +929,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         if (sub.end_pos) sub.end_pos[t0 + t] = st[t].pos;
     }
     if (persist && P.root_fused) { c->fused_root_rows += (uint64_t)tw * n; c->fused_root_read += n; }
-    if (P.shadow_stats) {
-        unsigned long long hs[3] = {0, 0, 0};
-        CK(cudaMemcpyAsync(hs, P.shadow_stats, 24, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaStreamSynchronize(c->stream));
-        c->shadow_rows += hs[0]; c->shadow_rescored += hs[1]; c->shadow_stage2 += hs[2];
-    }
-    CK(cudaStreamSynchronize(c->stream));
-    c->d2h_bytes += (uint64_t)pool_used * pool_stride * 4 + sizeof(TreeState) * tw + sizeof(Record) * total_recs + 4ull * n * tw;
+    if (P.shadow_stats) { c->shadow_rows += hs[0]; c->shadow_rescored += hs[1]; c->shadow_stage2 += hs[2]; }
+    if (late_bytes) CK(cudaStreamSynchronize(c->stream));
+    c->d2h_bytes += sizeof(TreeState) * tw + exported + late_bytes;
     c->breakdown[3] += ms_since(t_d2h);
 }
 
@@ -934,9 +961,9 @@ void do_build_begin(arroy_ctx* c, uint32_t n_trees, const uint8_t (*seeds)[32], 
     size_t free_b = 0, total_b = 0;
     if (!same_shape) CK(cudaMemGetInfo(&free_b, &total_b));
     const uint64_t leaves_est = n / K + 1;
-    const uint64_t per_tree = n * (4 + 4 + 1 + 4) + (n / SCAN_UNIT + 1) * 4 + sizeof(Frame) * (uint64_t)MAX_DEPTH + 16ull * 8 * leaves_est +
+    const uint64_t per_tree = n * (4 + 4 + 1) + (n / SCAN_UNIT + 1) * 4 + sizeof(Frame) * (uint64_t)MAX_DEPTH + 16ull * 8 * leaves_est +
                               4ull * (c->ld + NORMAL_HDR) * 4 * leaves_est + 4096;
-    uint64_t reusable = c->wave.perm0.cap + c->wave.perm1.cap + c->wave.flags.cap + c->wave.final_ids.cap + c->wave.pool.cap + c->wave.recs.cap;
+    uint64_t reusable = c->wave.perm0.cap + c->wave.perm1.cap + c->wave.flags.cap + c->wave.pool.cap + c->wave.recs.cap;
     uint64_t max_wave = same_shape ? c->wave_max : (uint64_t)((free_b + reusable) * 0.7) / std::max<uint64_t>(per_tree, 1);
     if (!same_shape) c->wave_max = max_wave;
     if (const char* e = getenv("ARROY_B200_MAX_WAVE")) max_wave = std::min<uint64_t>(max_wave, (uint64_t)atoi(e));

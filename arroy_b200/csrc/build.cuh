@@ -54,6 +54,8 @@ struct TreeState {
     uint64_t scanned;        // rows that went through side()
     uint32_t slot_end;
     uint32_t n_misspec;      // create_split calls whose speculative two_means had to be redone sequentially
+    uint32_t exported;       // records [exported, n_recs) are not yet in the host result buffers (export_records)
+    uint32_t pad;
 };
 
 // Persistent schedule (control_kernel<.., CS = 0>): one launch per wave holds one control CTA per tree and worker CTAs on
@@ -114,6 +116,12 @@ struct BuildParams {
     int32_t root_fused;
     uint32_t* root_ready;         // number of trees whose root normal is published
     uint32_t* root_ticket;        // next unclaimed chunk of the fused pass
+    // the host result buffers (mapped pinned memory, at their device addresses): each control CTA copies its tree's records
+    // there as they close, with the ids of their leaves and the normals of their splits (export_records)
+    Record* h_recs;               // n_trees x rec_cap
+    uint32_t* h_rows;             // n_trees x n: each tree's ids in final order (a leaf's ids where its record points)
+    float* h_pool;                // pool slots [0, h_pool_slots) at their device index; the host copies the ones above
+    uint32_t h_pool_slots;
 };
 
 __device__ __forceinline__ double split_imbalance_dev(uint32_t l, uint32_t r) {  // src/writer.rs:1348-1353
@@ -813,6 +821,48 @@ __device__ __forceinline__ bool pwait(const BuildParams& P, PSlot& sl, uint32_t 
     }
 }
 
+// ---- result export ----------------------------------------------------------------------------------------------------------
+// count words from src to dst, where both sit at the same offset modulo 16 bytes: the aligned interior in 16-byte stores, so
+// that writes to host memory cross PCIe as whole lines. Reads bypass L1: a wide partition's ids were written by other CTAs.
+__device__ __forceinline__ void export_words(const uint32_t* src, uint32_t* dst, uint32_t count, uint32_t rank, uint32_t nthr) {
+    const uint32_t head = min(count, (uint32_t)((16u - ((uintptr_t)src & 15u)) & 15u) / 4u);
+    const uint32_t body = (count - head) / 4u, tail = head + 4u * body;
+    for (uint32_t j = rank; j < head; j += nthr) dst[j] = __ldcg(src + j);
+    const uint4* s4 = reinterpret_cast<const uint4*>(src + head);
+    uint4* d4 = reinterpret_cast<uint4*>(dst + head);
+    for (uint32_t j = rank; j < body; j += nthr) d4[j] = __ldcg(s4 + j);
+    for (uint32_t j = tail + rank; j < count; j += nthr) dst[j] = __ldcg(src + j);
+}
+
+// Copy records [lo, hi) of tree t to the host result buffers, with the ids of their leaves and the normals of their splits.
+// Threads rank = 0 .. nthr - 1 of the CTA take part, without a barrier. Both are final once the record is written: a leaf's
+// ids never move again (later partitions write other ranges of the tree's id buffers), and a split's normal is the accepted
+// one (its slot is never handed out again). Slots at or above h_pool_slots are left to the host.
+__device__ __forceinline__ void export_records(const BuildParams& P, uint32_t t, uint32_t lo, uint32_t hi, uint32_t rank, uint32_t nthr) {
+    const Record* recs = P.recs + (size_t)t * P.rec_cap;
+    Record* h_recs = P.h_recs + (size_t)t * P.rec_cap;
+    for (uint32_t i = lo; i < hi; ++i) {
+        const uint4 raw = __ldcg(reinterpret_cast<const uint4*>(recs + i));
+        if (rank == i % nthr) *reinterpret_cast<uint4*>(h_recs + i) = raw;
+        if (raw.x == REC_DESC) {
+            const size_t off = (size_t)t * P.n + raw.y;
+            export_words(P.perm[raw.w & 1u] + off, P.h_rows + off, raw.z, rank, nthr);
+        } else if (raw.w != NO_SLOT && raw.w < P.h_pool_slots) {
+            const size_t off = (size_t)raw.w * P.pool_stride;
+            export_words(reinterpret_cast<const uint32_t*>(P.pool + off), reinterpret_cast<uint32_t*>(P.h_pool + off), P.pool_stride, rank, nthr);
+        }
+    }
+}
+// The persistent kernel calls it out of line: inlined at its three call sites, it moves ptxas' spills of the control code.
+__device__ __noinline__ void export_records_outlined(const BuildParams& P, uint32_t t, uint32_t lo, uint32_t hi, uint32_t rank, uint32_t nthr) {
+    export_records(P, t, lo, hi, rank, nthr);
+}
+template <int CS>
+__device__ __forceinline__ void export_pending(const BuildParams& P, uint32_t t, uint32_t lo, uint32_t hi, uint32_t rank, uint32_t nthr) {
+    if constexpr (CS == 0) export_records_outlined(P, t, lo, hi, rank, nthr);
+    else export_records(P, t, lo, hi, rank, nthr);
+}
+
 // ---- fused root scan -------------------------------------------------------------------------------------------------------
 // The root of every tree is the whole index, so the first side() scan of each of the wave's T trees reads all n rows: T passes
 // over the item matrix (at 50 trees, one eleventh of all the bytes a C2 build reads). Here the workers wait until the T root
@@ -1354,8 +1404,9 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
                     ppublish(P.slots[t], job, s_pseq, groups, chunk);
                     s_wait_ok = pwait(P, P.slots[t], s_pseq, groups) ? 1 : 0;
                     }
-                }
+                } else if (tid >= 32) export_pending<CS>(P, t, S.exported, S.n_recs, tid - 32, CTRL_THREADS - 32);   // while thread 0 waits
                 __syncthreads();
+                if (tid == 0) S.exported = S.n_recs;
                 if (!s_wait_ok) break;
                 total_left = cta_exclusive_scan(unit_left, units, sm_tmp);
                 __syncthreads();
@@ -1410,7 +1461,9 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
             __syncthreads();
             const uint32_t units = (f.len + PART_UNIT - 1) / PART_UNIT;
             if (tid == 0) { s_pseq += 1; const uint32_t groups = (units + 3u) / 4u; ppublish(P.slots[t], job, s_pseq, groups, 4u); s_wait_ok = pwait(P, P.slots[t], s_pseq, groups) ? 1 : 0; }
+            else if (tid >= 32) export_pending<CS>(P, t, S.exported, S.n_recs, tid - 32, CTRL_THREADS - 32);
             __syncthreads();
+            if (tid == 0) S.exported = S.n_recs;
             if (!s_wait_ok) break;
             if (tid == 0) { FR(S.sp).stage = 1; S.phase = PH_AWAIT_PART; }
             total_left = 0;
@@ -1429,21 +1482,11 @@ __global__ void __launch_bounds__(CTRL_THREADS, (CS == 0 ? 2 : 1)) control_kerne
     __syncthreads();
     if (CS > 1) cooperative_groups::this_cluster().sync();   // releases the helpers (job.pad == 0)
     for (int i = tid; i <= S.sp && i < SMF; i += blockDim.x) gframes[i] = sm_frames[i];
-    if (tid == 0) { S.pos = s_rng.pos; P.st[t] = S; }
-}
-
-// Merge the two ping-pong id buffers into `final_ids` following each leaf's parity.
-__global__ void finalize_kernel(BuildParams P, uint32_t* __restrict__ final_ids) {
-    const uint32_t t = blockIdx.y;
-    const TreeState& S = P.st[t];
-    const Record* recs = P.recs + (size_t)t * P.rec_cap;
-    for (uint32_t r = blockIdx.x; r < S.n_recs; r += gridDim.x) {
-        const Record rc = recs[r];
-        if (rc.kind != REC_DESC) continue;
-        const uint32_t* src = P.perm[rc.c & 1] + (size_t)t * P.n + rc.a;
-        uint32_t* dst = final_ids + (size_t)t * P.n + rc.a;
-        for (uint32_t i = threadIdx.x; i < rc.b; i += blockDim.x) dst[i] = src[i];
-    }
+    // what closed since the last export leaves before the launch does (persistent schedule: once, when the tree is done; the
+    // others: after every attempt, the cursor lives in TreeState)
+    export_pending<CS>(P, t, S.exported, S.n_recs, tid, CTRL_THREADS);
+    __syncthreads();
+    if (tid == 0) { S.exported = S.n_recs; S.pos = s_rng.pos; P.st[t] = S; }
 }
 
 __global__ void init_trees_kernel(BuildParams P, const uint32_t* __restrict__ keys /* n_trees x 8 */, const uint64_t* __restrict__ start_pos /* words already consumed, or NULL */) {
@@ -1451,7 +1494,7 @@ __global__ void init_trees_kernel(BuildParams P, const uint32_t* __restrict__ ke
     if (threadIdx.x == 0) {
         TreeState s;
         for (int i = 0; i < 8; ++i) s.key[i] = keys[t * 8 + i];
-        s.pos = start_pos ? start_pos[t] : 0; s.phase = PH_START; s.sp = -1; s.attempts_left = 0; s.cur_slot = NO_SLOT; s.n_recs = 0;
+        s.pos = start_pos ? start_pos[t] : 0; s.phase = PH_START; s.sp = -1; s.attempts_left = 0; s.cur_slot = NO_SLOT; s.n_recs = 0; s.exported = 0; s.pad = 0;
         s.n_splits_tried = 0; s.n_random = 0; s.n_misspec = 0; s.scanned = 0; s.slot_next = 0; s.slot_end = 0;
         P.st[t] = s;
         P.jobs[t].kind = JOB_NONE;

@@ -398,16 +398,19 @@ uint64_t arroy_b200_arena_stats(arroy_b200_arena* arena, uint64_t* out_total_byt
 int32_t arroy_b200_arena_get(arroy_b200_arena* arena, uint32_t node_id, const uint8_t** out_bytes, uint64_t* out_len);
 
 /* Host-side wall-clock breakdown of the last build (ms): [0] buffer setup + tree init,
- * [1] CUDA graph capture + instantiate, [2] device step loop, [3] finalize + device->host copies,
+ * [1] CUDA graph capture + instantiate, [2] device step loop, [3] read-back after the kernels (tree states, pool fill,
+ * pre-filter counters; the results themselves reach host memory while the wave builds),
  * [4] NodeCodec encoding + sink calls, [5] graph launches (count), [6] the schedules the build's
  * waves ran, one bit each, OR-ed over the waves: 1 persistent (one cooperative launch per wave),
  * 2 lockstep, 4 async CUDA graph with one control CTA per tree, 8 / 16 async with a thread-block
  * cluster of 8 / 16 control CTAs per tree, 32 two_means workspace in global memory (rows wider
- * than 3648 floats), 64 speculative two_means; [7] reserved. */
+ * than 3648 floats), 64 speculative two_means; [7] normal pool slots copied after the kernels because
+ * the host pool had no room for them (count; ARROY_B200_EXPORT_SLOTS). */
 int32_t arroy_b200_build_breakdown(arroy_ctx* ctx, double out[8]);
 
 /* Counters since arroy_b200_create: out[0] = kernel launches issued by this library,
- * out[1] = bytes copied host->device, out[2] = bytes copied device->host, out[3] = (query batches re-ranked by
+ * out[1] = bytes copied host->device, out[2] = bytes copied device->host (builds: including what the kernels write to
+ * host memory), out[3] = (query batches re-ranked by
  * the fused bf16-pre-filter kernel << 32) | batches that fell back to the plain distance + top-k kernels. */
 int32_t arroy_b200_counters(arroy_ctx* ctx, uint64_t out[4]);
 
