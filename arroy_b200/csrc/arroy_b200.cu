@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <stdexcept>
@@ -245,6 +246,7 @@ struct arroy_ctx {
     DevBuf x_gather, x_cnorm, x_ca, x_cb, x_gmax, x_qa, x_qb, x_twoe, x_qnorm, x_S, x_sel, x_beg, x_end, x_flag;
     DevBuf x_gh0, x_iota;   // host placement: the gathered candidates' headers and their positions for the exact dense path
     uint64_t xf_calls = 0, xf_fallbacks = 0, xf_selected = 0, xf_queries = 0;
+    int tg_clusters = 0;   // tcgemm_tf32's resident clusters on this device, once measured
     Event xev[8];
     double xbreak[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     double sbreak[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -299,20 +301,42 @@ uint32_t placement_plan(int32_t metric, uint32_t dim, uint64_t n, uint64_t free_
 
 bool host_items_forced() { const char* e = getenv("ARROY_B200_HOST_ITEMS"); return e != nullptr && atoi(e) == 1; }
 
-size_t work_smem(uint32_t ld, int njobs) { return (size_t)ld * 4 + (size_t)(njobs + 1) * 4 + 16; }
+// Lets kernel `fn` take `bytes` of dynamic shared memory on `device` (the current device) where that is above the 48 KB any kernel
+// may take. The limit belongs to the kernel on one device, whichever context set it, so it is only ever raised: a launch that asks
+// for less must not take away what another launch still needs. One table for the process, read and set under one lock.
+void raise_smem_limit(int device, const void* fn, size_t bytes) {
+    if (bytes <= 48 * 1024) return;
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> limits;
+    std::lock_guard<std::mutex> lk(mu);
+    size_t& limit = limits[{device, fn}];
+    if (bytes <= limit) return;
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    limit = bytes;
+}
 
-// the scan kernel of the staged items: f32 rows, or bit-string rows for the binary-quantized metrics
-auto work_fn(int metric) { return is_bq(metric) ? &work_kernel<true> : &work_kernel<false>; }
+PlaneRows plane_rows(arroy_ctx* c) { return PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}; }
 
-void launch_work(arroy_ctx* c, const Job* jobs, int njobs, int grid) {
-    size_t smem = work_smem(c->ld, njobs);
-    const auto work = work_fn(c->metric);
-    // set on every launch: build_wave sets the same attribute to its own (possibly smaller) request, so a value remembered
-    // here could be stale
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    work<<<grid, WORK_THREADS, smem, c->stream>>>(jobs, njobs, items_f32(c), c->h0.as<float>(), c->dim, c->ld, c->metric);
-    CK(cudaGetLastError());
-    c->n_launches += 1;
+// A side() scan through the 8-bit planes: jobs of more than min_units units go through them, their stage counts to stats (or null).
+struct ScanPlanes { uint32_t min_units; unsigned long long* stats; };
+
+// The dynamic shared memory of a side() scan over njobs jobs, its kernel's limit raised to it: the normal, the jobs' unit-prefix
+// table and, through the planes, the normal's limbs.
+size_t scan_smem(arroy_ctx* c, int njobs, bool planes) {
+    const size_t smem = (size_t)c->ld * 4 + (size_t)(njobs + 1) * 4 + 16 + (planes ? (size_t)PLANES_LIMBS * c->ld : 0);
+    raise_smem_limit(c->device, planes ? (const void*)work_kernel_planes : is_bq(c->metric) ? (const void*)work_kernel<true> : (const void*)work_kernel<false>, smem);
+    return smem;
+}
+
+// A side() scan of the staged items over njobs jobs on `grid` CTAs: work_kernel (binary-quantized metrics: on the bit strings), or
+// with `pl` work_kernel_planes. Once the limit is raised, the launch is its only CUDA call (build_wave captures it in a graph);
+// the caller checks and counts it.
+void launch_scan(arroy_ctx* c, cudaStream_t s, const Job* jobs, int njobs, unsigned grid, const ScanPlanes* pl) {
+    const size_t smem = scan_smem(c, njobs, pl != nullptr);
+    const float *items = items_f32(c), *ih0 = c->h0.as<float>();
+    if (pl) work_kernel_planes<<<grid, WORK_THREADS, smem, s>>>(jobs, njobs, items, plane_rows(c), ih0, c->dim, c->ld, c->metric, pl->min_units, pl->stats);
+    else if (is_bq(c->metric)) work_kernel<true><<<grid, WORK_THREADS, smem, s>>>(jobs, njobs, items, ih0, c->dim, c->ld, c->metric);
+    else work_kernel<false><<<grid, WORK_THREADS, smem, s>>>(jobs, njobs, items, ih0, c->dim, c->ld, c->metric);
 }
 
 // norms_kernel over n rows of d = c->dim in a matrix of pitch c->ld (one 8-lane group per row); max_bits: their atomic max, or null
@@ -531,31 +555,41 @@ struct Subsets {   // host arrays, indexed by global tree
     uint64_t* end_pos = nullptr;           // optional: ... and has consumed when its tree is finished
 };
 
+// f(std::integral_constant<int, METRIC>{}) for the metric: kernels are instantiated per metric, and this is their one dispatch
+template <class F>
+decltype(auto) with_metric(int metric, F&& f) {
+    switch (metric) {
+        case EUCLIDEAN: return f(std::integral_constant<int, EUCLIDEAN>{});
+        case COSINE: return f(std::integral_constant<int, COSINE>{});
+        case DOT_PRODUCT: return f(std::integral_constant<int, DOT_PRODUCT>{});
+        case MANHATTAN: return f(std::integral_constant<int, MANHATTAN>{});
+        case BQ_EUCLIDEAN: return f(std::integral_constant<int, BQ_EUCLIDEAN>{});
+        case BQ_COSINE: return f(std::integral_constant<int, BQ_COSINE>{});
+        default: return f(std::integral_constant<int, BQ_MANHATTAN>{});
+    }
+}
+
 // The control kernel is compiled once per metric (and per cluster size): it is bound by instruction fetch, so every
-// instantiation only carries its own metric's code.
+// instantiation only carries its own metric's code. The binary-quantized metrics have no cluster variants (null).
 template <bool SMEM_WS, int CS>
 const void* control_fn(int metric) {
-    switch (metric) {
-        case EUCLIDEAN: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, EUCLIDEAN>);
-        case COSINE: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, COSINE>);
-        case DOT_PRODUCT: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, DOT_PRODUCT>);
-        case MANHATTAN: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, MANHATTAN>);
-        default: break;
-    }
-    // binary-quantized metrics: persistent, single-CTA and global-workspace variants only (no cluster variants)
-    if constexpr (CS <= 1) {
-        switch (metric) {
-            case BQ_EUCLIDEAN: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, BQ_EUCLIDEAN>);
-            case BQ_COSINE: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, BQ_COSINE>);
-            default: return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, BQ_MANHATTAN>);
-        }
-    }
-    return nullptr;
+    return with_metric(metric, [](auto m) -> const void* {
+        if constexpr (CS > 1 && is_bq(decltype(m)::value)) return nullptr;
+        else return reinterpret_cast<const void*>(&control_kernel<SMEM_WS, CS, decltype(m)::value>);
+    });
 }
 inline const void* control_fn(bool smem_ws, int cs, int metric) {
     if (!smem_ws) return control_fn<false, 1>(metric);
     if (cs == 0) return control_fn<true, 0>(metric);   // persistent schedule
     return cs == 16 ? control_fn<true, 16>(metric) : (cs == 8 ? control_fn<true, 8>(metric) : control_fn<true, 1>(metric));
+}
+// The two_means workspace of a control CTA at row pitch ld (build.cuh): WS_VECS vectors, in shared memory when they fit in
+// 200 KB, and WS_VECS_SPEC vectors for the speculative two_means when those fit as well.
+struct TwoMeansWs { size_t bytes; bool smem, spec; };   // bytes per CTA
+TwoMeansWs two_means_ws(uint32_t ld) {
+    const size_t plain = (size_t)WS_VECS * ld * 4, spec = (size_t)WS_VECS_SPEC * ld * 4;
+    if (spec <= 200 * 1024) return {spec, true, true};
+    return {plain, plain <= 200 * 1024, false};
 }
 // launch (cluster dimension cs > 1: thread-block cluster of cs CTAs per tree)
 inline void launch_control(const void* fn, unsigned n_trees, int cs, size_t smem, cudaStream_t s, BuildParams& P, uint32_t tree_base) {
@@ -599,12 +633,8 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     W.active.ensure(4);
     W.error.ensure(4);
     W.keys.ensure(32ull * tw);
-    size_t ws_bytes = (size_t)WS_VECS * ld * 4;
-    int use_smem = ws_bytes <= 200 * 1024 ? 1 : 0;
-    if (!use_smem) W.scratch.ensure(ws_bytes * tw);
-    // speculative two_means (build.cuh): needs the 24-vector workspace in shared memory
-    const int spec = (use_smem && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024) ? 1 : 0;
-    if (spec) ws_bytes = (size_t)WS_VECS_SPEC * ld * 4;
+    const TwoMeansWs ws = two_means_ws(ld);
+    if (!ws.smem) W.scratch.ensure(ws.bytes * tw);
 
     BuildParams P{};
     P.items = items_f32(c); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
@@ -613,7 +643,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     P.perm[0] = W.perm0.as<uint32_t>(); P.perm[1] = W.perm1.as<uint32_t>();
     P.flags = W.flags.as<uint8_t>(); P.unit_left = W.unit_left.as<uint32_t>(); P.units_per_tree = units;
     P.pool = W.pool.as<float>(); P.pool_stride = pool_stride; P.pool_cap = pool_cap; P.pool_counter = W.pool_counter.as<uint32_t>();
-    P.jobs = W.jobs.as<Job>(); P.scratch = W.scratch.as<float>(); P.use_smem_ws = use_smem; P.spec = spec;
+    P.jobs = W.jobs.as<Job>(); P.scratch = W.scratch.as<float>(); P.use_smem_ws = ws.smem; P.spec = ws.spec;
     P.active = W.active.as<uint32_t>(); P.error = W.error.as<int32_t>();
     P.sub_rows = nullptr; P.sub_off = nullptr;
     // cluster-resident nodes: up to ~6 MB of item rows per scan (2048 rows at d = 768, every node of a 10k x 64 index)
@@ -668,14 +698,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     CK(cudaGetLastError());
     c->n_launches += 1;
 
-    const size_t ctrl_smem = use_smem ? ws_bytes : 0;
-    if (ctrl_smem > 48 * 1024) CK(cudaFuncSetAttribute(control_fn(true, 1, c->metric), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
-    const size_t wsmem = work_smem(ld, (int)tw);
-    const auto work = work_fn(c->metric);
-    if (wsmem > 48 * 1024) CK(cudaFuncSetAttribute(work, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
-    const size_t limb_smem = (size_t)PLANES_LIMBS * ld;   // work_kernel_shadow's limbs of the normal
-    if (wsmem + limb_smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(wsmem + limb_smem)));
-    const int work_grid = c->sm_count * 3;
+    const size_t ctrl_smem = ws.smem ? ws.bytes : 0;
 
     // Three schedules over the same kernels:
     //  * persistent (below): one cooperative launch for the whole wave.
@@ -689,17 +712,16 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     const bool profile = getenv("ARROY_B200_PROFILE") != nullptr && atoi(getenv("ARROY_B200_PROFILE")) != 0;
     const bool lockstep = profile || (getenv("ARROY_B200_LOCKSTEP") != nullptr && atoi(getenv("ARROY_B200_LOCKSTEP")) != 0);
     const int steps_per_batch = lockstep ? LOCKSTEP_BATCH : ASYNC_BATCH;
-    const void* ctrl1 = control_fn(use_smem != 0, 1, c->metric);
+    const void* ctrl1 = control_fn(ws.smem, 1, c->metric);
+    raise_smem_limit(c->device, ctrl1, ctrl_smem);
     // Few trees on this GPU = the chain of attempts of each tree is the critical path: the async schedule runs the control kernel
     // as a thread-block cluster that scans small nodes itself (build.cuh control_kernel<.., CS = 8 | 16>).
     // measured: d = 64, 1-10 trees: 24 -> 20 us per attempt; d = 768: 38 -> 37 us for one tree but slower from ~6 trees on
     // (not for host-placed items: the cluster kernels scan their small nodes from the f32 rows)
-    const int cluster = (!lockstep && use_smem && c->dim <= 256 && !is_bq(c->metric) && !c->host_items) ? (tw <= 8 ? 16 : (tw <= 16 ? 8 : 1)) : 1;
-    const void* ctrlc = control_fn(use_smem != 0, cluster, c->metric);
-    if (cluster > 1) {
-        CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctrl_smem));
-        if (cluster == 16) CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    }
+    const int cluster = (!lockstep && ws.smem && c->dim <= 256 && !is_bq(c->metric) && !c->host_items) ? (tw <= 8 ? 16 : (tw <= 16 ? 8 : 1)) : 1;
+    const void* ctrlc = control_fn(ws.smem, cluster, c->metric);
+    raise_smem_limit(c->device, ctrlc, ctrl_smem);
+    if (cluster == 16) CK(cudaFuncSetAttribute(ctrlc, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
 
     // Persistent schedule (default): ONE cooperative launch per wave — a control CTA per tree plus worker CTAs on every SM
     // (build.cuh control_kernel<.., CS = 0>). Needs two CTAs per SM to have enough workers next to the control CTAs; with
@@ -710,12 +732,12 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     const void* ctrlp = nullptr;
     // It wins where the chain of attempts is the critical path (few trees per GPU, small indexes); a wave that is bandwidth-bound
     // from start to end (10M x 100 trees) runs a little faster on work_kernel's three scanning CTAs per SM.
-    if ((double)n * (double)tw <= 2.0e8 && !lockstep && use_smem && ld <= 8u * CTRL_THREADS && n < (1ull << 29)) {
+    if ((double)n * (double)tw <= 2.0e8 && !lockstep && ws.smem && ld <= 8u * CTRL_THREADS && n < (1ull << 29)) {
         ctrlp = control_fn(true, 0, c->metric);
         const size_t cand[2] = {persistent_smem(ctrl_smem, ld), persistent_smem((size_t)WS_VECS * ld * 4, ld)};
         for (int k = 0; k < 2 && !persist; ++k) {
             if (k == 1 && !P.spec) break;
-            CK(cudaFuncSetAttribute(ctrlp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cand[k]));
+            raise_smem_limit(c->device, ctrlp, cand[k]);
             int nb = 0;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ctrlp, CTRL_THREADS, cand[k]));
             const int cap = nb * c->sm_count;
@@ -726,7 +748,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     // Host-placed items: every scan, so that only the rows the planes cannot decide are read over PCIe.
     if (!is_bq(c->metric) && P.d >= 64 && P.d <= PLANES_MAX_D && (n * (uint64_t)ld >= (1ull << 22) || c->host_items)) {
         planes_prepare(c);
-        P.planes = PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()};
+        P.planes = plane_rows(c);
         W.shadow_stats.ensure(24);
         CK(cudaMemsetAsync(W.shadow_stats.p, 0, 24, c->stream));
         P.shadow_stats = W.shadow_stats.as<unsigned long long>();
@@ -734,6 +756,9 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
         // small nodes keep the one-unit claims of the exact scan (more CTAs per node)
         P.shadow_min_units = c->host_items ? 0u : (!persist || tw >= 32) ? 12u : (tw >= 12 ? 64u : 128u);
     }
+    const ScanPlanes scan_planes{P.shadow_min_units, P.shadow_stats};
+    const ScanPlanes* pl = P.planes.hi ? &scan_planes : nullptr;
+    scan_smem(c, (int)tw, pl != nullptr);   // the limit of the wave's largest scan, raised before the graph is captured
     if (persist) {
         W.slots.ensure(sizeof(PSlot) * tw);
         W.abort.ensure(4);
@@ -755,7 +780,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
     // the schedule this wave runs, OR-ed over the waves of the build (bits: arroy_b200_build_breakdown in arroy_b200.h)
     {
         const uint32_t sched = persist ? 1u : lockstep ? 2u : cluster == 16 ? 16u : cluster == 8 ? 8u : 4u;
-        c->breakdown[6] = (double)((uint32_t)c->breakdown[6] | sched | (use_smem ? 0u : 32u) | (P.spec ? 64u : 0u));
+        c->breakdown[6] = (double)((uint32_t)c->breakdown[6] | sched | (ws.smem ? 0u : 32u) | (P.spec ? 64u : 0u));
     }
 
     CK(cudaStreamSynchronize(c->stream));
@@ -774,7 +799,6 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             c->cached_graph_key.clear();
             while (c->tree_streams.size() < tw) c->tree_streams.push_back(new_stream());
             while (c->tree_events.size() < (size_t)tw + 1) c->tree_events.push_back(new_event(cudaEventDisableTiming));
-            const size_t wsmem1 = work_smem(ld, 1);
             cudaGraph_t graph = nullptr;
             CK(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
             CK(cudaEventRecord(c->tree_events[0], c->stream));
@@ -783,8 +807,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
                 CK(cudaStreamWaitEvent(st, c->tree_events[0], 0));
                 for (int i = 0; i < ASYNC_BATCH; ++i) {
                     launch_control(ctrlc, 1, cluster, ctrl_smem, st, P, t);
-                    if (P.planes.hi) work_kernel_shadow<<<c->sm_count, WORK_THREADS, wsmem1 + limb_smem, st>>>(P.jobs + t, 1, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-                    else work<<<c->sm_count, WORK_THREADS, wsmem1, st>>>(P.jobs + t, 1, P.items, P.ih0, P.d, P.ld, P.metric);
+                    launch_scan(c, st, P.jobs + t, 1, c->sm_count, pl);
                 }
                 CK(cudaEventRecord(c->tree_events[1 + t], st));
                 CK(cudaStreamWaitEvent(c->stream, c->tree_events[1 + t], 0));
@@ -855,8 +878,7 @@ void build_wave(arroy_ctx* c, size_t wave_no, uint32_t t0, uint32_t tw, const ui
             for (int i = 0; i < LOCKSTEP_BATCH; ++i) {
                 launch_control(ctrl1, tw, 1, ctrl_smem, c->stream, P, 0u);
                 if (profile) CK(cudaEventRecord(pev[2 * i], c->stream));
-                if (P.planes.hi) work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, wsmem + limb_smem, c->stream>>>(P.jobs, (int)tw, P.items, P.planes, P.ih0, P.d, P.ld, P.metric, P.shadow_min_units, P.shadow_stats);
-                else work<<<work_grid, WORK_THREADS, wsmem, c->stream>>>(P.jobs, (int)tw, P.items, P.ih0, P.d, P.ld, P.metric);
+                launch_scan(c, c->stream, P.jobs, (int)tw, c->sm_count * (pl ? 2 : 3), pl);
                 if (profile) CK(cudaEventRecord(pev[2 * i + 1], c->stream));
             }
             CK(cudaGetLastError());
@@ -1135,8 +1157,9 @@ void do_side_batch(arroy_ctx* c, const float* normal, float h0, float h1, const 
     jb.flags = c->s_flags.as<uint8_t>(); jb.margins = out_margin ? c->s_margins.as<float>() : nullptr; jb.unit_left = c->s_unit.as<uint32_t>();
     CK(cudaMemcpyAsync(c->s_job.p, &jb, sizeof(Job), cudaMemcpyHostToDevice, c->stream));
     uint64_t units = (n_rows + SCAN_UNIT - 1) / SCAN_UNIT;
-    int grid = (int)std::min<uint64_t>(units, (uint64_t)c->sm_count * 3);
-    launch_work(c, c->s_job.as<Job>(), 1, grid);
+    launch_scan(c, c->stream, c->s_job.as<Job>(), 1, (unsigned)std::min<uint64_t>(units, (uint64_t)c->sm_count * 3), nullptr);
+    CK(cudaGetLastError());
+    c->n_launches += 1;
     CK(cudaMemcpyAsync(out_side, c->s_flags.p, n_rows, cudaMemcpyDeviceToHost, c->stream));
     if (out_margin) CK(cudaMemcpyAsync(out_margin, c->s_margins.p, n_rows * 4, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
@@ -1160,7 +1183,8 @@ const float* xf_candidates(arroy_ctx* c, const uint32_t* rows, uint32_t nc) {
 // kernel of tcgemm.cuh; engine 1: cuBLAS (kept as the cross-check of the hand-written kernel)
 void xf_scores(arroy_ctx* c, const float* q, uint32_t m, const float* cand, uint32_t nc, float* S, uint32_t lds, TgEpilogue ep, int engine) {
     if (engine == 0) {
-        if (!tcgemm_tf32(q, m, cand, nc, c->ld, S, lds, ep, c->sm_count, c->stream)) throw CudaError(std::string("tcgemm_tf32 launch failed: ") + cudaGetErrorString(cudaGetLastError()));
+        raise_smem_limit(c->device, (const void*)tcgemm_tf32_kernel, TG_SMEM);
+        if (!tcgemm_tf32(q, m, cand, nc, c->ld, S, lds, ep, c->sm_count, c->tg_clusters, c->stream)) throw CudaError(std::string("tcgemm_tf32 launch failed: ") + cudaGetErrorString(cudaGetLastError()));
         c->n_launches += 1;
         return;
     }
@@ -1260,8 +1284,7 @@ void frerank_launch(arroy_ctx* c, int src, uint32_t m, const DevQueries& Q, cons
     }
     const auto kernel = src == FR_BF16 ? frerank_kernel<FR_BF16> : frerank_kernel<FR_PLANES>;
     const size_t smem = frerank_smem(c->ld);
-    static std::atomic<size_t> configured[2] = {0, 0};
-    if (smem > 48 * 1024 && smem > configured[src].load()) { CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); configured[src] = smem; }
+    raise_smem_limit(c->device, (const void*)kernel, smem);
     kernel<<<m, FR_THREADS, smem, c->stream>>>(P);
     CK(cudaGetLastError());
     c->n_launches += 1;
@@ -1830,12 +1853,12 @@ int32_t arroy_b200_side_multi(arroy_ctx* c, uint32_t n_jobs, const float* normal
         for (uint64_t i = 0; i < total; ++i) if (rows[i] >= c->n) throw ArgError("row index out of range");
         if (total == 0) return;
         const uint32_t ld = c->ld, slot = ld + NORMAL_HDR;
-        // Host-placed items: every job goes through the 8-bit planes (work_kernel_shadow, no minimum size), so that only the rows
+        // Host-placed items: every job goes through the 8-bit planes (work_kernel_planes, no minimum size), so that only the rows
         // the planes cannot decide are read over PCIe; the flags are the f32 scan's.
         const bool planes = c->host_items;
         if (planes) planes_prepare(c);
         const size_t limb_smem = planes ? (size_t)PLANES_LIMBS * ld : 0;
-        // jobs per launch bounded by the shared-memory unit-prefix table of work_kernel (and next to the limbs of work_kernel_shadow)
+        // jobs per launch bounded by the shared-memory unit-prefix table of work_kernel (and next to the limbs of work_kernel_planes)
         const uint32_t max_jobs = planes ? (uint32_t)std::min<size_t>(40000, (160 * 1024 - 4ull * ld - limb_smem) / 4 - 1) : 40000;
         c->s_rows.ensure(4ull * total);
         c->s_flags.ensure(total);
@@ -1862,15 +1885,11 @@ int32_t arroy_b200_side_multi(arroy_ctx* c, uint32_t n_jobs, const float* normal
             }
             CK(cudaMemcpyAsync(c->s_normal.p, slots.data(), slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
             CK(cudaMemcpyAsync(c->s_job.p, jobs.data(), sizeof(Job) * m, cudaMemcpyHostToDevice, c->stream));
-            int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(units, (uint64_t)c->sm_count * 3));
-            if (planes) {
-                const size_t smem = work_smem(ld, (int)m) + limb_smem;
-                if (smem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                work_kernel_shadow<<<(unsigned)std::min<int>(grid, c->sm_count * 2), WORK_THREADS, smem, c->stream>>>(c->s_job.as<Job>(), (int)m, items_f32(c),
-                    PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}, c->h0.as<float>(), c->dim, ld, c->metric, 0u, nullptr);
-                CK(cudaGetLastError());
-                c->n_launches += 1;
-            } else launch_work(c, c->s_job.as<Job>(), (int)m, grid);
+            const int grid = (int)std::max<uint64_t>(1, std::min<uint64_t>(units, (uint64_t)c->sm_count * 3));
+            const ScanPlanes all{0u, nullptr};
+            launch_scan(c, c->stream, c->s_job.as<Job>(), (int)m, (unsigned)(planes ? std::min<int>(grid, c->sm_count * 2) : grid), planes ? &all : nullptr);
+            CK(cudaGetLastError());
+            c->n_launches += 1;
             CK(cudaStreamSynchronize(c->stream));   // slots / jobs host vectors are reused by the next chunk
         }
         CK(cudaMemcpyAsync(out_side, c->s_flags.p, total, cudaMemcpyDeviceToHost, c->stream));
@@ -1895,23 +1914,14 @@ int32_t arroy_b200_create_split(arroy_ctx* c, const uint32_t rng_key[8], uint64_
         BuildParams P{};
         P.items = items_f32(c); P.ih0 = c->h0.as<float>(); P.ih1 = c->h1.as<float>();
         P.n = (uint32_t)c->n; P.d = c->dim; P.ld = ld; P.metric = c->metric;
-        size_t ws_bytes = (size_t)WS_VECS * ld * 4;
-        P.use_smem_ws = ws_bytes <= 200 * 1024;
-        P.spec = (P.use_smem_ws && (size_t)WS_VECS_SPEC * ld * 4 <= 200 * 1024) ? 1 : 0;
-        if (P.spec) ws_bytes = (size_t)WS_VECS_SPEC * ld * 4;
+        const TwoMeansWs ws = two_means_ws(ld);
+        P.use_smem_ws = ws.smem; P.spec = ws.spec;
         P.scratch = reinterpret_cast<float*>(c->s_misc.as<uint8_t>() + 64);
-        size_t smem = P.use_smem_ws ? ws_bytes : 0;
-        const void* fn = nullptr;
-        switch (c->metric) {
-            case EUCLIDEAN: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, EUCLIDEAN> : (const void*)&create_split_kernel<false, EUCLIDEAN>; break;
-            case COSINE: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, COSINE> : (const void*)&create_split_kernel<false, COSINE>; break;
-            case DOT_PRODUCT: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, DOT_PRODUCT> : (const void*)&create_split_kernel<false, DOT_PRODUCT>; break;
-            case MANHATTAN: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, MANHATTAN> : (const void*)&create_split_kernel<false, MANHATTAN>; break;
-            case BQ_EUCLIDEAN: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, BQ_EUCLIDEAN> : (const void*)&create_split_kernel<false, BQ_EUCLIDEAN>; break;
-            case BQ_COSINE: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, BQ_COSINE> : (const void*)&create_split_kernel<false, BQ_COSINE>; break;
-            default: fn = P.use_smem_ws ? (const void*)&create_split_kernel<true, BQ_MANHATTAN> : (const void*)&create_split_kernel<false, BQ_MANHATTAN>; break;
-        }
-        if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const size_t smem = ws.smem ? ws.bytes : 0;
+        const void* fn = with_metric(c->metric, [&](auto m) {
+            return ws.smem ? (const void*)&create_split_kernel<true, decltype(m)::value> : (const void*)&create_split_kernel<false, decltype(m)::value>;
+        });
+        raise_smem_limit(c->device, fn, smem);
         {
             const uint32_t* d_rows = c->s_rows.as<uint32_t>(); uint32_t len32 = (uint32_t)n_rows; const uint32_t* d_key = c->s_misc.as<uint32_t>(); uint64_t pos0 = *rng_word_pos;
             float* d_slot = c->s_normal.as<float>(); uint64_t* d_pos = reinterpret_cast<uint64_t*>(c->s_misc.as<uint8_t>() + 32);
@@ -2209,14 +2219,6 @@ int32_t arroy_b200_load_forest(arroy_ctx* c, uint32_t n_nodes, const uint8_t* ki
 extern "C++" {
 namespace {
 
-template <bool FILTER, bool MULTI = false> void configure_walk_kernels() {
-    static bool configured = false;
-    if (configured) return;
-    CK(cudaFuncSetAttribute(walk_kernel<FILTER, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)WALK_WARPS * WALK_SHEAP * 8)));
-    CK(cudaFuncSetAttribute(walk1_kernel<FILTER, MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk1_smem<FILTER>(W1_MAX_LD)));
-    configured = true;
-}
-
 // The checks every batched search starts with. false: nothing to search (nq == 0, or count == 0 and the results are empty).
 bool batch_begin(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const float* queries, uint64_t count, uint32_t* out_rows, float* out_dist,
                  uint32_t* out_len, int32_t* out_status) {
@@ -2338,6 +2340,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 }
                 const auto walk1 = multi ? &walk1_kernel<true, true> : filtered ? &walk1_kernel<true> : &walk1_kernel<false>;
                 const size_t w1smem = filtered ? walk1_smem<true>(ld) : walk1_smem<false>(ld);
+                raise_smem_limit(c->device, (const void*)walk1, w1smem);
                 walk1<<<m_walk, W1_THREADS, w1smem, c->stream>>>(F, items_f32(c), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0, d_pre, c->f_n_normals, w1debug,
                                                                  search_k, c->w_cand2.as<uint32_t>(), cand_cap, c->w_count.as<uint32_t>(), c->w_status.as<int32_t>(), Fl);
                 CK(cudaGetLastError());
@@ -2387,6 +2390,7 @@ void run_batch(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, const floa
                 WalkFilter Fl = Fl0;
                 if (multi) Fl.qfilter += q0;
                 const auto walk = multi ? &walk_kernel<true, true> : filtered ? &walk_kernel<true> : &walk_kernel<false>;
+                raise_smem_limit(c->device, (const void*)walk, walk_smem);
                 walk<<<(m_walk + WALK_WARPS - 1) / WALK_WARPS, WALK_WARPS * 32, walk_smem, c->stream>>>(F, items_f32(c), c->dim, ld, c->metric, m_walk, Q.rows, Q.vecs, Q.h0,
                                                                                                         search_k, c->w_heaps.as<unsigned long long>(), heap_cap, c->w_cand.as<uint32_t>(), cand_cap,
                                                                                                         c->w_count.as<uint32_t>(), c->w_bitmap.as<uint32_t>(), bm_words, c->w_status.as<int32_t>(), Fl);
@@ -2424,7 +2428,6 @@ void search_batch_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
         const bool filtered = filter_bits != nullptr;
         const BatchShape S = batch_shape(c, count, search_k, filtered);
         const uint32_t bm_words = S.bm_words;
-        if (filtered) configure_walk_kernels<true>(); else configure_walk_kernels<false>();
         for (double& x : c->sbreak) x = 0;
         // ---- the filter's summary: fcount / live per node and ftotal (search.cuh filter_count_kernel). When ftotal <= search_k
         //      the reference's walk only ends with an empty queue, so its candidates are every filtered row of a reachable leaf:
@@ -2494,7 +2497,6 @@ void multi_filter_body(arroy_ctx* c, uint32_t nq, const uint32_t* query_rows, co
         const DevForest& F = c->forest;
         const BatchShape S = batch_shape(c, count, search_k, true);
         const uint32_t k = S.k, d = c->dim;
-        configure_walk_kernels<true, true>();
         for (double& x : c->sbreak) x = 0;
         // the used filters in order of first use: filter used[u] is bit u % 32 of group u / 32
         std::vector<uint32_t> used, slot(n_filters, UINT32_MAX);
@@ -2679,18 +2681,16 @@ int32_t arroy_b200_time_scan(arroy_ctx* c, const float* normal, float hdr0, floa
         CK(cudaMemcpyAsync(c->s_job.p, &jb, sizeof(Job), cudaMemcpyHostToDevice, c->stream));
         int grid = (int)std::min<uint64_t>(units, (uint64_t)c->sm_count * 3);
         const size_t flush_bytes = 256ull << 20;
-        // variant 1: work_kernel_shadow on the one job with every unit through the 8-bit pre-filter (scan_claim_planes), two CTAs
+        // variant 1: work_kernel_planes on the one job with every unit through the 8-bit pre-filter (scan_claim_planes), two CTAs
         // per SM as in the build; the stage counts of its last launch are what build_prefilter_stats reports afterwards
         const size_t stats_off = flush_l2 ? flush_bytes : 0;
         c->s_misc.ensure(stats_off + 32);
         unsigned long long* pstats = reinterpret_cast<unsigned long long*>(c->s_misc.as<uint8_t>() + stats_off);
-        const size_t psmem = work_smem(c->ld, 1) + (size_t)PLANES_LIMBS * c->ld;
-        if (planes && psmem > 48 * 1024) CK(cudaFuncSetAttribute(work_kernel_shadow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+        const ScanPlanes all{0u, pstats};
         auto launch = [&] {
-            if (!planes) { launch_work(c, c->s_job.as<Job>(), 1, grid); return; }
-            work_kernel_shadow<<<c->sm_count * 2, WORK_THREADS, psmem, c->stream>>>(c->s_job.as<Job>(), 1, items_f32(c),
-                PlaneRows{c->pl_hi.as<int8_t>(), c->pl_lo.as<int8_t>(), c->pl_scale.as<float>()}, c->h0.as<float>(), c->dim, c->ld, c->metric, 0u, pstats);
+            launch_scan(c, c->stream, c->s_job.as<Job>(), 1, planes ? c->sm_count * 2 : grid, planes ? &all : nullptr);
             CK(cudaGetLastError());
+            if (!planes) c->n_launches += 1;
         };
         launch();  // warm-up
         CK(cudaStreamSynchronize(c->stream));

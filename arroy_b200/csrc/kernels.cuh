@@ -735,7 +735,7 @@ work_kernel(const Job* __restrict__ jobs, int njobs, const float* __restrict__ i
 // PLANES_CHUNK units and go through scan_claim_planes; everything else is work_kernel's. Shared memory: the normal, its limbs
 // (PLANES_LIMBS * ld bytes) and the prefix table.
 __global__ void __launch_bounds__(WORK_THREADS, 2)
-work_kernel_shadow(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const PlaneRows planes, const float* __restrict__ ih0,
+work_kernel_planes(const Job* __restrict__ jobs, int njobs, const float* __restrict__ items, const PlaneRows planes, const float* __restrict__ ih0,
                    uint32_t d, uint32_t ld, int metric, uint32_t min_units, unsigned long long* stats) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sm_normal = reinterpret_cast<float*>(smem_raw);

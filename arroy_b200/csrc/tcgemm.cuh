@@ -298,16 +298,13 @@ inline bool tg_make_map(CUtensorMap* map, const float* ptr, uint64_t rows, uint3
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// S[m x nc] (pitch lds, lds % 4 == 0) = Q[m x ld] . C[nc x ld]^T; false if the tensor maps cannot be built
-inline bool tcgemm_tf32(const float* Q, uint32_t m, const float* C, uint32_t nc, uint32_t ld, float* S, uint32_t lds, TgEpilogue ep, int sm_count, cudaStream_t stream) {
+// S[m x nc] (pitch lds, lds % 4 == 0) = Q[m x ld] . C[nc x ld]^T; false if the tensor maps cannot be built. The caller raises the
+// kernel's shared-memory limit to TG_SMEM. max_clusters: the clusters that can be resident at once on this device (GPCs need not
+// hold an even SM count), 0 until measured here.
+inline bool tcgemm_tf32(const float* Q, uint32_t m, const float* C, uint32_t nc, uint32_t ld, float* S, uint32_t lds, TgEpilogue ep, int sm_count,
+                        int& max_clusters, cudaStream_t stream) {
     CUtensorMap mq, mcand;
     if (!tg_make_map(&mq, Q, m, ld, TG_BM) || !tg_make_map(&mcand, C, nc, ld, TG_BN / TG_MC)) return false;
-    static bool configured = false;
-    static int max_clusters = 0;   // clusters that can be resident at once (GPCs need not hold an even SM count)
-    if (!configured) {
-        if (cudaFuncSetAttribute(tcgemm_tf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TG_SMEM) != cudaSuccess) return false;
-        configured = true;
-    }
     cudaLaunchConfig_t cfg{};
     cfg.blockDim = dim3(TG_THREADS); cfg.dynamicSmemBytes = TG_SMEM; cfg.stream = stream;
     cudaLaunchAttribute at[1];

@@ -378,7 +378,7 @@ int32_t arroy_b200_synth_device(arroy_ctx* ctx, const uint8_t seed[32], uint32_t
  * (rows == NULL: rows 0..n_rows-1) with CUDA events on the library's stream; optional
  * L2 flush between launches. Returns the average milliseconds per launch. Results stay on
  * the device (this measures the kernel, not the boundary). variant 0: the f32 scan
- * (work_kernel); variant 1: the build's 8-bit pre-filter (work_kernel_shadow, every unit
+ * (work_kernel); variant 1: the build's 8-bit pre-filter (work_kernel_planes, every unit
  * through the planes; float metrics, 64 <= dim <= 8192), whose stage counts of the last
  * launch arroy_b200_build_prefilter_stats then reports. */
 int32_t arroy_b200_time_scan(arroy_ctx* ctx, const float* normal, float hdr0, float hdr1,

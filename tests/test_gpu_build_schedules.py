@@ -73,7 +73,7 @@ WIDE = {
     2144: ASYNC,                       # ... no longer does
     3648: ASYNC,                       # the largest 14-vector workspace in shared memory
     3680: ASYNC | GLOBAL_WS,           # workspace in global memory
-    8192: ASYNC | GLOBAL_WS,           # the widest row with the 8-bit pre-filter planes (work_kernel_shadow)
+    8192: ASYNC | GLOBAL_WS,           # the widest row with the 8-bit pre-filter planes (work_kernel_planes)
     8224: ASYNC | GLOBAL_WS,           # f32 work_kernel scans
 }
 WIDE_CASES = [(m, d) for d in WIDE for m in ("euclidean", "cosine")] + \
@@ -153,7 +153,7 @@ def test_async_graph_reuse_restage_and_cancel(ctx):
 # ---- (c) the cluster control kernels on a full index ----------------------------------------------------------------------
 def test_cluster_kernels_on_a_full_index(ctx, monkeypatch):
     # 16 trees x 12.6M rows > 2e8: the first wave runs the async graph with clusters of 8 CTAs per tree; the second wave of 4
-    # trees (50.4M) runs the persistent kernel. Nodes of more than small_max = 24576 rows are scanned by work_kernel_shadow,
+    # trees (50.4M) runs the persistent kernel. Nodes of more than small_max = 24576 rows are scanned by work_kernel_planes,
     # smaller ones inside the cluster, and every tree crosses the 1024-attempt limit of one control launch many times.
     # split_after = 1000 keeps the forest at tens of thousands of nodes per tree: at the default (64) the host-side comparison
     # of ~8M nodes takes minutes, while the nodes of 1000 ... 24576 rows still go through the cluster scans.

@@ -46,7 +46,7 @@ def test_claims_over_an_id_list(metric, d, n_rows):
 
 
 # (metric, schedule, d, n, trees) -> the pre-filter counters (rows_via_prefilter, rows_stage2, rows_rescored_f32) of the build.
-# Every node above 12 scan units goes through the pre-filter: on the persistent kernel's workers (32 trees), on work_kernel_shadow
+# Every node above 12 scan units goes through the pre-filter: on the persistent kernel's workers (32 trees), on work_kernel_planes
 # in the lockstep schedule, and in the async graph (rows wider than 2048 floats). Node sizes are arbitrary, so most claims end
 # inside a 128-row block. The counters are those the builds gave before claims kept their ids and scales in shared memory.
 FOREST_CASES = {
